@@ -1,8 +1,8 @@
-"""B200-native AudioLM hot path (SoundStream codec convs + RVQ, Semantic/Coarse/Fine transformers).
+"""CUDA-native AudioLM hot path for the H100 (SoundStream codec convs + RVQ, Semantic/Coarse/Fine transformers).
 
 Same class names, constructor kwargs, forward()/generate()/tokenize() signatures and state_dict keys
 as lucidrains/audiolm-pytorch (audiolm_pytorch/__init__.py exports the same public names); the arithmetic
-underneath is hand-written sm_100a CUDA reached through the C ABI in include/alm_b200.h (libalm_b200.so).
+underneath is hand-written sm_90a CUDA reached through the C ABI in include/alm_b200.h (libalm_b200.so).
 """
 __version__ = "0.2.0"
 

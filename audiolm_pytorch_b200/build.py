@@ -1,7 +1,7 @@
-"""Builds libalm_b200.so (hand-written sm_100a CUDA + C ABI) in-tree with nvcc.
+"""Builds libalm_b200.so (hand-written sm_90a CUDA + C ABI) in-tree with nvcc.
 
 `python -m audiolm_pytorch_b200.build` or `__graft_entry__.build()`.  nvcc cross-compiles for
-sm_100a without a GPU; the resulting .so is git-ignored but travels with the tree to the GPU box.
+sm_90a (H100) without a GPU; the resulting .so is git-ignored and must be built on every checkout.
 """
 from __future__ import annotations
 
@@ -19,12 +19,12 @@ OBJ_DIR = PKG_DIR / "_build"
 LIB_PATH = PKG_DIR / "libalm_b200.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",
-    *os.environ.get("ALM_EXTRA_NVCC_FLAGS", "").split(),  # e.g. -DALM_RU_TRACE for tools/ru_trace.py
+    *os.environ.get("ALM_EXTRA_NVCC_FLAGS", "").split(),
 ]
 
 

@@ -276,9 +276,8 @@ rvq_encode_kernel(const float* __restrict__ x, long long ldx, const float* __res
 // residual VQ, second generation: same arithmetic (dot products accumulate over d in ascending order with one fp32
 // FMA chain, so every distance - and therefore every index - is bit-identical to rvq_encode_kernel above), but
 //   * a thread owns 8 rows x 4 codes (32 accumulators): per 4 channels it issues 8 broadcast LDS.128 (rows) and
-//     4 conflict-free LDS.128 (codes) for 128 FMAs - the first version issued 4 LDS.128 per 16 FMAs and ran at 4 %
-//     of the FMA peak, stalled on shared-memory bandwidth and on synchronous codebook loads
-//     (profiles/r01_ncu_rvq_v1.csv: issue active 16 %, long_scoreboard 402k samples);
+//     4 conflict-free LDS.128 (codes) for 128 FMAs - the first version issued 4 LDS.128 per 16 FMAs and stalled on
+//     shared-memory bandwidth and on synchronous codebook loads;
 //   * the codebook streams through shared memory in [256 codes x 32 channels] chunks with cp.async double buffering.
 // CTA = 32 rows (4 row groups x 8) x 256 codes per tile (2 code groups x 32 lanes x 4), all Q stages.
 // ------------------------------------------------------------------------------------------------

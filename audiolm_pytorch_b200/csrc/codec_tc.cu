@@ -1,51 +1,33 @@
-// SoundStream encoder on the tcgen05 tensor cores (sm_100a): split-bf16 ("bf16x3") implicit-GEMM causal convs.
+// SoundStream encoder / decoder convs on the Hopper tensor cores (sm_90a wgmma): split-bf16 ("bf16x3") implicit-GEMM
+// causal convs.
 //
 // Reference arithmetic: soundstream.py:332-345 (CausalConv1d), :362-369 (ResidualUnit), :371-383 (EncoderBlock).
 //
-// Why tensor cores: the fp32 CUDA-core kernels (conv_tiled.cuh) are FMA-bound at 4 % of the HBM roofline the codec
-// is quoted against (18.4 GFLOP per 2-s clip vs 133.8 MB of algorithmic traffic).  fp32 operands are split as
+// Why tensor cores: fp32 CUDA-core conv kernels (conv_tiled.cuh) are FMA-bound.  fp32 operands are split as
 // x = x_hi + x_lo (two bf16, |x - x_hi - x_lo| <= 2^-17 |x|) and every product is evaluated as
-//   x_hi w_hi + x_lo w_hi + x_hi w_lo          (three kind::f16 MMAs, fp32 accumulation in TMEM)
+//   x_hi w_hi + x_lo w_hi + x_hi w_lo          (three bf16 wgmmas, fp32 accumulation in registers)
 // which keeps the result within ~2^-16 relative of the fp32 product (the dropped x_lo w_lo term is 2^-18).
 //
 // Activation format between the encoder's layers ("C8S", channels-8 split): bf16 [B][2C/8][P][T/P][8]
 //   chunk c < C/8 holds the hi halves of channels 8c..8c+7, chunk C/8 + c their lo halves;
 //   P = 1 normally; a layer feeding a stride-s conv writes P = s phase planes (row t -> plane t % s, row t / s) so
 //   that every tap of the strided conv reads unit-stride rows.
-// Same bytes as fp32 [B][C][T].  One time step of one chunk is 16 B = one row of an UMMA no-swizzle core matrix:
+// Same bytes as fp32 [B][C][T].  One time step of one chunk is 16 B = one row of a wgmma no-swizzle core matrix:
 // a tile [chunk][row][8] is a K-major operand whose rows are 16 B apart (SBO = 128), so the start address of the
-// A descriptor can point at ANY row.  One staged tile [128 + 6d rows] therefore serves all 7 taps of a dilated conv
+// A descriptor can point at ANY row.  One staged tile [rows + 6d] therefore serves all 7 taps of a dilated conv
 // by shifting the descriptor start by j*d rows: no im2col, no per-tap reload.
 //
 // Kernels
 //   first_conv_kernel      fp32 wave [B][T] (C_in = 1) -> C8S, CUDA cores (7 FMAs per output, HBM-bound on the write)
 //   ru_tc_kernel<C>        fused ResidualUnit: y = x + ELU(W1 ELU(W7 *_d x + b7) + b1); the k=7 result goes
-//                          TMEM -> registers (bias, ELU, split) -> back into the SAME TMEM columns as the bf16 A operand
-//                          of the 1x1 conv (tcgen05.mma with A from tensor memory): it never touches shared memory
+//                          registers -> (bias, ELU, split) -> shared memory as the bf16 A operand of the 1x1 conv
 //   conv_tc_kernel<..>     strided / plain causal conv as a pipelined implicit GEMM over (tap, k-step) units
-// Warp roles (all kernels): warp 0 = bulk-copy producer, warp 1 = MMA issuer, warp 2 = TMEM allocator,
-// warps 4-11 = epilogue (one accumulator row per thread, two warps per TMEM lane quadrant splitting the columns).
-// Activation tiles are staged with 16-B cp.async by the whole producer warp (1-D bulk copies of ~2 KB measured
-// ~8 B/clk/SM: profiles/r02_codec_layers_a.txt), weights with large bulk copies.
+// Activation tiles are staged with 16-B cp.async by whole producer warps, weights with large bulk copies.
 #include "alm_common.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace alm {
 namespace ctc {
-
-__device__ uint4 g_zero_rows[64];
-#ifdef ALM_RU_TRACE
-// wait-time accounting of the MMA issuer / one epilogue warp (cycles summed over CTAs): build with -DALM_RU_TRACE
-__device__ unsigned long long g_ru_trace[16];
-#define RU_TRACE_WAIT(slot, stmt)                                  \
-  do {                                                             \
-    const long long _t = clock64();                                \
-    stmt;                                                          \
-    if ((threadIdx.x & 31) == 0) atomicAdd(&g_ru_trace[slot], (unsigned long long)(clock64() - _t)); \
-  } while (0)
-#else
-#define RU_TRACE_WAIT(slot, stmt) stmt
-#endif  // 1 KB of zeros (static storage): source of constant-padding halo rows
 
 constexpr int TILE_M = 128;
 constexpr int MAX_HALO = 54;  // 6 * dilation 9
@@ -182,10 +164,6 @@ __global__ void __launch_bounds__(128) last_conv_kernel(const __nv_bfloat16* __r
 // ---------------------------------------------------------------------------------------------
 // shared pieces
 // ---------------------------------------------------------------------------------------------
-constexpr int NEW = 8;                       // epilogue warps (two per TMEM lane quadrant)
-constexpr int NSUB = NEW / 4;
-constexpr int CTA_THREADS = 32 * (4 + NEW);  // warp 0 producer, 1 MMA issuer, 2 TMEM allocator, 3 idle, 4.. epilogue
-
 // row `t` of a C8S tensor with P phase planes: element offset of chunk 0 (add c * chunk_stride for chunk c)
 struct RowAddr {
   size_t off;           // ((b * nch) * P + t % P) * (T / P) + t / P, in 8-element rows, times 8
@@ -199,19 +177,17 @@ __device__ __forceinline__ RowAddr c8s_row(int b, int t, int nch, int P, int T) 
   return a;
 }
 
-// 16 fp32 (+ bias, ELU) -> 8 packed hi words, 8 packed lo words
-__device__ __forceinline__ void bias_elu_split16(const uint32_t (&r)[16], const float* bias, uint32_t (&o)[16]) {
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const float v0 = elu1(__uint_as_float(r[2 * e]) + bias[2 * e]);
-    const float v1 = elu1(__uint_as_float(r[2 * e + 1]) + bias[2 * e + 1]);
-    split_bf16x2(v0, v1, o[e], o[8 + e]);
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
 // fused ResidualUnit
+//   warps 0 (and 3 when the weights are resident) : producers      warps 4-7 : one consumer warpgroup (wgmma + epilogues)
+// One tile = RU_TILE_M time steps.  D1 (the k=7 dilated conv) accumulates in registers; E1 adds b7, applies ELU and
+// writes the split bf16 activation to shared memory in the no-swizzle K-major layout, which is the A operand of the
+// 1x1 conv (D2); E2 adds b1, applies ELU, adds the skip input and stores C8S.  One warpgroup per CTA keeps the
+// register budget at 255 per thread, which the C = 256 layer (two 128-register accumulators in sequence) needs.
 // ---------------------------------------------------------------------------------------------
+constexpr int RU_TILE_M = 64;
+constexpr int RU_THREADS = 256;
+
 struct RuParams {
   const __nv_bfloat16* x;
   __nv_bfloat16* y;
@@ -220,7 +196,7 @@ struct RuParams {
   const float* b1;
   int B, T, d, pad_mode, out_phases;
   int tiles_per_clip, total_tiles;
-  int ar;      // rows of one staged chunk: 128 + 6 d
+  int ar;      // rows of one staged chunk: RU_TILE_M + 6 d
   int na, nw;  // staged activation tiles (1 or 2), weight ring stages (streamed mode)
 };
 
@@ -229,54 +205,47 @@ struct RuCfg {
   static constexpr int NCHUNK = C / 8;
   static constexpr int KSTEPS = C / 16;
   static constexpr bool RESIDENT = C <= 64;       // all weights stay in shared memory for the CTA's lifetime
-  static constexpr int NBUF = C <= 128 ? 2 : 1;   // tiles in flight in tensor memory (each: D1 | D2 = 2C columns)
   static constexpr int UNIT_BYTES = 2 * 2 * C * 16;  // hi [2 chunks][C][16 B] + lo
   static constexpr int NUNITS = 8 * KSTEPS;
   static constexpr int MAX_NW = 16;
-  // C == 128: the two tiles in flight consume every streamed weight unit TOGETHER (an M = 128 tile alone needs 42.7 B/clk
-  // of weights per SM, the whole chip's L2 throughput; paired tiles halve that).  C == 256 cannot: one tile fills TMEM.
-  static constexpr bool PAIR = C == 128;
-  static constexpr int TMEM_COLS = NBUF * 2 * C;
-  static constexpr int FIXED_BYTES = 2 * C * 4 + 512 + 128;  // biases, barriers, alignment slack
+  static constexpr int A2_BYTES = 2 * NCHUNK * RU_TILE_M * 16;  // E1 output: [hi / lo][chunk][64 rows][16 B]
+  static constexpr int FIXED_BYTES = A2_BYTES + 2 * C * 4 + 512 + 128;  // A2, biases, barriers, alignment slack
   static constexpr int MAX_SMEM = 232448;
+  // two CTAs per SM only where shared memory allows it at every dilation (resident weights, largest halo); the
+  // occupancy hint of the kernel and the grid size of launch_ru both follow from it
+  static constexpr int RESIDENT_MAX_SMEM =
+      2 * (2 * NCHUNK * (RU_TILE_M + MAX_HALO) * 16) + NUNITS * UNIT_BYTES + FIXED_BYTES;
+  static constexpr int CTAS_PER_SM = RESIDENT && RESIDENT_MAX_SMEM <= 113 * 1024 ? 2 : 1;
 };
 
 template <int C>
-__global__ void __launch_bounds__(CTA_THREADS, (C <= 32 ? 2 : 1)) ru_tc_kernel(const RuParams p) {
+__global__ void __launch_bounds__(RU_THREADS, RuCfg<C>::CTAS_PER_SM) ru_tc_kernel(const RuParams p) {
   using Cfg = RuCfg<C>;
-  constexpr int NCHUNK = Cfg::NCHUNK, KSTEPS = Cfg::KSTEPS, NBUF = Cfg::NBUF;
-  constexpr bool RESIDENT = Cfg::RESIDENT, PAIR = Cfg::PAIR;
+  constexpr int NCHUNK = Cfg::NCHUNK, KSTEPS = Cfg::KSTEPS;
+  constexpr bool RESIDENT = Cfg::RESIDENT;
   const int NA = p.na, NW = p.nw, A_ROWS = p.ar;
   const int A_BYTES = 2 * NCHUNK * A_ROWS * 16;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
-  uint8_t* sA = smem;
+  uint8_t* sA2 = smem;
+  uint8_t* sA = sA2 + Cfg::A2_BYTES;
   uint8_t* sW = sA + NA * A_BYTES;
   float* sBias = reinterpret_cast<float*>(sW + (RESIDENT ? Cfg::NUNITS : NW) * Cfg::UNIT_BYTES);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + 2 * C);
   uint64_t* a_full = bars;              // [2]
   uint64_t* a_empty = bars + 2;         // [2]
-  uint64_t* d1_full = bars + 4;         // [2]
-  uint64_t* a2_full = bars + 6;         // [2]
-  uint64_t* d2_full = bars + 8;         // [2]
-  uint64_t* d2_empty = bars + 10;       // [2]
-  uint64_t* w_full = bars + 12;         // [<= 16] (resident: [0] only)
-  uint64_t* w_empty = bars + 28;        // [<= 16]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 44);
+  uint64_t* w_full = bars + 4;          // [<= 16] (resident: [0] only)
+  uint64_t* w_empty = bars + 20;        // [<= 16]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int i = 0; i < 2; ++i) {
       mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
-      mbar_init(&d1_full[i], 1);
-      mbar_init(&a2_full[i], NEW);
-      mbar_init(&d2_full[i], 1);
-      mbar_init(&d2_empty[i], NEW);
+      mbar_init(&a_empty[i], 4);  // one arrive per consumer warp
     }
     for (int i = 0; i < Cfg::MAX_NW; ++i) {
       mbar_init(&w_full[i], 1);
-      mbar_init(&w_empty[i], 1);
+      mbar_init(&w_empty[i], 4);
     }
     fence_mbar_init();
   }
@@ -284,22 +253,18 @@ __global__ void __launch_bounds__(CTA_THREADS, (C <= 32 ? 2 : 1)) ru_tc_kernel(c
     sBias[i] = p.b7 ? p.b7[i] : 0.f;
     sBias[C + i] = p.b1 ? p.b1[i] : 0.f;
   }
-  if (warp == 2) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int halo = 6 * p.d;
   auto tile_of = [&](int i) { return (int)blockIdx.x + i * (int)gridDim.x; };
   auto has = [&](int i) { return i >= 0 && tile_of(i) < p.total_tiles; };
 
-  if (warp == 0 || (RESIDENT && warp == 3)) {
+  if (warp < 4) {
+    if (!(warp == 0 || (RESIDENT && warp == 3))) return;
     // ===================== producer(s) =====================
     // activation tiles: 16-B cp.async by all 32 lanes (the padding rule is just an address per row); weights: bulk copies.
     // Resident-weight layers (C <= 64) run TWO producer warps, warp 0 owning staging buffer 0 (even tiles) and warp 3
-    // buffer 1 (odd tiles): one warp's address arithmetic + ~90 cp.async per lane per tile left the MMA issuer waiting
-    // on a_full for 20-30 % of its time (profiles/r02_ru_trace_b.txt)
+    // buffer 1 (odd tiles).
     if (RESIDENT && warp == 0 && lane == 0) {
       mbar_arrive_expect_tx(&w_full[0], Cfg::NUNITS * Cfg::UNIT_BYTES);
       constexpr int PIECE = 16384;  // few large copies
@@ -323,8 +288,8 @@ __global__ void __launch_bounds__(CTA_THREADS, (C <= 32 ? 2 : 1)) ru_tc_kernel(c
       mbar_wait(&a_empty[ab], (((uint32_t)(i / NA)) & 1u) ^ 1u);
       const int tile = tile_of(i);
       const int b = tile / p.tiles_per_clip;
-      const int t0 = (tile - b * p.tiles_per_clip) * TILE_M;
-      const int rows = halo + min(TILE_M, p.T - t0);  // smem row r <-> time t0 - halo + r
+      const int t0 = (tile - b * p.tiles_per_clip) * RU_TILE_M;
+      const int rows = halo + min(RU_TILE_M, p.T - t0);  // smem row r <-> time t0 - halo + r
       uint8_t* dst = sA + ab * A_BYTES;
       for (int r = lane; r < rows; r += 32) {
         int tau = t0 - halo + r;
@@ -341,14 +306,14 @@ __global__ void __launch_bounds__(CTA_THREADS, (C <= 32 ? 2 : 1)) ru_tc_kernel(c
       }
       cp_async_commit();
     };
-    // HBM latency under load (3-4 us) exceeds one tile period: pull the tiles PF steps ahead into L2 so that the
-    // cp.async of the staged tile (and the epilogue's skip reads) hit L2
+    // HBM latency under load exceeds one tile period: pull the tiles PF steps ahead into L2 so that the cp.async of
+    // the staged tile (and the epilogue's skip reads) hit L2
     constexpr int PF = 3;
     auto prefetch_tile = [&](int i) {
       const int tile = tile_of(i);
       const int b = tile / p.tiles_per_clip;
-      const int t0 = (tile - b * p.tiles_per_clip) * TILE_M;
-      const int first = max(0, t0 - halo), last = min(p.T, t0 + TILE_M);
+      const int t0 = (tile - b * p.tiles_per_clip) * RU_TILE_M;
+      const int first = max(0, t0 - halo), last = min(p.T, t0 + RU_TILE_M);
       const int lpc = ((last - first) * 16 + 127) / 128 + 1;  // 128-B lines per chunk (+1: unaligned start)
       const uint8_t* base = reinterpret_cast<const uint8_t*>(p.x + ((size_t)b * 2 * NCHUNK * p.T + first) * 8);
       const size_t span = (size_t)(last - first) * 16 - 1;
@@ -362,359 +327,157 @@ __global__ void __launch_bounds__(CTA_THREADS, (C <= 32 ? 2 : 1)) ru_tc_kernel(c
       if (has(pid + 2)) prefetch_tile(pid + 2);
       for (int i = pid; has(i); i += 2) {
         if (has(i + 4)) prefetch_tile(i + 4);
-        issue_a(i);                  // waits until P1(i - 2) has released the buffer
+        issue_a(i);                  // waits until the consumer has released the buffer
         cp_async_wait<0>();
-        fence_proxy_async_smem();    // cp.async writes (generic proxy) -> UMMA operand reads (async proxy)
+        fence_proxy_async_smem();    // cp.async writes (generic proxy) -> wgmma operand reads (async proxy)
         __syncwarp();
         if (lane == 0) mbar_arrive(&a_full[i % NA]);
       }
-    } else if (PAIR) {
-      // tiles 2 ip and 2 ip + 1 are staged together (buffers 0 / 1) and share one pass over the weight units
-      if (has(0)) issue_a(0);
-      if (has(1)) issue_a(1);
-      for (int i0 = 0; has(i0); i0 += 2) {
-        if (has(i0 + 2)) prefetch_tile(i0 + 2);
-        if (has(i0 + 3)) prefetch_tile(i0 + 3);
-        cp_async_wait<0>();
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(&a_full[0]);
-          if (has(i0 + 1)) mbar_arrive(&a_full[1]);
-          stream_units(0, 7 * KSTEPS);
-        }
-        __syncwarp();
-        // next pair's activations: the buffers are released by the commit after P1 of this pair; the copies then run
-        // under E1 / P2 / E2 of this pair
-        if (has(i0 + 2)) issue_a(i0 + 2);
-        if (has(i0 + 3)) issue_a(i0 + 3);
-        if (lane == 0) stream_units(7 * KSTEPS, 8 * KSTEPS);
-        __syncwarp();
-      }
     } else {
-    if (has(0)) issue_a(0);
-    for (int k = 1; k < PF; ++k)
-      if (has(k)) prefetch_tile(k);
-    for (int i = 0;; ++i) {
-      const bool h1 = has(i), h2 = has(i - (NBUF - 1));
-      if (!h1 && !h2) break;
-      if (h1) {
+      if (has(0)) issue_a(0);
+      for (int k = 1; k < PF; ++k)
+        if (has(k)) prefetch_tile(k);
+      for (int i = 0; has(i); ++i) {
         if (has(i + PF)) prefetch_tile(i + PF);
         cp_async_wait<0>();        // tile i (issued one step ago)
-        fence_proxy_async_smem();  // cp.async writes (generic proxy) -> UMMA operand reads (async proxy)
+        fence_proxy_async_smem();  // cp.async writes (generic proxy) -> wgmma operand reads (async proxy)
         __syncwarp();
         if (lane == 0) mbar_arrive(&a_full[i % NA]);
         // publish tile i BEFORE staging tile i + 1: the staging waits for a_empty and takes ~1 k clk of issue
         if (NA == 2 && has(i + 1)) issue_a(i + 1);
-        if (!RESIDENT) {
-          if (lane == 0) stream_units(0, 7 * KSTEPS);
-          __syncwarp();
-        }
+        if (lane == 0) stream_units(0, 8 * KSTEPS);
+        __syncwarp();
         if (NA == 1 && has(i + 1)) issue_a(i + 1);
       }
-      if (!RESIDENT && h2) {
-        if (lane == 0) stream_units(7 * KSTEPS, 8 * KSTEPS);
-        __syncwarp();
-      }
     }
-    }
-  } else if (warp == 1) {
-    {
-      // ===================== MMA issuer: the whole warp runs the (uniform) control flow, one elected lane issues =======
-      constexpr uint32_t idesc = umma_idesc_bf16_f32(TILE_M, C, false, false);
-#ifdef ALM_RU_TRACE
-      const long long t_begin = clock64();
-#endif
-      if (RESIDENT) mbar_wait(&w_full[0], 0);
-      int wstage = 0;
-      uint32_t wphase = 0;
-      const uint32_t sw_addr = smem_u32(sW);
-      if constexpr (PAIR) {
-        const uint64_t b0 = umma_smem_desc_nosw(sw_addr, 128, C * 16);
-        const uint32_t kstep_units = 2 * A_ROWS;
-        for (int i0 = 0; has(i0); i0 += 2) {
-          const bool two = has(i0 + 1);
-          const uint32_t ph = ((uint32_t)(i0 / 2)) & 1u;   // buffers 0 / 1 are used once per pair
-          RU_TRACE_WAIT(0, mbar_wait(&a_full[0], ph));
-          if (two) mbar_wait(&a_full[1], ph);
-          tc_fence_after_sync();
-          uint64_t a_hi0[2], a_lo0[2];
-#pragma unroll
-          for (int t = 0; t < 2; ++t) {
-            const uint32_t a_addr = smem_u32(sA + t * A_BYTES);
-            a_hi0[t] = umma_smem_desc_nosw(a_addr, 128, A_ROWS * 16);
-            a_lo0[t] = umma_smem_desc_nosw(a_addr + NCHUNK * (A_ROWS * 16), 128, A_ROWS * 16);
-          }
-          const uint32_t d1a = tmem_base, d1b = tmem_base + 2 * C;
-#pragma unroll 1
-          for (int j = 0; j < 7; ++j) {
-            const uint32_t row_units = (uint32_t)(j * p.d);
-#pragma unroll
-            for (int kk = 0; kk < KSTEPS; ++kk) {
-              RU_TRACE_WAIT(3, mbar_wait(&w_full[wstage], wphase));
-              tc_fence_after_sync();
-              const uint64_t b_hi = b0 + (uint64_t)(wstage * (Cfg::UNIT_BYTES / 16));
-              const uint64_t b_lo = b_hi + (uint64_t)(2 * C);
-              const uint64_t off = (uint64_t)(kk * kstep_units + row_units);
-              const uint32_t acc = (j > 0 || kk > 0) ? 1u : 0u;
-              if (elect_one_sync()) {
-                umma_bf16_ss(d1a, a_hi0[0] + off, b_hi, idesc, acc);
-                umma_bf16_ss(d1a, a_lo0[0] + off, b_hi, idesc, 1u);
-                umma_bf16_ss(d1a, a_hi0[0] + off, b_lo, idesc, 1u);
-                if (two) {
-                  umma_bf16_ss(d1b, a_hi0[1] + off, b_hi, idesc, acc);
-                  umma_bf16_ss(d1b, a_lo0[1] + off, b_hi, idesc, 1u);
-                  umma_bf16_ss(d1b, a_hi0[1] + off, b_lo, idesc, 1u);
-                }
-                umma_commit(&w_empty[wstage]);
-              }
-              if (++wstage == NW) { wstage = 0; wphase ^= 1u; }
-            }
-          }
-          if (elect_one_sync()) {
-            umma_commit(&a_empty[0]);
-            umma_commit(&d1_full[0]);
-            if (two) {
-              umma_commit(&a_empty[1]);
-              umma_commit(&d1_full[1]);
-            }
-          }
-          RU_TRACE_WAIT(1, mbar_wait(&a2_full[0], ph));
-          RU_TRACE_WAIT(2, mbar_wait(&d2_empty[0], ph ^ 1u));
-          if (two) {
-            mbar_wait(&a2_full[1], ph);
-            mbar_wait(&d2_empty[1], ph ^ 1u);
-          }
-          tc_fence_after_sync();
-#pragma unroll
-          for (int kk = 0; kk < KSTEPS; ++kk) {
-            mbar_wait(&w_full[wstage], wphase);
-            tc_fence_after_sync();
-            const uint64_t b_hi = b0 + (uint64_t)(wstage * (Cfg::UNIT_BYTES / 16));
-            const uint64_t b_lo = b_hi + (uint64_t)(2 * C);
-            if (elect_one_sync()) {
-              umma_bf16_ts(d1a + C, d1a + 16 * kk, b_hi, idesc, kk > 0 ? 1u : 0u);
-              umma_bf16_ts(d1a + C, d1a + 16 * kk + 8, b_hi, idesc, 1u);
-              umma_bf16_ts(d1a + C, d1a + 16 * kk, b_lo, idesc, 1u);
-              if (two) {
-                umma_bf16_ts(d1b + C, d1b + 16 * kk, b_hi, idesc, kk > 0 ? 1u : 0u);
-                umma_bf16_ts(d1b + C, d1b + 16 * kk + 8, b_hi, idesc, 1u);
-                umma_bf16_ts(d1b + C, d1b + 16 * kk, b_lo, idesc, 1u);
-              }
-              umma_commit(&w_empty[wstage]);
-            }
-            if (++wstage == NW) { wstage = 0; wphase ^= 1u; }
-          }
-          if (elect_one_sync()) {
-            umma_commit(&d2_full[0]);
-            if (two) umma_commit(&d2_full[1]);
-          }
-        }
-      } else
-      for (int i = 0;; ++i) {
-        const int i2 = i - (NBUF - 1);
-        const bool h1 = has(i), h2 = has(i2);
-        if (!h1 && !h2) break;
-        if (h1) {
-          const int ab = i % NA, tb = i % NBUF;
-          RU_TRACE_WAIT(0, mbar_wait(&a_full[ab], ((uint32_t)(i / NA)) & 1u));
-          tc_fence_after_sync();
-          const uint32_t a_addr = smem_u32(sA + ab * A_BYTES);
-          const uint32_t d1 = tmem_base + tb * 2 * C;
-          // descriptors are built once; between MMAs only the 14-bit start-address field (>> 4) of the low word moves
-          // (tools/mma_bench.cu: with the issue path this lean an N <= 64 MMA retires every ~45 clk, N = 128 / 256 at
-          // their 64 / 128 clk floors; rebuilding descriptors per MMA costs several times that)
-          const uint64_t a_hi0 = umma_smem_desc_nosw(a_addr, 128, A_ROWS * 16);
-          const uint64_t a_lo0 = umma_smem_desc_nosw(a_addr + NCHUNK * (A_ROWS * 16), 128, A_ROWS * 16);
-          const uint64_t b0 = umma_smem_desc_nosw(sw_addr, 128, C * 16);
-          const uint32_t kstep_units = 2 * A_ROWS;       // two chunks, in 16-B units
-#pragma unroll 1
-          for (int j = 0; j < 7; ++j) {
-            const uint32_t row_units = (uint32_t)(j * p.d);
-#pragma unroll
-            for (int kk = 0; kk < KSTEPS; ++kk) {
-              const int u = j * KSTEPS + kk;
-              uint32_t w_units;  // offset of this unit's weights from sW, in 16-B units
-              if (RESIDENT) {
-                w_units = u * (Cfg::UNIT_BYTES / 16);
-              } else {
-                RU_TRACE_WAIT(3, mbar_wait(&w_full[wstage], wphase));
-                tc_fence_after_sync();
-                w_units = wstage * (Cfg::UNIT_BYTES / 16);
-              }
-              const uint64_t a_hi = a_hi0 + (uint64_t)(kk * kstep_units + row_units);
-              const uint64_t a_lo = a_lo0 + (uint64_t)(kk * kstep_units + row_units);
-              const uint64_t b_hi = b0 + (uint64_t)w_units;
-              const uint64_t b_lo = b_hi + (uint64_t)(2 * C);
-              if (elect_one_sync()) {
-                umma_bf16_ss(d1, a_hi, b_hi, idesc, (j > 0 || kk > 0) ? 1u : 0u);
-                umma_bf16_ss(d1, a_lo, b_hi, idesc, 1u);
-                umma_bf16_ss(d1, a_hi, b_lo, idesc, 1u);
-                if (!RESIDENT) umma_commit(&w_empty[wstage]);
-              }
-              if (!RESIDENT) {
-                if (++wstage == NW) { wstage = 0; wphase ^= 1u; }
-              }
-            }
-          }
-          if (elect_one_sync()) {
-            umma_commit(&a_empty[ab]);  // the staged tile may be overwritten once these MMAs have read it
-            umma_commit(&d1_full[tb]);
-          }
-        }
-        if (h2) {
-          const int tb = i2 % NBUF;
-          const uint32_t ph = ((uint32_t)(i2 / NBUF)) & 1u;
-          RU_TRACE_WAIT(1, mbar_wait(&a2_full[tb], ph));
-          RU_TRACE_WAIT(2, mbar_wait(&d2_empty[tb], ph ^ 1u));
-          tc_fence_after_sync();
-          const uint32_t d1 = tmem_base + tb * 2 * C;
-          const uint32_t d2 = d1 + C;
-          const uint64_t b0 = umma_smem_desc_nosw(sw_addr, 128, C * 16);
-#pragma unroll
-          for (int kk = 0; kk < KSTEPS; ++kk) {
-            const int u = 7 * KSTEPS + kk;
-            uint32_t w_units;
-            if (RESIDENT) {
-              w_units = u * (Cfg::UNIT_BYTES / 16);
-            } else {
-              mbar_wait(&w_full[wstage], wphase);
-              tc_fence_after_sync();
-              w_units = wstage * (Cfg::UNIT_BYTES / 16);
-            }
-            const uint64_t b_hi = b0 + (uint64_t)w_units;
-            const uint64_t b_lo = b_hi + (uint64_t)(2 * C);
-            // A operand of k-step kk sits where E1 left it: hi pairs in columns [16 kk, 16 kk + 8), lo in the next 8
-            if (elect_one_sync()) {
-              umma_bf16_ts(d2, d1 + 16 * kk, b_hi, idesc, kk > 0 ? 1u : 0u);
-              umma_bf16_ts(d2, d1 + 16 * kk + 8, b_hi, idesc, 1u);
-              umma_bf16_ts(d2, d1 + 16 * kk, b_lo, idesc, 1u);
-              if (!RESIDENT) umma_commit(&w_empty[wstage]);
-            }
-            if (!RESIDENT) {
-              if (++wstage == NW) { wstage = 0; wphase ^= 1u; }
-            }
-          }
-          if (elect_one_sync()) umma_commit(&d2_full[tb]);
-        }
-      }
-#ifdef ALM_RU_TRACE
-      if (lane == 0) {
-        atomicAdd(&g_ru_trace[8], (unsigned long long)(clock64() - t_begin));
-        atomicAdd(&g_ru_trace[9], 1ull);
-      }
-#endif
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue: one accumulator row per thread, 16-column units split over NSUB warps =====
-    const int ew = warp - 4;
-    const int q = ew & 3, sub = ew >> 2;
-    const int row = q * 32 + lane;
-    const uint32_t lane_sel = (uint32_t)(q * 32) << 16;
-    auto e1 = [&](const int i) {
-        // ---- E1: D1 -> (+b7, ELU, split) -> the same columns as the packed bf16 A operand of the 1x1 conv ----
-        const int tb = i % NBUF;
-        if (warp == 4 && lane == 0) { RU_TRACE_WAIT(4, mbar_wait(&d1_full[tb], ((uint32_t)(i / NBUF)) & 1u)); } else mbar_wait(&d1_full[tb], ((uint32_t)(i / NBUF)) & 1u);
-        tc_fence_after_sync();
-        const uint32_t d1 = tmem_base + tb * 2 * C + lane_sel;
-#pragma unroll 1
-        for (int u = sub; u < KSTEPS; u += NSUB) {
-          uint32_t r[16], o[16];
-          tmem_ld_32x32b_x16(d1 + 16 * u, r);
-          tmem_ld_wait();
-          bias_elu_split16(r, sBias + 16 * u, o);
-          tmem_st_32x32b_x16(d1 + 16 * u, o);
-        }
-        tmem_st_wait();
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&a2_full[tb]);
-    };
-    auto e2 = [&](const int i2) {
-        // ---- E2: D2 -> (+b1, ELU, + skip) -> split -> global (C8S) ----
-        const int tb = i2 % NBUF;
-        const int tile = tile_of(i2);
-        const int b = tile / p.tiles_per_clip;
-        const int t = (tile - b * p.tiles_per_clip) * TILE_M + row;
-        const bool valid = t < p.T;
-        const __nv_bfloat16* xrow = p.x + ((size_t)b * 2 * NCHUNK * p.T + (valid ? t : 0)) * 8;
-        const RowAddr ya = c8s_row(b, valid ? t : 0, 2 * NCHUNK, p.out_phases, p.T);
-        uint4 xh[2], xl[2];
-        auto load_skip = [&](int u) {
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            xh[c] = __ldg(reinterpret_cast<const uint4*>(xrow + (size_t)(2 * u + c) * p.T * 8));
-            xl[c] = __ldg(reinterpret_cast<const uint4*>(xrow + (size_t)(NCHUNK + 2 * u + c) * p.T * 8));
-          }
-        };
-        if (sub < KSTEPS) load_skip(sub);  // in flight while we wait for the accumulator
-        if (warp == 4 && lane == 0) { RU_TRACE_WAIT(5, mbar_wait(&d2_full[tb], ((uint32_t)(i2 / NBUF)) & 1u)); } else mbar_wait(&d2_full[tb], ((uint32_t)(i2 / NBUF)) & 1u);
-        tc_fence_after_sync();
-        const uint32_t d2 = tmem_base + tb * 2 * C + C + lane_sel;
-#pragma unroll 1
-        for (int u = sub; u < KSTEPS; u += NSUB) {
-          const uint4 ch[2] = {xh[0], xh[1]}, cl[2] = {xl[0], xl[1]};
-          if (u + NSUB < KSTEPS) load_skip(u + NSUB);
-          uint32_t r[16];
-          tmem_ld_32x32b_x16(d2 + 16 * u, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const uint32_t hw[4] = {ch[c].x, ch[c].y, ch[c].z, ch[c].w};
-            const uint32_t lw[4] = {cl[c].x, cl[c].y, cl[c].z, cl[c].w};
-            uint32_t oh[4], ol[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int chn = 16 * u + 8 * c + 2 * e;
-              const float x0 = bf16_lo(hw[e]) + bf16_lo(lw[e]);
-              const float x1 = bf16_hi(hw[e]) + bf16_hi(lw[e]);
-              const float v0 = x0 + elu1(__uint_as_float(r[8 * c + 2 * e]) + sBias[C + chn]);
-              const float v1 = x1 + elu1(__uint_as_float(r[8 * c + 2 * e + 1]) + sBias[C + chn + 1]);
-              split_bf16x2(v0, v1, oh[e], ol[e]);
-            }
-            if (valid) {
-              *reinterpret_cast<uint4*>(p.y + ya.off + (size_t)(2 * u + c) * ya.chunk_stride) =
-                  make_uint4(oh[0], oh[1], oh[2], oh[3]);
-              *reinterpret_cast<uint4*>(p.y + ya.off + (size_t)(NCHUNK + 2 * u + c) * ya.chunk_stride) =
-                  make_uint4(ol[0], ol[1], ol[2], ol[3]);
-            }
-          }
-        }
-        tc_fence_before_sync();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&d2_empty[tb]);
-    };
-    if constexpr (PAIR) {
-      // both tiles of a pair through E1 first (the paired 1x1-conv MMAs wait for both), then both through E2
-      for (int i0 = 0; has(i0); i0 += 2) {
-        const bool two = has(i0 + 1);
-        e1(i0);
-        if (two) e1(i0 + 1);
-        e2(i0);
-        if (two) e2(i0 + 1);
-      }
-    } else {
-      for (int i = 0;; ++i) {
-        const int i2 = i - (NBUF - 1);
-        const bool h1 = has(i), h2 = has(i2);
-        if (!h1 && !h2) break;
-        if (h1) e1(i);
-        if (h2) e2(i2);
-      }
-    }
+    return;
   }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  if (warp == 2) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+  // ===================== consumer warpgroup =====================
+  // fragment: rows rl + 8 h (h = 0, 1) of the tile, of every 8-column group j the columns 8 j + c_lane + {0, 1}
+  const int rl = (warp & 3) * 16 + (lane >> 2);
+  const int c_lane = 2 * (lane & 3);
+  if (RESIDENT) mbar_wait(&w_full[0], 0);
+  int wstage = 0;
+  uint32_t wphase = 0;
+  int prev_w = -1;
+  const uint32_t sw_addr = smem_u32(sW);
+  const uint64_t b0 = wgmma_desc_nosw(sw_addr, 128, C * 16);
+  const uint32_t a2_addr = smem_u32(sA2);
+  // weights of unit u: resident at a fixed offset, else the next slot of the ring (released one unit later, when the
+  // wgmma group that read it has retired)
+  auto unit_b = [&](int u) -> uint64_t {
+    if (RESIDENT) return b0 + (uint64_t)(u * (Cfg::UNIT_BYTES / 16));
+    mbar_wait(&w_full[wstage], wphase);
+    return b0 + (uint64_t)(wstage * (Cfg::UNIT_BYTES / 16));
+  };
+  auto unit_done = [&]() {
+    wgmma_commit();
+    if (!RESIDENT) {
+      wgmma_wait<1>();
+      if (prev_w >= 0 && lane == 0) mbar_arrive(&w_empty[prev_w]);
+      prev_w = wstage;
+      if (++wstage == NW) { wstage = 0; wphase ^= 1u; }
+    }
+  };
+  auto drain = [&]() {
+    wgmma_wait<0>();
+    if (!RESIDENT && prev_w >= 0 && lane == 0) mbar_arrive(&w_empty[prev_w]);
+    prev_w = -1;
+  };
+  for (int i = 0; has(i); ++i) {
+    const int ab = i % NA;
+    mbar_wait(&a_full[ab], ((uint32_t)(i / NA)) & 1u);
+    // ---- D1 = W7 *_d x: 7 taps x KSTEPS units, three bf16 products each (x_hi w_hi + x_lo w_hi + x_hi w_lo) ----
+    float d[C / 2];
+    {
+      const uint32_t a_addr = smem_u32(sA + ab * A_BYTES);
+      // descriptors are built once; between MMAs only the 14-bit start-address field (>> 4) of the low word moves
+      const uint64_t a_hi0 = wgmma_desc_nosw(a_addr, 128, A_ROWS * 16);
+      const uint64_t a_lo0 = wgmma_desc_nosw(a_addr + NCHUNK * (A_ROWS * 16), 128, A_ROWS * 16);
+      const uint32_t kstep_units = 2 * A_ROWS;       // two chunks, in 16-B units
+#pragma unroll 1
+      for (int j = 0; j < 7; ++j) {
+        const uint32_t row_units = (uint32_t)(j * p.d);
+#pragma unroll
+        for (int kk = 0; kk < KSTEPS; ++kk) {
+          const uint64_t b_hi = unit_b(j * KSTEPS + kk);
+          const uint64_t b_lo = b_hi + (uint64_t)(2 * C);
+          const uint64_t off = (uint64_t)(kk * kstep_units + row_units);
+          wgmma_fence();
+          wgmma_ss<C>(d, a_hi0 + off, b_hi, (j > 0 || kk > 0) ? 1u : 0u);
+          wgmma_ss<C>(d, a_lo0 + off, b_hi, 1u);
+          wgmma_ss<C>(d, a_hi0 + off, b_lo, 1u);
+          unit_done();
+        }
+      }
+      drain();
+      wgmma_fence_acc(d);
+    }
+    if (lane == 0) mbar_arrive(&a_empty[ab]);  // the staged tile may be overwritten
+    // ---- E1: D1 (+b7, ELU, split) -> sA2, [hi / lo][chunk][64 rows][16 B] ----
+#pragma unroll
+    for (int j = 0; j < C / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int col = 8 * j + c_lane;
+        uint32_t hi, lo;
+        split_bf16x2(elu1(d[4 * j + 2 * h] + sBias[col]), elu1(d[4 * j + 2 * h + 1] + sBias[col + 1]), hi, lo);
+        const uint32_t off = (uint32_t)(j * RU_TILE_M + rl + 8 * h) * 16 + c_lane * 2;
+        *reinterpret_cast<uint32_t*>(sA2 + off) = hi;
+        *reinterpret_cast<uint32_t*>(sA2 + NCHUNK * RU_TILE_M * 16 + off) = lo;
+      }
+    fence_proxy_async_smem();  // generic-proxy writes -> wgmma operand reads
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    // ---- D2 = W1 ELU(D1 + b7): A from sA2 ----
+#pragma unroll
+    for (int kk = 0; kk < KSTEPS; ++kk) {
+      const uint64_t b_hi = unit_b(7 * KSTEPS + kk);
+      const uint64_t b_lo = b_hi + (uint64_t)(2 * C);
+      const uint32_t a_off = a2_addr + kk * 2 * (RU_TILE_M * 16);
+      const uint64_t a_hi = wgmma_desc_nosw(a_off, 128, RU_TILE_M * 16);
+      const uint64_t a_lo = wgmma_desc_nosw(a_off + NCHUNK * (RU_TILE_M * 16), 128, RU_TILE_M * 16);
+      wgmma_fence();
+      wgmma_ss<C>(d, a_hi, b_hi, kk > 0 ? 1u : 0u);
+      wgmma_ss<C>(d, a_lo, b_hi, 1u);
+      wgmma_ss<C>(d, a_hi, b_lo, 1u);
+      unit_done();
+    }
+    drain();
+    wgmma_fence_acc(d);
+    // ---- E2: D2 (+b1, ELU, + skip) -> split -> global (C8S) ----
+    const int tile = tile_of(i);
+    const int b = tile / p.tiles_per_clip;
+    const int t0 = (tile - b * p.tiles_per_clip) * RU_TILE_M;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int t = t0 + rl + 8 * h;
+      if (t >= p.T) continue;
+      const __nv_bfloat16* xrow = p.x + ((size_t)b * 2 * NCHUNK * p.T + t) * 8 + c_lane;
+      const RowAddr ya = c8s_row(b, t, 2 * NCHUNK, p.out_phases, p.T);
+#pragma unroll
+      for (int j = 0; j < C / 8; ++j) {
+        const int col = 8 * j + c_lane;
+        const uint32_t hw = __ldg(reinterpret_cast<const uint32_t*>(xrow + (size_t)j * p.T * 8));
+        const uint32_t lw = __ldg(reinterpret_cast<const uint32_t*>(xrow + (size_t)(NCHUNK + j) * p.T * 8));
+        const float v0 = bf16_lo(hw) + bf16_lo(lw) + elu1(d[4 * j + 2 * h] + sBias[C + col]);
+        const float v1 = bf16_hi(hw) + bf16_hi(lw) + elu1(d[4 * j + 2 * h + 1] + sBias[C + col + 1]);
+        uint32_t oh, ol;
+        split_bf16x2(v0, v1, oh, ol);
+        *reinterpret_cast<uint32_t*>(p.y + ya.off + (size_t)j * ya.chunk_stride + c_lane) = oh;
+        *reinterpret_cast<uint32_t*>(p.y + ya.off + (size_t)(NCHUNK + j) * ya.chunk_stride + c_lane) = ol;
+      }
+    }
+    // every thread's sA2 reads by the D2 wgmmas have retired (drain above); E1 of the next tile may overwrite it
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+  }
 }
 
 template <int C>
 static int launch_ru(RuParams p, cudaStream_t stream) {
   using Cfg = RuCfg<C>;
   auto kfn = ru_tc_kernel<C>;
-  p.ar = TILE_M + 6 * p.d;
+  p.ar = RU_TILE_M + 6 * p.d;
   const int a_bytes = 2 * Cfg::NCHUNK * p.ar * 16;
   int smem;
   if (Cfg::RESIDENT) {
@@ -722,12 +485,12 @@ static int launch_ru(RuParams p, cudaStream_t stream) {
     p.nw = 0;
     smem = 2 * a_bytes + Cfg::NUNITS * Cfg::UNIT_BYTES + Cfg::FIXED_BYTES;
   } else {
-    // the weight ring must cover ~1 us of L2 latency at ~42 B/clk of consumption (~70 KB): as many stages as fit; a
-    // second staged activation tile only if that still leaves at least 48 KB of ring
+    // the weight ring must cover the L2 latency of the streamed units: as many stages as fit; a second staged
+    // activation tile only if that still leaves at least 48 KB of ring
     auto stages = [&](int na) {
       return min(Cfg::MAX_NW, (Cfg::MAX_SMEM - na * a_bytes - Cfg::FIXED_BYTES) / Cfg::UNIT_BYTES);
     };
-    p.na = (Cfg::PAIR || (Cfg::NBUF == 2 && stages(2) * Cfg::UNIT_BYTES >= 48 * 1024)) ? 2 : 1;
+    p.na = stages(2) * Cfg::UNIT_BYTES >= 48 * 1024 ? 2 : 1;
     p.nw = stages(p.na);
     if (p.nw < 2) return ALM_ERR_UNSUPPORTED;
     smem = p.na * a_bytes + p.nw * Cfg::UNIT_BYTES + Cfg::FIXED_BYTES;
@@ -738,9 +501,8 @@ static int launch_ru(RuParams p, cudaStream_t stream) {
     ALM_CUDA_OK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_smem = smem;
   }
-  const int ctas_per_sm = (smem <= 110 * 1024 && 2 * Cfg::TMEM_COLS <= 512) ? 2 : 1;
-  const int grid = min(p.total_tiles, num_sms() * ctas_per_sm);
-  kfn<<<grid, CTA_THREADS, smem, stream>>>(p);
+  const int grid = min(p.total_tiles, num_sms() * Cfg::CTAS_PER_SM);
+  kfn<<<grid, RU_THREADS, smem, stream>>>(p);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);
   return ALM_OK;
@@ -751,8 +513,11 @@ static int launch_ru(RuParams p, cudaStream_t stream) {
 //   out[t, co] = b[co] + sum_{j < K} sum_ci W[co, ci, j] xp[ci, t*s + j],  xp[u] = x[u - (K - s)]  (soundstream.py:332-345)
 // Input: C8S with P = s phase planes, so tap j of output row t reads plane ((j - pad) mod s), row t + floor((j - pad) / s):
 // unit-stride rows for every tap.  One pipeline stage = one (tap, 16-channel k-step) unit: A hi/lo [2][128][16 B] each
-// (cp.async, 16 B per lane), W hi/lo [2][BN][16 B] each (one bulk copy); three MMAs per stage.
+// (cp.async, 16 B per lane), W hi/lo [2][BN][16 B] each (one bulk copy); three wgmmas per stage and consumer warpgroup.
+// Warps 0 and 3: producers; warps 4-7 / 8-11: consumer warpgroups for tile rows [0, 64) / [64, 128).
 // ---------------------------------------------------------------------------------------------
+constexpr int CTA_THREADS = 384;
+
 struct ConvParams {
   const __nv_bfloat16* x;   // C8S [B][2 Cin/8][s][Tin/s][8]
   void* y;                  // C8S (out_phases) or fp32 [B][n_out][Cout]
@@ -770,7 +535,6 @@ struct ConvCfg {
   static constexpr int STAGE_BYTES = A_BYTES + W_BYTES;
   static constexpr int STAGES = BN == 256 ? 8 : 10;
   static constexpr int LOOKAHEAD = 3;                   // cp.async groups in flight PER PRODUCER WARP before its oldest is published
-  static constexpr int TMEM_COLS = 2 * BN < 32 ? 32 : 2 * BN;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 512 + 128;
 };
 
@@ -782,27 +546,16 @@ __global__ void __launch_bounds__(CTA_THREADS, 1) conv_tc_kernel(const ConvParam
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
   uint64_t* full = bars;                  // [STAGES]  count 2: W bulk copy (expect_tx) + A (cp.async groups)
-  uint64_t* empty = bars + STAGES;        // [STAGES]
-  uint64_t* acc_full = bars + 2 * STAGES; // [2]
-  uint64_t* acc_empty = acc_full + 2;     // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
+  uint64_t* empty = bars + STAGES;        // [STAGES]  one arrive per consumer warp
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 2);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&acc_full[i], 1);
-      mbar_init(&acc_empty[i], NEW);
+      mbar_init(&empty[i], 8);
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int ksteps = p.Cin / 16;
   const int nch = p.Cin / 8;            // chunks per part
@@ -817,14 +570,14 @@ __global__ void __launch_bounds__(CTA_THREADS, 1) conv_tc_kernel(const ConvParam
     b = r / p.m_tiles;
   };
 
-  if (warp == 0 || warp == 3) {
+  if (warp < 4) {
+    if (warp == 1 || warp == 2) return;
     // ===================== two producer warps (all 32 lanes each): warp 0 stages the even units, warp 3 the odd ones
-    // (one warp's address arithmetic + issue of 16 cp.async per stage could not keep the small-N layers fed:
-    // profiles/r02_ncu_codec_summary.md, conv_tc_kernel<64> at 7 % tensor-pipe activity) =====================
+    // (one warp's address arithmetic + issue of 16 cp.async per stage cannot keep the small-N layers fed) ============
     const int pid = warp == 0 ? 0 : 1;
     int stage = 0, pending = 0, k = 0, done_m = 0;
     uint32_t phase = 0;
-    auto publish_oldest = [&]() {  // this warp's oldest cp.async group has landed: make it visible to the UMMA, signal
+    auto publish_oldest = [&]() {  // this warp's oldest cp.async group has landed: make it visible to wgmma, signal
       fence_proxy_async_smem();
       __syncwarp();
       if (lane == 0) mbar_arrive(&full[(2 * done_m + pid) % STAGES]);
@@ -837,7 +590,6 @@ __global__ void __launch_bounds__(CTA_THREADS, 1) conv_tc_kernel(const ConvParam
       const int t0 = mt * TILE_M;
       const int nrows = min(TILE_M, p.n_out - t0);
       const __nv_bfloat16* xb = p.x + (size_t)b * 2 * nch * p.s * (size_t)rows_in * 8;
-      // (an L2 prefetch of the next tile's rows was tried here and made every layer slower: profiles/r02_codec_layers_c.txt)
       for (int j = 0; j < p.K; ++j) {
         const int q = j - pad;
         const int plane = ((q % p.s) + p.s) % p.s;
@@ -895,112 +647,79 @@ __global__ void __launch_bounds__(CTA_THREADS, 1) conv_tc_kernel(const ConvParam
     }
     cp_async_wait<0>();
     while (pending > 0) publish_oldest();
-  } else if (warp == 1) {
-    {
-      constexpr uint32_t idesc = umma_idesc_bf16_f32(TILE_M, BN, false, false);
-      int stage = 0;
-      uint32_t phase = 0;
-      int iter = 0;
-      // descriptors built once; per stage only the start-address field moves (see ru_tc_kernel)
-      const uint64_t a0 = umma_smem_desc_nosw(smem_u32(smem), 128, TILE_M * 16);
-      const uint64_t b0 = umma_smem_desc_nosw(smem_u32(smem) + Cfg::A_BYTES, 128, BN * 16);
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++iter) {
-        const int acc = iter & 1;
-        mbar_wait(&acc_empty[acc], (((uint32_t)(iter >> 1)) & 1u) ^ 1u);
-        tc_fence_after_sync();
-        const uint32_t d = tmem_base + acc * BN;
-        for (int u = 0; u < units; ++u) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after_sync();
-          const uint64_t off = (uint64_t)(stage * (Cfg::STAGE_BYTES / 16));
-          const uint64_t a_hi = a0 + off, a_lo = a_hi + 2 * TILE_M;
-          const uint64_t b_hi = b0 + off, b_lo = b_hi + 2 * BN;
-          if (elect_one_sync()) {
-            umma_bf16_ss(d, a_hi, b_hi, idesc, u > 0 ? 1u : 0u);
-            umma_bf16_ss(d, a_lo, b_hi, idesc, 1u);
-            umma_bf16_ss(d, a_hi, b_lo, idesc, 1u);
-            umma_commit(&empty[stage]);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        if (elect_one_sync()) umma_commit(&acc_full[acc]);
-      }
+    return;
+  }
+
+  // ===================== consumer warpgroups =====================
+  const int cw = (warp >> 2) - 1;
+  const int rl = cw * 64 + (warp & 3) * 16 + (lane >> 2);  // fragment rows rl, rl + 8 of the tile
+  const int c_lane = 2 * (lane & 3);
+  const int nch_out = p.Cout / 8;
+  int stage = 0;
+  uint32_t phase = 0;
+  // descriptors built once; per stage only the start-address field moves
+  const uint64_t a0 = wgmma_desc_nosw(smem_u32(smem) + cw * 64 * 16, 128, TILE_M * 16);
+  const uint64_t b0 = wgmma_desc_nosw(smem_u32(smem) + Cfg::A_BYTES, 128, BN * 16);
+  float acc[BN / 2];
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    int b, mt, nt;
+    decode(tile, b, mt, nt);
+    int prev = -1;
+    for (int u = 0; u < units; ++u) {
+      mbar_wait(&full[stage], phase);
+      const uint64_t off = (uint64_t)(stage * (Cfg::STAGE_BYTES / 16));
+      const uint64_t a_hi = a0 + off, a_lo = a_hi + 2 * TILE_M;
+      const uint64_t b_hi = b0 + off, b_lo = b_hi + 2 * BN;
+      wgmma_fence();
+      wgmma_ss<BN>(acc, a_hi, b_hi, u > 0 ? 1u : 0u);
+      wgmma_ss<BN>(acc, a_lo, b_hi, 1u);
+      wgmma_ss<BN>(acc, a_hi, b_lo, 1u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1u; }
     }
-  } else if (warp >= 4) {
-    const int ew = warp - 4;
-    const int q = ew & 3, sub = ew >> 2;
-    const int row = q * 32 + lane;
-    const uint32_t lane_sel = (uint32_t)(q * 32) << 16;
-    const int nch_out = p.Cout / 8;
-    int iter = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++iter) {
-      int b, mt, nt;
-      decode(tile, b, mt, nt);
-      const int acc = iter & 1;
-      const int t = mt * TILE_M + row;
-      const bool valid = t < p.n_out;
-      const int n0 = nt * BN;
-      const RowAddr ya = c8s_row(b, valid ? t : 0, 2 * nch_out, p.out_fp32 ? 1 : p.out_phases, p.n_out);
-      mbar_wait(&acc_full[acc], ((uint32_t)(iter >> 1)) & 1u);
-      tc_fence_after_sync();
-      const uint32_t d = tmem_base + acc * BN + lane_sel;
-#pragma unroll 1
-      for (int g = sub; g < BN / 16; g += NSUB) {
-        uint32_t r[16];
-        tmem_ld_32x32b_x16(d + g * 16, r);
-        tmem_ld_wait();
-        const int ch0 = n0 + g * 16;
-        float v[16];
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+
+    const int n0 = nt * BN;
 #pragma unroll
-        for (int e = 0; e < 16; ++e) v[e] = __uint_as_float(r[e]) + (p.bias ? __ldg(p.bias + ch0 + e) : 0.f);
-        if (valid) {
-          if (p.out_fp32) {
-            float* dst = reinterpret_cast<float*>(p.y) + ((size_t)b * p.n_out + t) * p.Cout + ch0;
+    for (int h = 0; h < 2; ++h) {
+      const int t = mt * TILE_M + rl + 8 * h;
+      if (t >= p.n_out) continue;
+      const RowAddr ya = c8s_row(b, t, 2 * nch_out, p.out_fp32 ? 1 : p.out_phases, p.n_out);
 #pragma unroll
-            for (int e = 0; e < 16; e += 4)
-              *reinterpret_cast<float4*>(dst + e) = make_float4(v[e], v[e + 1], v[e + 2], v[e + 3]);
-          } else if (p.up > 1) {
-            // CausalConvTranspose1d as a 2-tap conv with up * C' output columns: column block r is output time t * up + r
-            __nv_bfloat16* yb = reinterpret_cast<__nv_bfloat16*>(p.y);
-            const int creal = p.Cout / p.up, r_ = ch0 / creal, cbase = ch0 - r_ * creal;
-            const size_t t_out = (size_t)t * p.up + r_, T_out = (size_t)p.n_out * p.up;
-            const int nchr = creal / 8;
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-              uint32_t oh[4], ol[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) split_bf16x2(v[8 * c + 2 * e], v[8 * c + 2 * e + 1], oh[e], ol[e]);
-              const int chunk = cbase / 8 + c;
-              *reinterpret_cast<uint4*>(yb + (((size_t)b * 2 * nchr + chunk) * T_out + t_out) * 8) =
-                  make_uint4(oh[0], oh[1], oh[2], oh[3]);
-              *reinterpret_cast<uint4*>(yb + (((size_t)b * 2 * nchr + nchr + chunk) * T_out + t_out) * 8) =
-                  make_uint4(ol[0], ol[1], ol[2], ol[3]);
-            }
-          } else {
-            __nv_bfloat16* yb = reinterpret_cast<__nv_bfloat16*>(p.y);
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-              uint32_t oh[4], ol[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) split_bf16x2(v[8 * c + 2 * e], v[8 * c + 2 * e + 1], oh[e], ol[e]);
-              const int chunk = ch0 / 8 + c;
-              *reinterpret_cast<uint4*>(yb + ya.off + (size_t)chunk * ya.chunk_stride) =
-                  make_uint4(oh[0], oh[1], oh[2], oh[3]);
-              *reinterpret_cast<uint4*>(yb + ya.off + (size_t)(nch_out + chunk) * ya.chunk_stride) =
-                  make_uint4(ol[0], ol[1], ol[2], ol[3]);
-            }
-          }
+      for (int j = 0; j < BN / 8; ++j) {
+        const int ch = n0 + 8 * j + c_lane;  // this thread's channels ch, ch + 1 of the 8-channel chunk n0 / 8 + j
+        const float v0 = acc[4 * j + 2 * h] + (p.bias ? __ldg(p.bias + ch) : 0.f);
+        const float v1 = acc[4 * j + 2 * h + 1] + (p.bias ? __ldg(p.bias + ch + 1) : 0.f);
+        if (p.out_fp32) {
+          float* dst = reinterpret_cast<float*>(p.y) + ((size_t)b * p.n_out + t) * p.Cout + ch;
+          *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+          continue;
+        }
+        uint32_t oh, ol;
+        split_bf16x2(v0, v1, oh, ol);
+        __nv_bfloat16* yb = reinterpret_cast<__nv_bfloat16*>(p.y);
+        if (p.up > 1) {
+          // CausalConvTranspose1d as a 2-tap conv with up * C' output columns: column block r is output time t * up + r
+          const int ch0 = ch - c_lane;
+          const int creal = p.Cout / p.up, r_ = ch0 / creal, cbase = ch0 - r_ * creal;
+          const size_t t_out = (size_t)t * p.up + r_, T_out = (size_t)p.n_out * p.up;
+          const int nchr = creal / 8;
+          const int chunk = cbase / 8;
+          *reinterpret_cast<uint32_t*>(yb + (((size_t)b * 2 * nchr + chunk) * T_out + t_out) * 8 + c_lane) = oh;
+          *reinterpret_cast<uint32_t*>(yb + (((size_t)b * 2 * nchr + nchr + chunk) * T_out + t_out) * 8 + c_lane) = ol;
+        } else {
+          const int chunk = (n0 >> 3) + j;
+          *reinterpret_cast<uint32_t*>(yb + ya.off + (size_t)chunk * ya.chunk_stride + c_lane) = oh;
+          *reinterpret_cast<uint32_t*>(yb + ya.off + (size_t)(nch_out + chunk) * ya.chunk_stride + c_lane) = ol;
         }
       }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[acc]);
     }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  if (warp == 2) tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
 }
 
 template <int BN>
@@ -1054,7 +773,7 @@ extern "C" int alm_codec_ru_tc(const void* x, void* y, const void* w_units, cons
   p.b7 = b7;
   p.b1 = b1;
   p.B = B; p.T = T; p.d = dilation; p.pad_mode = pad_mode; p.out_phases = out_phases;
-  p.tiles_per_clip = ceil_div(T, ctc::TILE_M);
+  p.tiles_per_clip = ceil_div(T, ctc::RU_TILE_M);
   p.total_tiles = p.tiles_per_clip * B;
   switch (C) {
     case 32: return ctc::launch_ru<32>(p, stream);
@@ -1096,25 +815,13 @@ extern "C" int alm_codec_conv_tc(const void* x, void* y, const void* w_units, co
   return ctc::launch_conv<64>(p, stream);
 }
 
-#ifdef ALM_RU_TRACE
-extern "C" int alm_debug_ru_trace(unsigned long long* out16, int reset) {
-  cudaDeviceSynchronize();
-  if (cudaMemcpyFromSymbol(out16, alm::ctc::g_ru_trace, sizeof(unsigned long long) * 16) != cudaSuccess) return -1;
-  if (reset) {
-    unsigned long long z[16] = {0};
-    cudaMemcpyToSymbol(alm::ctc::g_ru_trace, z, sizeof(z));
-  }
-  return 0;
-}
-#endif
-
 extern "C" int alm_codec_pack_c8s(const float* x, void* y, int B, int n, int C, alm_stream_t stream_) {
   using namespace alm;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ALM_REQUIRE(x && y && B > 0 && n > 0 && C > 0 && C % 8 == 0, ALM_ERR_ARG);
   const long long total = (long long)B * n * (C / 8);
   const long long want_blocks = (total + 255) / 256;
-  const int grid = (int)(want_blocks < 148 * 16 ? want_blocks : 148 * 16);
+  const int grid = (int)(want_blocks < num_sms() * 16 ? want_blocks : num_sms() * 16);
   ctc::pack_c8s_kernel<<<grid, 256, 0, stream>>>(x, reinterpret_cast<__nv_bfloat16*>(y), B, n, C);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);

@@ -1,8 +1,8 @@
 // Register-tiled causal Conv1d for the SoundStream stacks (soundstream.py:332-345, 362-395), fp32 CUDA cores.
 //
 // The first-generation kernel (causal_conv1d_kernel in codec.cu) gave each thread a 4 x 4 output tile and spent
-// 5 shared-memory loads per 16 FMAs with run-time kernel size / stride / dilation: 10.8 TFLOP/s (14 % of the
-// fp32 FMA peak, profiles/r01_bench_n1_v8.json).  Here
+// 5 shared-memory loads per 16 FMAs with run-time kernel size / stride / dilation, far below the fp32 FMA peak.
+// Here
 //   * (K, stride, dilation) are template parameters (the 10 shapes SoundStream uses; anything else falls back),
 //     so the tap loop is fully unrolled and all smem offsets are immediates;
 //   * a thread owns COT output channels x TQ output samples (8 x 8 = 64 accumulators): per (channel, tap) it
@@ -10,8 +10,7 @@
 //   * the staged input is split by phase (sample p -> xs[c][p % S][p / S]) so strided convs read consecutive
 //     words across a warp as well;
 //   * input-channel stages are double buffered with cp.async (zero-fill handles padding and ragged edges), so the
-//     global-load latency of stage n+1 hides behind the FMAs of stage n (the synchronous version lost 25 % of its
-//     issue slots to long-scoreboard stalls, profiles/r01_ncu_conv_tiled_k7d9.txt);
+//     global-load latency of stage n+1 hides behind the FMAs of stage n;
 //   * the accumulation order per output is unchanged (input channels ascending, taps ascending, one fp32 FMA
 //     chain), so results are bit-identical to the first-generation kernel and the RVQ indices stay bit-exact.
 // fp32 on CUDA cores is deliberate: the RVQ code search downstream is compared bit-exactly against the fp32
@@ -21,6 +20,11 @@
 
 namespace alm {
 namespace cvt {
+
+// two IEEE fp32 FMAs on a pair of accumulators (sm_90 has no packed f32x2 FMA)
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
 
 constexpr int THREADS = 256;
 // input channels per pipeline stage: more for short kernels so a stage carries enough FMAs to hide its copies
@@ -65,9 +69,7 @@ conv_kernel(const float* __restrict__ x, const float* __restrict__ w, const floa
   const int t0 = blockIdx.x * G::T_TILE, o0 = blockIdx.y * CO_TILE, b = blockIdx.z;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int in0 = t0 * S;
-  // accumulators as float2 pairs along time: the FMAs are issued as packed fma.rn.f32x2 (FFMA2), two IEEE fp32
-  // FMAs per instruction - the kernel is issue-bound (85 % issue-active at 64 % FMA-pipe utilisation with scalar
-  // FFMA, profiles/r01_ncu_conv_tiled_cpasync.txt), and each output still sees the same single FMA chain
+  // accumulators as float2 pairs along time (two time steps per weight load); each output sees a single FMA chain
   float2 acc[COT][TQ / 2];
 #pragma unroll
   for (int i = 0; i < COT; ++i)
@@ -141,7 +143,7 @@ conv_kernel(const float* __restrict__ x, const float* __restrict__ w, const floa
         for (int i = 0; i < COT; ++i) {
           const float2 w2 = make_float2(wv[i], wv[i]);
 #pragma unroll
-          for (int q = 0; q < TQ / 2; ++q) acc[i][q] = __ffma2_rn(w2, xv[q], acc[i][q]);
+          for (int q = 0; q < TQ / 2; ++q) acc[i][q] = ffma2(w2, xv[q], acc[i][q]);
         }
       }
     }
@@ -169,8 +171,7 @@ conv_kernel(const float* __restrict__ x, const float* __restrict__ w, const floa
 // Fused ResidualUnit (soundstream.py:362-369):  y = x + ELU(b1 + W1 . ELU(b7 + conv7_dil(x)))
 // One CTA owns ALL C channels of a time tile, so the k=7 result never leaves the SM: it is written (after bias +
 // ELU) to a [C][T_TILE] shared-memory tile and immediately contracted with the 1x1 weights.  Saves the HBM round
-// trip of the intermediate and the standalone 1x1 launch (which ran at 8-19 TFLOP/s: too little work per byte to
-// hide its own latency).  Both contractions keep the channel-ascending single-FMA-chain order of the unfused
+// trip of the intermediate and the standalone 1x1 launch (too little work per byte to hide its own latency).  Both contractions keep the channel-ascending single-FMA-chain order of the unfused
 // kernels, so the result is bit-identical to conv7 -> conv1.
 // Thread tile: COT = C/8 channels x TQ = 64/COT samples (64 accumulators); T_TILE = 32*TQ; C * T_TILE = 16384.
 // ------------------------------------------------------------------------------------------------
@@ -259,7 +260,7 @@ residual_unit_kernel(const float* __restrict__ x, const float* __restrict__ w7 /
           for (int u = 0; u < 4; ++u) {
             const float2 w2 = make_float2(wv[u], wv[u]);
 #pragma unroll
-            for (int q = 0; q < TQ / 2; ++q) acc[i4 * 4 + u][q] = __ffma2_rn(w2, xv[q], acc[i4 * 4 + u][q]);
+            for (int q = 0; q < TQ / 2; ++q) acc[i4 * 4 + u][q] = ffma2(w2, xv[q], acc[i4 * 4 + u][q]);
           }
         }
       }
@@ -319,7 +320,7 @@ residual_unit_kernel(const float* __restrict__ x, const float* __restrict__ w7 /
         for (int u = 0; u < 4; ++u) {
           const float2 w2 = make_float2(wv[u], wv[u]);
 #pragma unroll
-          for (int q = 0; q < TQ / 2; ++q) acc[i4 * 4 + u][q] = __ffma2_rn(w2, xv[q], acc[i4 * 4 + u][q]);
+          for (int q = 0; q < TQ / 2; ++q) acc[i4 * 4 + u][q] = ffma2(w2, xv[q], acc[i4 * 4 + u][q]);
         }
       }
     }

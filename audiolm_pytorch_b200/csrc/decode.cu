@@ -133,7 +133,7 @@ __global__ void mqa_attn_decode_combine_kernel(const float* __restrict__ partial
 
 // ------------------------------------------------------------------------------------------------
 // out[r, n] = sum_k x[r, k] * W[n, k] (+ bias[n])  for a handful of rows r (decode: r = batch <= 8).
-// With one or a few rows a "GEMM" is a matrix-vector product bound by reading W once; the 128-row tcgen05 tile
+// With one or a few rows a "GEMM" is a matrix-vector product bound by reading W once; the 128-row wgmma tile
 // kernel would put N/256 CTAs on it (4 CTAs for the FFN down projection).  Here every warp owns output columns
 // n, n + warps, ... and streams W rows with 16-byte loads from all SMs; x sits in shared memory.
 // Replaces the nn.Linear calls of a decode step (audiolm_pytorch.py:293-303, 255-259, 621).

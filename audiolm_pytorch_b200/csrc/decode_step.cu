@@ -35,7 +35,7 @@
 // summation order inside dot products differs and 1/sqrt, 1/d use the fast units.  tests/test_decode_gpu.py compares
 // the two paths.
 #include "alm_common.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace alm {
 namespace dstep {

@@ -74,7 +74,7 @@ extern "C" int alm_embed_gather(const float* const* tables, int n_tables, const 
     t.t[i] = tables[i];
   }
   const long long work = (long long)M * (d / 4);
-  const int grid = (int)((work + 255) / 256 < 148 * 16 ? (work + 255) / 256 : 148 * 16);
+  const int grid = (int)((work + 255) / 256 < num_sms() * 16 ? (work + 255) / 256 : num_sms() * 16);
   embed_gather_kernel<<<grid, 256, 0, stream>>>(t, src, out, M, d);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);
@@ -93,7 +93,7 @@ extern "C" int alm_embed_scatter(float* const* grad_tables, int n_tables, const 
     t.t[i] = grad_tables[i];
   }
   const long long work = (long long)M * (d / 4);
-  const int grid = (int)((work + 255) / 256 < 148 * 16 ? (work + 255) / 256 : 148 * 16);
+  const int grid = (int)((work + 255) / 256 < num_sms() * 16 ? (work + 255) / 256 : num_sms() * 16);
   embed_scatter_kernel<<<grid, 256, 0, stream>>>(t, src, dout, M, d);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);

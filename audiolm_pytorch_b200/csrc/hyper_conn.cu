@@ -661,7 +661,7 @@ extern "C" int alm_hc_pre_fwd(const void* R_in, const void* Y, const float* beta
   ALM_REQUIRE((x_expand != nullptr) != (R_in != nullptr), ALM_ERR_ARG);
   if (d <= 1024) {  // second-generation kernel: 2 or 4 warps per token, no CTA-wide barriers
     hc2::Params p2{gamma_hc, dyn_alpha, dyn_beta, static_alpha, static_beta, alpha_scale, beta_scale, ln_gamma};
-    const int tpt = 64;  // 4 warps per token (tpt 128) measured slower at d=1024: 297 vs 227 us
+    const int tpt = 64;  // 2 warps per token (4 warps per token was slower at d=1024)
     const int tok = hc2::THREADS / tpt;
     const int grid = min(ceil_div(M, tok), num_sms() * 2);
     const size_t smem = hc2::fwd_smem(d, tpt);
@@ -732,7 +732,7 @@ extern "C" int alm_hc_pre_bwd(const void* R_in, const void* Y, const float* beta
     hc2::Params p2{gamma_hc, dyn_alpha, dyn_beta, static_alpha, static_beta, alpha_scale, beta_scale, ln_gamma};
     hc2::Grads g2{g_gamma_hc, g_dyn_alpha, g_dyn_beta, g_static_alpha, g_static_beta, g_alpha_scale, g_beta_scale,
                   g_ln_gamma};
-    const int tpt = 64;  // tpt 128 (4 warps per token, 2 CTAs/SM, 128-register cap) measured slower: 883 vs 713 us
+    const int tpt = 64;  // 2 warps per token (tpt 128: 4 warps per token, 2 CTAs/SM, 128-register cap, was slower)
     const int tok = hc2::THREADS / tpt;
     const int grid2 = min(ceil_div(M, tok), num_sms());
     const size_t smem = hc2::bwd_smem(d, tpt);

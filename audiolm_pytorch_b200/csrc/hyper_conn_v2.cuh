@@ -1,6 +1,6 @@
 // Hyper-Connections kernels, second generation: 2 warps per token, 4 tokens per CTA, no CTA-wide barrier.
-// (The first generation in hyper_conn.cu used one CTA per token with 5-6 __syncthreads per token and ran
-// 8-14x off the HBM roofline: profiles/r01_launches_bench_step_v1.csv.)
+// (The first generation in hyper_conn.cu uses one CTA per token with 5-6 __syncthreads per token and runs far off
+// the HBM roofline.)
 //
 //  - a token's 64 threads each own NCH chunks of 8 channels (16-B vector loads, fully coalesced);
 //  - reductions: warp shuffle + one 64-thread named barrier (bar.sync id, 64) through a tiny smem mailbox;

@@ -1,15 +1,15 @@
 // Hyper-Connections backward, third generation (depth(prev) + width + pre-LayerNorm backward of one branch).
 //
 // hc2::pre_bwd_kernel held a token's 16 channels x 10 arrays in registers (255 regs) and the per-channel
-// parameter-gradient accumulators in 128 KB of shared memory: 8 warps per SM, 43 % of the issue slots lost to
-// global-load latency (profiles/r01_ncu_hc_bwd.csv).  This version
+// parameter-gradient accumulators in 128 KB of shared memory: 8 warps per SM, too few to hide global-load latency.
+// This version
 //   * streams the token twice in 4-channel pieces (pass 1: every per-token dot product in ONE reduction,
 //     pass 2: gradients; the second read hits L1/L2), so it fits 128 registers -> 2 CTAs (16 warps) per SM;
 //   * uses the forward's pre-activations z (kept in aux) so that the RMS-norm backward needs no reduction:
 //       sum_d u_s[d] R_s[d] = (1/inv_s) * sum_c dz[s][c] z[s][c];
 //   * moves the per-channel parameter gradients (dyn_alpha, dyn_beta, gamma) out of the kernel: it emits
 //     W[t,s,c] = inv_s * dz[s][c] and the caller forms G[d,c] = sum_{t,s} R[t,s,d] W[t,s,c] with two skinny
-//     tcgen05 GEMMs (R = R_in + beta_prev (x) Y), finished by hc_param_finish_kernel.
+//     wgmma GEMMs (R = R_in + beta_prev (x) Y), finished by hc_param_finish_kernel.
 // Reference semantics: hyper_connections.HyperConnections width/depth connections as called from
 // audiolm_pytorch.py:446-454, 524-551 (third-party dependency, restated in oracle/third_party.py).
 #pragma once
@@ -44,11 +44,13 @@ __device__ __forceinline__ void slot_sum(float (&v)[N], float* mail /*[2][WPT][M
   which ^= 1;
 }
 
-// packed fp32 pairs (fma.rn.f32x2 / add / mul): the kernel is FMA-issue bound, two channels per instruction
+// fp32 channel pairs (two IEEE fp32 operations each; sm_90 has no packed f32x2 arithmetic)
 __device__ __forceinline__ float2 dup2(float a) { return make_float2(a, a); }
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return __ffma2_rn(a, b, c); }
-__device__ __forceinline__ float2 add2(float2 a, float2 b) { return __fadd2_rn(a, b); }
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return __fmul2_rn(a, b); }
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 __device__ __forceinline__ void unpack4p(const uint2& u, float2* f) {  // 4 bf16 -> two (even, odd) channel pairs
   f[0] = make_float2(bf16_lo(u.x), bf16_hi(u.x));
   f[1] = make_float2(bf16_lo(u.y), bf16_hi(u.y));

@@ -6,14 +6,14 @@
 //
 // The 2 N C D flops of r.e_c (8.4 MFLOP per frame) are what made the fp32 CUDA-core kernel (codec.cu) FMA-bound.
 // Here, per stage:
-//   1. S = R' B'^T on the tcgen05 GEMM (alm_gemm_bf16) with the split-bf16 trick folded into K:
+//   1. S = R' B'^T on the wgmma GEMM (alm_gemm_bf16) with the split-bf16 trick folded into K:
 //        R' = [r_hi | r_lo | r_hi]  (N x 3D),  B' = [e_hi | e_hi | e_lo]  (C x 3D)   =>  S ~ r.e to ~2^-16 relative
 //   2. rvq_select_kernel (one warp per row): approximate scores a_c = |e_c|^2 - 2 S_c pick the CANDIDATES
 //      (everything within the bf16x3 error bound of the best); each candidate's distance is then re-evaluated in
 //      fp32 with the reference's expansion and the winner (lowest index on ties) is chosen among them, so the emitted
 //      index is the fp32 argmin, not the approximate one.  The warp then updates r, quantized and the next stage's R'.
 #include "alm_common.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace alm {
 namespace rvq {

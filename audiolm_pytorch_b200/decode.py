@@ -2,8 +2,8 @@
 1608-1740, 1896-2039).
 
 The reference (and `Transformer._forward_cached`) re-concatenate the per-layer cache with `torch.cat` every step
-and launch ~60 kernels + as many torch ops per token from Python: 1.9-2.3 ms per token, all of it host and
-launch overhead (profiles/r01_decode_latency_c5.json).  Here one decode step
+and launch ~60 kernels + as many torch ops per token from Python, so a token costs host and launch overhead rather
+than GPU work.  Here one decode step
 
     embed(last token) -> 6 x [hyper-connection pre, q/kv GEMMs, kv append, decode attention, out GEMM,
                               hyper-connection pre, W1 GEMM, GEGLU+LN, W2 GEMM] -> post + LN -> head -> top-k Gumbel
@@ -25,9 +25,10 @@ bf16 = torch.bfloat16
 f32 = torch.float32
 
 
-# one persistent kernel per token (csrc/decode_step.cu) instead of ~11 launches per layer; off = the multi-kernel step
-# (kept: it is the independent implementation the fused step is tested against, and it takes more than 4 rows)
-FUSED_STACK_STEP = True
+# on = one persistent kernel per token (csrc/decode_step.cu) instead of ~11 launches per layer; off = the multi-kernel
+# step replayed from a CUDA graph.  Off by default: on the H100 the one-kernel step measured slower (486 vs 401 us per
+# token at batch 1, 600 cached positions; DESIGN.md §4.3).  Both paths are tested against each other.
+FUSED_STACK_STEP = False
 
 
 def engine_supported(tr: Transformer) -> bool:

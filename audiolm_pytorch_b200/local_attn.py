@@ -55,7 +55,7 @@ class LocalMHA(nn.Module):
         if not (causal and prenorm and qk_rmsnorm and use_xpos and use_rotary_pos_emb and gate_values_per_head):
             raise NotImplementedError("LocalMHA is built for the configuration soundstream.py:418-427 uses")
         if dim_head != 64:
-            raise NotImplementedError("the sm_100a attention kernel is built for dim_head=64")
+            raise NotImplementedError("the sm_90a attention kernel is built for dim_head=64")
         if dim % 8 != 0:
             raise ValueError("dim must be a multiple of 8")
         inner = dim_head * heads
@@ -104,7 +104,7 @@ class LocalMHA(nn.Module):
         wo = pk.get("o", [self.to_out.weight], lambda: pack_plain(self.to_out.weight))
         xn = F.layer_norm(x.to(f32), (dim,), self.norm.weight, self.norm.bias, self.norm.eps)
         xb = xn.reshape(b * n, dim).to(bf16)
-        qkv = ops.gemm(xb, wqkv).view(b, n, 3, h, dh).float()                     # tcgen05 GEMM
+        qkv = ops.gemm(xb, wqkv).view(b, n, 3, h, dh).float()                     # wgmma GEMM
         q, k, v = (qkv[:, :, i].transpose(1, 2) for i in range(3))               # [b, h, n, dh]
         q = F.normalize(q, dim=-1) * self.q_scale
         k = F.normalize(k, dim=-1) * self.k_scale

@@ -1,6 +1,6 @@
 """Python faces of the C-ABI kernels (raw ops; the autograd wiring lives in transformer.py / heads.py / rel_pos.py).
 
-Every function here launches hand-written sm_100a kernels from libalm_b200.so on the current CUDA
+Every function here launches hand-written sm_90a kernels from libalm_b200.so on the current CUDA
 stream.  No function has a CPU or stock-PyTorch implementation.
 """
 from __future__ import annotations
@@ -8,6 +8,20 @@ from __future__ import annotations
 import torch
 
 from . import _lib
+
+_SMS: dict[int, int] = {}
+
+
+def num_sms(device=None) -> int:
+    """SM count of a CUDA device (the current one by default) for the launch heuristics: 132 on an H100 SXM, 114 on
+    an H100 PCIe."""
+    idx = None if device is None else torch.device(device).index
+    if idx is None:
+        idx = torch.cuda.current_device()
+    if idx not in _SMS:
+        _SMS[idx] = torch.cuda.get_device_properties(idx).multi_processor_count
+    return _SMS[idx]
+
 
 bf16 = torch.bfloat16
 f32 = torch.float32
@@ -65,7 +79,7 @@ def _check_cuda(*ts):
 
 
 def gemm(a, b, *, a_mn=False, b_mn=False, out=None, out_dtype=bf16, alpha=1.0, bias=None,
-         acc_mode=0, split_k=1, cls="gemm_bf16_tcgen05"):
+         acc_mode=0, split_k=1, cls="gemm_bf16_wgmma"):
     """out[b,m,n] (op)= alpha * sum_k A(m,k) B(n,k) (+bias[n]).   bf16 operands, fp32 accumulate.
 
     a: [(batch,) M, K] (a_mn=False) or [(batch,) K, M] (a_mn=True); row stride must be a multiple of 8.
@@ -195,7 +209,7 @@ def mqa_attn_fwd(q, k, v, *, heads, key_mask=None, causal=True, scale=None, retu
     # algorithmic FLOPs: QK^T + PV over the visible (lower-triangle) part only
     vis = (n_q * n_k - n_q * (n_q - 1) / 2) if causal else n_q * n_k
     bhs, brs = _check_bias(bias, heads, n_q, n_k) if bias is not None else (0, 0)
-    with _timed("mqa_attn_fwd_tcgen05", 4.0 * b * heads * 64 * vis):
+    with _timed("mqa_attn_fwd_wgmma", 4.0 * b * heads * 64 * vis):
         _lib.call(
             "alm_mqa_attn_fwd",
             q, q.stride(1), k, k.stride(1), k.stride(0), v, v.stride(1), v.stride(0), key_mask,
@@ -231,7 +245,7 @@ def mqa_attn_bwd(q, k, v, o, d_o, lse, *, heads, key_mask=None, causal=True, sca
     if dbias is not None:
         assert bias is not None and dbias.dtype == f32 and dbias.shape == bias.shape and dbias.stride() == bias.stride()
     vis = (n_q * n_k - n_q * (n_q - 1) / 2) if causal else n_q * n_k
-    with _timed("mqa_attn_bwd_tcgen05", 10.0 * b * heads * 64 * vis):  # 5 matmuls (algorithmic; 7 executed)
+    with _timed("mqa_attn_bwd_wgmma", 10.0 * b * heads * 64 * vis):  # 5 matmuls (algorithmic; 7 executed)
         _lib.call(
             "alm_mqa_attn_bwd",
             q, q.stride(1), k, k.stride(1), k.stride(0), v, v.stride(1), v.stride(0), d_o, d_o.stride(1), key_mask,
@@ -274,7 +288,7 @@ def mqa_attn_decode(q, k_cache, v_cache, cache_len, *, heads, key_mask=None, sca
     if key_mask is not None:
         assert key_mask.dtype == torch.uint8 and key_mask.shape[0] == b and key_mask.shape[1] >= max_len
     if splits is None:  # enough CTAs to spread a long cache over the SMs, fixed per cache size (static launch)
-        splits = max(1, min(32, max_len // 128, 148 // max(1, b)))
+        splits = max(1, min(32, max_len // 128, num_sms(q.device) // max(1, b)))
     ws = torch.empty(b, splits, heads, 66, device=q.device, dtype=f32) if splits > 1 else None
     _lib.call("alm_mqa_attn_decode", q, q.stride(0), k_cache, v_cache, k_cache.stride(0), cache_len, max_len, key_mask,
               0 if key_mask is None else key_mask.stride(0), o, o.stride(0), ws, splits, b, heads,
@@ -428,7 +442,7 @@ def hc_pre_bwd(hc, ln_gamma, grads, g_ln_gamma, aux, dR_out, dxn, dbeta, *, dbin
         dR_in = torch.empty(M, streams, d, device=dev, dtype=bf16)
         dY = torch.empty(M, d, device=dev, dtype=bf16)
         dbp = torch.empty(M, streams, device=dev, dtype=f32)
-    # hc3 path: per-channel parameter gradients via two skinny tcgen05 GEMMs instead of in-kernel accumulators
+    # hc3 path: per-channel parameter gradients via two skinny wgmma GEMMs instead of in-kernel accumulators
     split = x_expand is None and d <= 1024 and HC_BWD_SPLIT
     w = torch.empty(M * streams, 8, device=dev, dtype=bf16) if split else None
     wy = torch.empty(M, 8, device=dev, dtype=bf16) if split else None
@@ -441,10 +455,10 @@ def hc_pre_bwd(hc, ln_gamma, grads, g_ln_gamma, aux, dR_out, dxn, dbeta, *, dbin
     if split:
         G = torch.zeros(d, 8, device=dev, dtype=f32)
         rows = M * streams
-        sk = max(1, min(64, (rows // 64) // 8, 2 * 148 // max(1, (d + 127) // 128)))
+        sk = max(1, min(64, (rows // 64) // 8, 2 * num_sms(dev) // max(1, (d + 127) // 128)))
         # (HBM-bound: they stream R_in / Y once; kept out of the tensor-bound GEMM class of the roofline)
         gemm(R_in.view(rows, d), w, a_mn=True, b_mn=True, out=G, acc_mode=2, split_k=sk, cls="gemm_skinny_hc_param_grad")
-        sk = max(1, min(64, (M // 64) // 8, 2 * 148 // max(1, (d + 127) // 128)))
+        sk = max(1, min(64, (M // 64) // 8, 2 * num_sms(dev) // max(1, (d + 127) // 128)))
         gemm(Y, wy, a_mn=True, b_mn=True, out=G, acc_mode=2, split_k=sk, cls="gemm_skinny_hc_param_grad")
         _lib.call("alm_hc_param_finish", G, hc["gamma"], hc["dyn_alpha"], hc["dyn_beta"], grads["gamma"],
                   grads["dyn_alpha"], grads["dyn_beta"], d)

@@ -5,7 +5,7 @@ override (:926-936) and the fine transformer's 2-D (position, quantizer) bias ML
 
 All three are "a small MLP evaluated on a few thousand relative offsets -> table [P, heads] -> gathered
 into a dense [heads, i, j] bias, with some positions replaced by a learned per-head scalar".  Here the
-D x D layers of the MLP run on the tcgen05 GEMM (through heads._LinearPacked: forward, dgrad, wgrad),
+D x D layers of the MLP run on the wgmma GEMM (through heads._LinearPacked: forward, dgrad, wgrad),
 the gather / scatter-add over the 134 MB dense bias is `alm_bias_gather_fwd/bwd`, and the attention
 kernels add the bias to the scores and accumulate d(bias) (`alm_mqa_attn_fwd/bwd`).  Only the first
 layer (fan-in 1 or 2: an outer product, not a GEMM) and the SiLUs on the [P, D] table are torch

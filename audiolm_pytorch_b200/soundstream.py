@@ -1,4 +1,4 @@
-"""SoundStream codec inference path on libalm_b200 (sm_100a): causal conv encoder -> residual VQ -> decoder.
+"""SoundStream codec inference path on libalm_b200 (sm_90a): causal conv encoder -> residual VQ -> decoder.
 
 Drop-in surface of /root/reference/audiolm_pytorch/soundstream.py:314-395, 451-866 for the calls the AudioLM
 hot path makes: `forward(x, return_encoded=True | return_codes_only=True | return_recons_only=True)`,

@@ -1,10 +1,10 @@
-"""Transformer blocks of the AudioLM hot path, running on libalm_b200 (sm_100a).
+"""Transformer blocks of the AudioLM hot path, running on libalm_b200 (sm_90a).
 
 Class names, constructor kwargs and state_dict keys follow the reference
 (/root/reference/audiolm_pytorch/audiolm_pytorch.py:191-560, attend.py:35-146) so checkpoints load
 unchanged; the arithmetic is one hand-orchestrated forward/backward over the C-ABI kernels:
 
-    per branch:   [hc_pre: depth(prev) + width + LayerNorm]  ->  tcgen05 GEMMs / attention / GEGLU+LN
+    per branch:   [hc_pre: depth(prev) + width + LayerNorm]  ->  wgmma GEMMs / attention / GEGLU+LN
     end of stack: [hc_post: depth + reduce_streams + final LayerNorm]
 
 Activations are bf16 with fp32 accumulation (the reference's bf16-autocast numerics), parameters stay
@@ -74,7 +74,7 @@ class Attention(nn.Module):
                  num_null_kv=0, dropout=0.1, scale=8, flash=False):
         super().__init__()
         if dim_head != 64:
-            raise NotImplementedError("the sm_100a attention kernels are built for dim_head=64")
+            raise NotImplementedError("the sm_90a attention kernels are built for dim_head=64")
         if num_null_kv > 0 or exists(dim_context) and dim_context != dim:
             raise NotImplementedError("cross attention / null kv (text conditioning) is out of scope")
         self.heads = heads
@@ -184,8 +184,11 @@ def pack_w1(w, inner):
     return out
 
 
-def best_split_k(M, N, K, n_sm=148):
-    """split-K factor for weight-gradient GEMMs (few output tiles, very long K)."""
+def best_split_k(M, N, K, n_sm=None):
+    """split-K factor for weight-gradient GEMMs (few output tiles, very long K); n_sm: SMs of the current device (132,
+    the H100 SXM's count, when no device is present: the heuristic itself is host logic)."""
+    if n_sm is None:
+        n_sm = ops.num_sms() if torch.cuda.is_available() else 132
     bn = 64 if N <= 64 else (128 if N <= 128 or (-(-N // 128) * 128) * 10 < (-(-N // 256) * 256) * 9 else 256)
     tiles = -(-M // 128) * -(-N // bn)
     kb = -(-K // 64)

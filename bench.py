@@ -69,7 +69,8 @@ def peaks():
         d = json.loads(p.read_text())
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sustained=d["bf16_tflops_sustained"],
                     src="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, src="fallback (B200_PROFILING.md)")
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0,
+                src="H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense BF16 at 700 W), not a measured peak")
 
 
 class ClockSampler(threading.Thread):
@@ -144,8 +145,8 @@ class ClockSampler(threading.Thread):
 
 
 # ------------------------------------------------------------------------------------------------
-# reference algorithm on the CPU (oracle port of the reference path; the real package cannot be
-# installed offline and /root/reference does not exist on the GPU box)
+# reference algorithm on the CPU (oracle port of the reference path; the real package and its third-party
+# dependencies are not installed alongside this project)
 # ------------------------------------------------------------------------------------------------
 def cpu_step_fn(batch):
     from oracle import transformer as ot
@@ -388,6 +389,7 @@ def decode_stack_step_us(dev, cache_len=600):
 
     tr = Transformer(dim=1024, depth=6, heads=8, flash_attn=True).to(dev).eval()
     res = {"cache_len": cache_len}
+    default = decode.FUSED_STACK_STEP
     for fused in (False, True):
         decode.FUSED_STACK_STEP = fused
         try:
@@ -406,33 +408,46 @@ def decode_stack_step_us(dev, cache_len=600):
             torch.cuda.synchronize()
             res["one_kernel_us" if fused else "multi_kernel_us"] = round(e0.elapsed_time(e1) * 10, 1)
         finally:
-            decode.FUSED_STACK_STEP = True
+            decode.FUSED_STACK_STEP = default
     return res
-
-
-def gemm_traffic_from_profile():
-    """DRAM bytes (read + write) per GEMM launch from the committed ncu capture of this command's step
-    (`--metrics dram__bytes_read.sum,dram__bytes_write.sum`): parsed at run time from profiles/, newest round first."""
-    import csv
-    for name in ("r02_ncu_gemm_dram_bytes_per_launch_one_step.csv", "r01_ncu_gemm_dram_bytes_per_launch_one_step.csv"):
-        f = ROOT / "profiles" / name
-        if not f.exists():
-            continue
-        total, ids = 0.0, set()
-        for row in csv.reader(open(f, errors="replace")):
-            # (the fused head + cross-entropy instantiation <BN, 0, 0, 1> is its own class, `gemm_head_ce_fused`)
-            if len(row) >= 15 and row[0].isdigit() and "gemm_bf16_tcgen05" in row[4] and ", 1>(" not in row[4] \
-                    and row[12].startswith("dram__bytes"):
-                total += float(row[14])
-                ids.add(row[0])
-        if ids:
-            return total / len(ids), f"profiles/{name} ({len(ids)} launches)"
-    return None, None
 
 
 # ------------------------------------------------------------------------------------------------
 # our CUDA path
 # ------------------------------------------------------------------------------------------------
+GRAD_SAMPLE = 1 << 22  # gradient entries kept by --dump-outputs (16 MB of fp32)
+
+
+def dump_outputs(out_dir, loss, model, bucket):
+    """What a caller of the timed step receives: the loss and every parameter gradient.  The flat fp32 gradient is
+    larger than a dump should be, so it is stored as a fixed, seeded sample of its entries (the same indices on every
+    run of the same configuration) plus the float64 norm of every parameter's gradient; inputs and weights are seeded,
+    so two builds can be compared file by file."""
+    import numpy as np
+
+    out_dir.mkdir(parents=True, exist_ok=True)
+    torch.cuda.synchronize()
+    n = bucket.flat.numel()
+    idx = torch.randint(0, n, (min(GRAD_SAMPLE, n),), generator=torch.Generator().manual_seed(0)).sort().values
+    arrays = {
+        "loss": loss.detach().float().reshape(1).cpu(),
+        "grad_sample": bucket.flat.index_select(0, idx.to(bucket.flat.device)).float().cpu(),
+        "grad_norms": torch.stack([p.grad.double().norm() for p in model.parameters()]).cpu(),
+    }
+    for name, t in arrays.items():
+        np.save(out_dir / f"{name}.npy", t.numpy())
+
+
+def power_limit_w(index):
+    """the card's power limit (the speed of a power-capped H100 depends on it), None when NVML is unavailable"""
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        return pynvml.nvmlDeviceGetEnforcedPowerLimit(pynvml.nvmlDeviceGetHandleByIndex(index)) / 1000.0
+    except Exception:
+        return None
+
+
 def main_ours(args):
     import torch.distributed as dist
 
@@ -454,13 +469,13 @@ def main_ours(args):
     model = CoarseTransformer(**CFG).to(dev).train()
     wrapper = CoarseTransformerWrapper(transformer=model, codec=_CodecStub()).train()  # reference defaults
     bucket = FlatGradBucket(model.parameters()).attach(model)
-    # default: ONE ncclAvg all-reduce of the flat bucket after the backward.  Overlapping (half / per layer) was measured
-    # at N=2 on B200 and lost both times (profiles/r02_allreduce_n2.md): the persistent GEMMs own all 148 SMs
+    # default: ONE ncclAvg all-reduce of the flat bucket after the backward.  Overlapping (half / per layer) is opt-in:
+    # the persistent GEMMs occupy every SM, so the collective's kernels find little room to run under the backward
     overlap = world > 1 and os.environ.get("ALM_OVERLAP_ALLREDUCE", "0") != "0"
     if overlap:
         # the upper half of the stack (layers depth/2 .. depth-1: ~half of the bucket) is all-reduced on NCCL's stream
         # as soon as its gradients are final, under the backward of the lower half; finish() sends the rest.
-        # (ALM_OVERLAP_ALLREDUCE=layers: one collective per layer - measured slower in round 1; =0: single all-reduce)
+        # (ALM_OVERLAP_ALLREDUCE=layers: one collective per layer; =0: single all-reduce)
         layers = model.transformer.layers
         ranges = [bucket.range_of(list(layer.parameters())) for layer in layers]
         if os.environ.get("ALM_OVERLAP_ALLREDUCE") == "layers":
@@ -532,8 +547,11 @@ def main_ours(args):
     if sampler:
         sampler.start()
     _lib.reset_launch_count()
-    ms_total = timed(lambda: step(wsem_d, wco_d), args.steps)
+    last = {}
+    ms_total = timed(lambda: last.__setitem__("loss", step(wsem_d, wco_d)), args.steps)
     launches = _lib.launch_count() / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(Path(args.dump_outputs), last["loss"], model, bucket)
 
     # ---- end to end: pinned host ids -> device, loss -> host, every step ----
     def e2e_step():
@@ -557,7 +575,7 @@ def main_ours(args):
         bucket.all_reduce_mean()
         ms_allreduce = timed(lambda: bucket.all_reduce_mean(), 5) / 5
 
-    # ---- roofline of the dominant kernel class (tcgen05 GEMM), events on the launching stream ----
+    # ---- roofline of the dominant kernel class (wgmma GEMM), events on the launching stream ----
     barrier()
     ops.profile_start()
     for _ in range(2):
@@ -571,17 +589,16 @@ def main_ours(args):
     pk = peaks()
     tokens = world * BATCH * SEQ
     ms_step = ms_total / args.steps
-    g_ms, g_flops, g_n = prof.get("gemm_bf16_tcgen05", (0.0, 0.0, 0))
+    g_ms, g_flops, g_n = prof.get("gemm_bf16_wgmma", (0.0, 0.0, 0))
     achieved = g_flops / (g_ms * 1e-3) / 1e12 if g_ms > 0 else 0.0
     kern = {}
     for cls, (ms_, work, n_) in prof.items():
         rate = work / (ms_ * 1e-3) if ms_ else 0.0
         kern[cls] = {"ms_per_step": ms_ / 2, "launches_per_step": n_ / 2}
-        if ops.CLASS_UNIT.get(cls) == "byte":  # HBM-bound classes: algorithmic bytes / time vs the measured copy peak
+        if ops.CLASS_UNIT.get(cls) == "byte":  # HBM-bound classes: algorithmic bytes / time vs the HBM peak
             kern[cls].update(gbps=rate / 1e9, frac_of_hbm_peak=rate / 1e9 / pk["hbm"] if pk.get("hbm") else None)
         else:
             kern[cls]["tflops"] = rate / 1e12
-    traffic, traffic_src = gemm_traffic_from_profile()
     step_tflop = 388e6 * BATCH * SEQ / 1e12  # SURVEY 8(d): 388 MFLOP/token fwd+bwd
 
     line = {
@@ -590,7 +607,7 @@ def main_ours(args):
         "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "config": {"workload": WORKLOAD + ((" + grad all-reduce" + (" (overlapped with the backward)" if overlap else "")) if world > 1 else ""),
                    "global_batch": world * BATCH, "seq_len": SEQ, "parallelism": f"dp{world}", "params": n_params,
-                   "l2": "working set (~9 GB of saved activations per step) far exceeds the 126 MB L2"},
+                   "l2": "working set (~9 GB of saved activations per step) far exceeds the 50 MB L2"},
         "e2e": {"value": tokens / (ms_e2e / args.steps * 1e-3), "unit": "tokens/s",
                 "h2d_bytes_per_step": (wsem_pin.numel() + wco_pin.numel()) * 8, "d2h_bytes_per_step": 4},
         "gpu_launches": launches,
@@ -601,11 +618,10 @@ def main_ours(args):
         "step_mfu": {"algorithmic_tflop_per_step_per_gpu": step_tflop,
                      "achieved_tflops": step_tflop / (ms_step * 1e-3), "peak": pk["tf_sustained"],
                      "frac": step_tflop / (ms_step * 1e-3) / pk["tf_sustained"]},
-        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_tcgen05_kernel (all fwd/dgrad/wgrad launches of a step)",
+        "gpu": {"name": torch.cuda.get_device_name(dev), "power_limit_w": power_limit_w(local)},
+        "roofline": {"bound": "tensor", "kernel": "gemm_bf16_wgmma_kernel (all fwd/dgrad/wgrad launches of a step)",
                      "achieved": achieved, "peak": pk["tf_sustained"], "unit": "TFLOP/s",
                      "frac": achieved / pk["tf_sustained"] if pk["tf_sustained"] else None,
-                     "traffic": traffic, "traffic_unit": "DRAM bytes (read + write) per launch, class average",
-                     "traffic_source": traffic_src,
                      "algorithmic_flops_per_launch": g_flops / g_n if g_n else None,
                      "peak_source": pk["src"] + ", sustained figure (kernel timed inside a long step)"},
         "kernels": kern,
@@ -632,7 +648,7 @@ def main_ours(args):
             tps, ms_cpu, cores = run_cpu(steps=1, warmup=1)
             line["cpu_baseline"] = {"value": tps, "unit": "tokens/s", "cores": cores, "kind": "port",
                                     "sample": f"1 warm-up + 1 timed fwd+bwd of batch 1 x {SEQ} tokens, fp32 oracle port "
-                                              "(restatement of the reference's modules; /root/reference is absent on the GPU box)"}
+                                              "(restatement of the reference's modules)"}
         except Exception as e:  # pragma: no cover
             line["cpu_baseline"] = {"error": repr(e)}
     emit(line)
@@ -640,14 +656,23 @@ def main_ours(args):
         dist.destroy_process_group()
 
 
+def _positive_int(text):
+    v = int(text)
+    if v < 1:
+        raise argparse.ArgumentTypeError(f"must be at least 1, got {v}")
+    return v
+
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=_positive_int, default=10, help="timed steps (at least 1)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the bounded CPU baseline leg")
     ap.add_argument("--headline-only", action="store_true", help="skip the extra C1/C2/C4/C5 legs of the N=1 line")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (loss, gradients) to DIR/<name>.npy")
     a = ap.parse_args()
     # NCCL / torch may print banners ("NCCL version ...") on fd 1: keep stdout for the JSON line only
     sys.stdout.flush()

@@ -1,10 +1,10 @@
 /*
- * libalm_b200 — C ABI of the B200-native AudioLM hot path.
+ * libalm_b200 — C ABI of the CUDA-native AudioLM hot path (H100, sm_90a).
  *
  * The reference (lucidrains/audiolm-pytorch) has no FFI / plugin registry: its hot path is reached
  * through Python classes that call torch library kernels.  This header is the boundary a maintainer
  * would bind instead (ctypes stub shown in INTEGRATION.md).  Each entry point names the reference
- * call it replaces (file:line under /root/reference/audiolm_pytorch/).
+ * call it replaces (file:line in the reference package audiolm_pytorch/).
  *
  * Conventions
  *   - every pointer is a DEVICE pointer owned by the caller (PyTorch allocates everything);
@@ -39,9 +39,9 @@ const char* alm_status_string(int code);
 unsigned long long alm_launch_count(void); /* kernels launched by this library since the last reset */
 void alm_reset_launch_count(void);
 
-/* ---- dense contractions (tcgen05 + TMA) ---------------------------------------------------- */
+/* ---- dense contractions (wgmma + TMA) ------------------------------------------------------ */
 /*
- * C[b,m,n] (op)= alpha * sum_k A(b,m,k) * B(b,n,k)  [+ bias[n]]        bf16 x bf16 -> fp32 accumulate in TMEM
+ * C[b,m,n] (op)= alpha * sum_k A(b,m,k) * B(b,n,k)  [+ bias[n]]        bf16 x bf16 -> fp32 accumulate in registers
  *   a_mn = 0: A(m,k) = A[b*strideA + m*lda + k]   ("K-major", e.g. activations x[M,K])
  *   a_mn = 1: A(m,k) = A[b*strideA + k*lda + m]   ("MN-major", e.g. dy^T for weight gradients)
  *   b_mn likewise for B(n,k).   c_fp32: 0 -> bf16 output, 1 -> fp32 output.
@@ -55,7 +55,7 @@ int alm_gemm_bf16(const void* A, int a_mn, int64_t lda, int64_t strideA, const v
                   int64_t strideB, void* C, int c_fp32, int64_t ldc, int64_t strideC, int M, int N, int K, int batch,
                   float alpha, const float* bias, int acc_mode, int split_k, alm_stream_t stream);
 
-/* ---- multi-query attention (tcgen05 + TMA, flash-style online softmax) ----------------------- */
+/* ---- multi-query attention (wgmma + TMA, flash-style online softmax) ------------------------- */
 /*
  * Token embeddings of the three transformers (audiolm_pytorch.py:686-699, 896-918, 1188-1223): every position is the
  * sum of up to two rows of a handful of fp32 parameter tables [rows_k, d] (start token, nn.Embedding rows, quantizer
@@ -94,8 +94,8 @@ int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int
                      int n_q, int n_k, int causal, float scale, alm_stream_t stream);
 
 /*
- * Backward of alm_mqa_attn_fwd (two tcgen05 kernels: dK/dV per key block accumulating over all heads
- * in TMEM, then dQ per query block).  lse/delta are [b, h, n_q_pad] with n_q_pad a multiple of 128;
+ * Backward of alm_mqa_attn_fwd (two wgmma kernels: dK/dV per key block accumulating over all heads
+ * in registers, then dQ per query block).  lse/delta are [b, h, n_q_pad] with n_q_pad a multiple of 128;
  * delta = rowsum(dO * O) from alm_attn_delta.  Autograd of attend.py:69-146.
  */
 int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int64_t k_bstride, const void* v,

@@ -11,16 +11,15 @@ from __future__ import annotations
 
 import sys
 import warnings
-from pathlib import Path
 
 import torch
 
 from . import codec as oc
-from . import ref_import
+from . import golden, ref_import
 from . import third_party as tp
 from . import transformer as ot
 
-GOLDEN = Path(__file__).resolve().parent.parent / "tests" / "golden"
+GOLDEN = golden.GOLDEN
 TOL = 2e-4
 
 
@@ -102,7 +101,7 @@ def golden_attend(ref):
     check("attend vs flash", ot.attend(q, k, v, mask=mask), out["flash_masked"])
     check("attend causal", ot.attend(q, k, v), out["math_causal"])
     check("attend cached", ot.attend(q[:, :, -5:], k, v, mask=mask), out["math_cached"])
-    torch.save(dict(q=q, k=k, v=v, mask=mask, bias=bias, out=out), GOLDEN / "attend.pt")
+    golden.save(dict(q=q, k=k, v=v, mask=mask, bias=bias, out=out), "attend.pt")
 
 
 def golden_semantic(ref):
@@ -143,9 +142,9 @@ def golden_semantic(ref):
     labels = torch.cat((ids, torch.full((2, 1), 50)), dim=1)
     ol, _ = ot.semantic_forward(st, labels[:, :-1], **hk)
     check("wrapper loss", ot.cross_entropy(ol, labels), loss.detach())
-    torch.save(dict(kwargs=kw, state=st, ids=ids, mask=mask, logits=logits, logits_masked=logits_masked,
+    golden.save(dict(kwargs=kw, state=st, ids=ids, mask=mask, logits=logits, logits_masked=logits_masked,
                     cache12=cache, logits_inc=l_inc, loss=loss.detach(), grads=grads, bf16_noise=noise),
-               GOLDEN / "semantic.pt")
+               "semantic.pt")
 
 
 def golden_semantic_plain(ref):
@@ -169,8 +168,8 @@ def golden_semantic_plain(ref):
     loss.backward()
     grads = {k: p.grad.detach().clone() for k, p in m.named_parameters() if p.grad is not None}
     noise = bf16_noise(m, lambda: w(semantic_token_ids=ids, return_loss=True), grads)
-    torch.save(dict(kwargs=kw, state=st, ids=ids, mask=mask, logits=logits, logits_masked=logits_masked,
-                    loss=loss.detach(), grads=grads, bf16_noise=noise), GOLDEN / "semantic_plain.pt")
+    golden.save(dict(kwargs=kw, state=st, ids=ids, mask=mask, logits=logits, logits_masked=logits_masked,
+                    loss=loss.detach(), grads=grads, bf16_noise=noise), "semantic_plain.pt")
 
 
 def golden_coarse(ref):
@@ -223,10 +222,10 @@ def golden_coarse(ref):
     wmask = torch.nn.functional.pad(sem_l != 50, (1, co_l.shape[1]), value=True)
     (wsl, wcl), _ = ot.coarse_forward(st, sem_l.masked_fill(sem_l == 50, 0), co_l[:, :-1], self_attn_mask=wmask, **hk)
     check("wrapper loss", ot.coarse_wrapper_loss(wsl, wcl, sem_l, co_l), loss.detach())
-    torch.save(dict(kwargs=kw, state=st, sem=sem, coarse=coarse, mask=mask, sem_logits=sl, coarse_logits=cl,
+    golden.save(dict(kwargs=kw, state=st, sem=sem, coarse=coarse, mask=mask, sem_logits=sl, coarse_logits=cl,
                     sem_logits_masked=slm, coarse_logits_masked=clm, kv_a=kv_a, emb_a=emb_a, coarse_logits_b=cl_b,
                     loss=loss.detach(), grads=grads, bf16_noise=noise, logits_bf16_noise=logits_bf16_noise),
-               GOLDEN / "coarse.pt")
+               "coarse.pt")
 
 
 def golden_fine(ref):
@@ -246,8 +245,8 @@ def golden_fine(ref):
     (ocl, ofl), _ = ot.fine_forward(st, coarse, fine, **hk)
     check("coarse logits", ocl, cl)
     check("fine logits", ofl, fl)
-    torch.save(dict(kwargs=kw, state=st, coarse=coarse, fine=fine, coarse_logits=cl, fine_logits=fl),
-               GOLDEN / "fine.pt")
+    golden.save(dict(kwargs=kw, state=st, coarse=coarse, fine=fine, coarse_logits=cl, fine_logits=fl),
+               "fine.pt")
 
 
 def golden_relpos(ref):
@@ -383,7 +382,7 @@ def golden_relpos(ref):
     out["fine"] = dict(kwargs=kw, state=st, coarse=coarse, fine=fine, c_labels=c_labels, f_labels=f_labels,
                        coarse_logits=cl, fine_logits=fl, fine_logits_b=fl_b, loss=loss.detach(), grads=grads,
                        bf16_noise=noise)
-    torch.save(out, GOLDEN / "relpos.pt")
+    golden.save(out, "relpos.pt")
 
 
 fixed_fcm = ot.fixed_fcm
@@ -465,7 +464,7 @@ def golden_wrappers(ref):
                                                                 return_loss=True), gr))
     finally:
         ref.lm.generate_mask_with_prob = saved
-    torch.save(out, GOLDEN / "wrappers.pt")
+    golden.save(out, "wrappers.pt")
 
 
 def golden_sampling(ref):
@@ -482,8 +481,8 @@ def golden_sampling(ref):
     print("  [ok] gumbel ids bit-exact")
     seq = torch.tensor([[3, 7, 64, 5, 64, 1], [1, 2, 3, 4, 5, 6]])
     masked = ref.lm.mask_out_after_eos_id(seq, 64, keep_eos=False)
-    torch.save(dict(logits=logits, filtered=filt, uniform=u, ids=ids, seq=seq, seq_masked=masked),
-               GOLDEN / "sampling.pt")
+    golden.save(dict(logits=logits, filtered=filt, uniform=u, ids=ids, seq=seq, seq_masked=masked),
+               "sampling.pt")
 
 
 def golden_soundstream(ref):
@@ -529,8 +528,8 @@ def golden_soundstream(ref):
             y = c(x)
         check(f"convT s{s}", oc.causal_conv_transpose1d(x, c.conv.weight, c.conv.bias, s), y)
         convs[f"convT{s}"] = dict(x=x, w=c.conv.weight.detach(), b=c.conv.bias.detach(), stride=s, y=y)
-    torch.save(dict(kwargs=kw, state=st, wave=wave, enc=enc, quant=quant, idx=idx, codes=codes, recon=recon,
-                    convs=convs), GOLDEN / "soundstream.pt")
+    golden.save(dict(kwargs=kw, state=st, wave=wave, enc=enc, quant=quant, idx=idx, codes=codes, recon=recon,
+                    convs=convs), "soundstream.pt")
 
 
 def golden_local_attn(ref):
@@ -558,8 +557,8 @@ def golden_local_attn(ref):
           if k.split(".")[0] in ("encoder", "decoder", "rq", "encoder_attn", "decoder_attn")}
     print("local attention bottleneck:")
     check("round trip with decoder_attn (README.md:100-113)", recon_idx, recon, tol=1e-5)
-    torch.save(dict(kwargs=kw, state=st, wave=wave, h=h, enc_attn_out=enc_attn_out, quant=quant, idx=idx, recon=recon),
-               GOLDEN / "local_attn.pt")
+    golden.save(dict(kwargs=kw, state=st, wave=wave, h=h, enc_attn_out=enc_attn_out, quant=quant, idx=idx, recon=recon),
+               "local_attn.pt")
 
 
 def main():
@@ -578,8 +577,8 @@ def main():
             # so each file is reproducible on its own, whatever ran before it
             random.seed(20240607 + sum(map(ord, fn.__name__)))
             fn(ref)
-    total = sum(p.stat().st_size for p in GOLDEN.glob("*.pt"))
-    print(f"wrote {len(list(GOLDEN.glob('*.pt')))} fixtures, {total / 1e6:.2f} MB")
+    files = sorted(GOLDEN.glob("*.pt*"))
+    print(f"wrote {len(files)} fixture files, {sum(p.stat().st_size for p in files) / 1e6:.2f} MB")
 
 
 if __name__ == "__main__":

@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with `-m gpu` on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a) GPU")
 
 
 def pytest_collection_modifyitems(config, items):

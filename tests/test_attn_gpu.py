@@ -1,4 +1,4 @@
-"""tcgen05 MQA attention vs an fp32 restatement of attend.py:98-146 (math path)."""
+"""wgmma MQA attention vs an fp32 restatement of attend.py:98-146 (math path)."""
 import pytest
 import torch
 

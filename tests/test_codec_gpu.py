@@ -1,16 +1,16 @@
-"""B200: SoundStream codec kernels (causal convs, convT, RVQ) vs goldens from the real reference + the oracle."""
-from pathlib import Path
+"""H100: SoundStream codec kernels (causal convs, convT, RVQ) vs goldens from the real reference + the oracle."""
 
 import pytest
 import torch
 
+from oracle import golden
+
 pytestmark = pytest.mark.gpu
-G = Path(__file__).parent / "golden"
 DEV = "cuda"
 
 
 def load(name):
-    return torch.load(G / name, map_location="cpu", weights_only=False)
+    return golden.load(name)
 
 
 def err(a, b):
@@ -91,7 +91,7 @@ def test_rvq_bit_exact_at_config_size(impl):
     x = torch.randn(600, 512) * 3
     q_ref, i_ref = oc.rvq_encode(x, cb)
     margin = oc.rvq_margin(x, cb)
-    if impl == "tensor_cores":   # distance GEMM on tcgen05 + exact fp32 re-rank of the candidates (csrc/rvq_tc.cu)
+    if impl == "tensor_cores":   # distance GEMM on wgmma + exact fp32 re-rank of the candidates (csrc/rvq_tc.cu)
         q, i = ops.rvq_encode_tc(x.to(DEV), ops.rvq_pack_codebooks(cb.to(DEV)))
     else:
         q, i = ops.rvq_encode(x.to(DEV), cb.to(DEV))
@@ -234,8 +234,8 @@ def test_codec_first_conv_tc():
 @pytest.mark.parametrize("C,T", [(32, 5000), (64, 3000), (128, 1500), (256, 700)])
 @pytest.mark.parametrize("d,phases,mode", [(1, 1, "reflect"), (3, 1, "constant"), (9, 4, "reflect"), (9, 5, "reflect")])
 def test_residual_unit_tc_vs_oracle(C, T, d, phases, mode):
-    """alm_codec_ru_tc (tcgen05, A operand of the 1x1 conv in tensor memory) vs soundstream.py:362-369 restated; ragged
-    last tile (T % 128 != 0), reflect / constant halo, phase-split output as fed to the strided convs."""
+    """alm_codec_ru_tc (wgmma, A operand of the 1x1 conv staged in shared memory) vs soundstream.py:362-369 restated; ragged
+    last tile (T not a multiple of the 64-row tile), reflect / constant halo, phase-split output as fed to the strided convs."""
     import torch.nn.functional as F
 
     from audiolm_pytorch_b200 import ops

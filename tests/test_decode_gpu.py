@@ -1,13 +1,13 @@
 """CUDA-graph decode engine (config C5): static-cache kernels vs the tile kernels, one-token stack step vs the
 cached forward, graph replay vs eager."""
-from pathlib import Path
 
 import pytest
 import torch
 
+from oracle import golden
+
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-G = Path(__file__).parent / "golden"
 bf16 = torch.bfloat16
 
 
@@ -52,7 +52,7 @@ def test_kv_append_and_decode_attention(b, h, n, masked):
 def _semantic_model():
     from audiolm_pytorch_b200.audiolm import SemanticTransformer
 
-    g = torch.load(G / "semantic.pt", map_location="cpu", weights_only=False)
+    g = golden.load("semantic.pt")
     m = SemanticTransformer(**g["kwargs"])
     m.load_state_dict(g["state"])
     return m.to(DEV).eval(), g["ids"].to(DEV)
@@ -150,7 +150,7 @@ def test_coarse_and_fine_generate_on_engine_match_slow_path_statistics():
         rq_groups = 1
         num_quantizers = 8
 
-    g = torch.load(G / "coarse.pt", map_location="cpu", weights_only=False)
+    g = golden.load("coarse.pt")
     m = CoarseTransformer(**g["kwargs"])
     m.load_state_dict(g["state"])
     m = m.to(DEV).eval()
@@ -163,7 +163,7 @@ def test_coarse_and_fine_generate_on_engine_match_slow_path_statistics():
     assert fast.shape == slow.shape == (2, 4, 3)
     assert (fast == slow).float().mean().item() > 0.9   # argmax ties / bf16 noise may flip an occasional id
 
-    g = torch.load(G / "fine.pt", map_location="cpu", weights_only=False)
+    g = golden.load("fine.pt")
     f = FineTransformer(**g["kwargs"])
     f.load_state_dict(g["state"])
     f = f.to(DEV).eval()
@@ -200,6 +200,7 @@ def test_fused_stack_step_matches_multi_kernel_step(b, d, heads, depth, n0):
         mask[:, 0] = True
     xs = torch.randn(3, b, d, device=DEV)
     res = []
+    default = decode.FUSED_STACK_STEP
     for fused in (False, True):
         decode.FUSED_STACK_STEP = fused
         try:
@@ -213,7 +214,7 @@ def test_fused_stack_step_matches_multi_kernel_step(b, d, heads, depth, n0):
             assert dec.barrier_timeouts() == 0
             res.append((torch.stack(outs), dec.kc[:, :, n0:n0 + 3].clone(), dec.vc[:, :, n0:n0 + 3].clone()))
         finally:
-            decode.FUSED_STACK_STEP = True
+            decode.FUSED_STACK_STEP = default
     (o0, k0, v0), (o1, k1, v1) = res
     assert torch.isfinite(o1.float()).all()
     assert rms_rel(o1, o0) < 2e-2, rms_rel(o1, o0)

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (alm_gemm_bf16) vs an fp32 torch reference of the same contraction."""
+"""wgmma GEMM (alm_gemm_bf16) vs an fp32 torch reference of the same contraction."""
 import pytest
 import torch
 

@@ -6,12 +6,13 @@ from pathlib import Path
 import pytest
 import torch
 
+from oracle import golden
+
 ROOT = Path(__file__).resolve().parent.parent
-G = ROOT / "tests" / "golden"
 
 
 def load(name):
-    return torch.load(G / name, map_location="cpu", weights_only=False)
+    return golden.load(name)
 
 
 @pytest.mark.parametrize("fixture,cls_name", [("semantic.pt", "SemanticTransformer"), ("coarse.pt", "CoarseTransformer"),
@@ -184,7 +185,8 @@ def test_regroup_rows_layout_of_the_decode_step_operands():
     alm_decode_stack_step documents in include/alm_b200.h (CTA c's rows of a projection become one contiguous block)."""
     from audiolm_pytorch_b200 import ops
 
-    for N, K, grid in [(640, 16, 148), (5472, 8, 148), (7, 8, 4), (148, 8, 148), (149, 8, 148)]:
+    for N, K, grid in [(640, 16, 148), (5472, 8, 148), (7, 8, 4), (148, 8, 148), (149, 8, 148),
+                       (640, 16, 132), (132, 8, 132), (133, 8, 132)]:
         w = torch.arange(N * K, dtype=torch.float32).view(N, K)
         wp = ops.regroup_rows(w, grid)
         pc = -(-N // grid)

@@ -1,13 +1,13 @@
-"""B200: SoundStream's LocalTransformer bottleneck (soundstream.py:397-440) on the attention / GEMM kernels vs the
+"""H100: SoundStream's LocalTransformer bottleneck (soundstream.py:397-440) on the attention / GEMM kernels vs the
 reference run over the restated `local-attention` package (tests/golden/local_attn.pt; PARITY UNPINNED upstream) and vs
 the oracle restatement at the C1 size (dim 512, window 128, 150 frames)."""
-from pathlib import Path
 
 import pytest
 import torch
 
+from oracle import golden
+
 pytestmark = pytest.mark.gpu
-G = Path(__file__).parent / "golden"
 DEV = "cuda"
 
 
@@ -19,7 +19,7 @@ def rms_rel(a, b):
 def test_local_transformer_golden_and_default_soundstream():
     from audiolm_pytorch_b200 import SoundStream
 
-    g = torch.load(G / "local_attn.pt", map_location="cpu", weights_only=False)
+    g = golden.load("local_attn.pt")
     ss = SoundStream(**g["kwargs"])                       # default use_local_attn=True constructs
     ss.load_state_dict(g["state"], strict=True)
     ss = ss.to(DEV).eval()

@@ -1,16 +1,15 @@
-"""B200: the product transformers (CUDA kernels through the C ABI) vs goldens produced by the real reference."""
-from pathlib import Path
-
+"""H100: the product transformers (CUDA kernels through the C ABI) vs goldens produced by the real reference."""
 import pytest
 import torch
 
+from oracle import golden
+
 pytestmark = pytest.mark.gpu
-G = Path(__file__).parent / "golden"
 DEV = "cuda"
 
 
 def load(name):
-    return torch.load(G / name, map_location="cpu", weights_only=False)
+    return golden.load(name)
 
 
 def rel(a, b):

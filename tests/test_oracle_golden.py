@@ -1,18 +1,15 @@
 """CPU: the oracle restatements reproduce the committed goldens (generated from the real reference by
 oracle/make_golden.py).  This is what pins the oracle; GPU tests then compare the CUDA path to it."""
-from pathlib import Path
-
 import pytest
 import torch
 
 from oracle import codec as oc
+from oracle import golden
 from oracle import transformer as ot
-
-G = Path(__file__).parent / "golden"
 
 
 def load(name):
-    return torch.load(G / name, map_location="cpu", weights_only=False)
+    return golden.load(name)
 
 
 def close(a, b, tol=2e-4):

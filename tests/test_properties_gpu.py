@@ -1,4 +1,4 @@
-"""B200, BASELINE.json full sizes: size-independent properties of the CUDA path (no oracle needed)."""
+"""H100, BASELINE.json full sizes: size-independent properties of the CUDA path (no oracle needed)."""
 import pytest
 import torch
 

@@ -1,14 +1,14 @@
 """flash_attn=False path on the GPU (SURVEY §8 a7): attention kernels with an additive bias (+ d bias), the
 bias gather / scatter-add kernels, and the three transformers against the reference goldens and the oracle."""
-from pathlib import Path
 
 import pytest
 import torch
 import torch.nn.functional as F
 
+from oracle import golden
+
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-G = Path(__file__).parent / "golden"
 
 
 def rms_rel(a, b):
@@ -139,7 +139,7 @@ def _check_grads(m, golden, tol=7e-2, noise=None):
 def test_semantic_rel_pos_bias_vs_reference_golden():
     from audiolm_pytorch_b200.audiolm import SemanticTransformer
 
-    g = torch.load(G / "relpos.pt", map_location="cpu", weights_only=False)["semantic"]
+    g = golden.load("relpos.pt")["semantic"]
     m = SemanticTransformer(**g["kwargs"])
     m.load_state_dict(g["state"])
     m = m.to(DEV).eval()
@@ -162,7 +162,7 @@ def test_semantic_rel_pos_bias_vs_reference_golden():
 def test_coarse_rel_pos_bias_vs_reference_golden():
     from audiolm_pytorch_b200.audiolm import CoarseTransformer
 
-    g = torch.load(G / "relpos.pt", map_location="cpu", weights_only=False)["coarse"]
+    g = golden.load("relpos.pt")["coarse"]
     m = CoarseTransformer(**g["kwargs"])
     m.load_state_dict(g["state"])
     m = m.to(DEV).eval()
@@ -203,7 +203,7 @@ def test_coarse_rel_pos_bias_vs_reference_golden():
 def test_fine_rel_pos_bias_vs_reference_golden():
     from audiolm_pytorch_b200.audiolm import FineTransformer
 
-    g = torch.load(G / "relpos.pt", map_location="cpu", weights_only=False)["fine"]
+    g = golden.load("relpos.pt")["fine"]
     m = FineTransformer(**g["kwargs"])
     m.load_state_dict(g["state"])
     m = m.to(DEV).eval()

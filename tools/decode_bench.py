@@ -15,6 +15,7 @@ n0 = int(sys.argv[1]) if len(sys.argv) > 1 else 600
 torch.manual_seed(0)
 tr = Transformer(dim=1024, depth=6, heads=8, flash_attn=True).to(dev).eval()
 res = {}
+default = decode.FUSED_STACK_STEP
 for b in (1, 4):
     for fused in (False, True):
         decode.FUSED_STACK_STEP = fused
@@ -40,6 +41,6 @@ for b in (1, 4):
         res[f"b{b}_{'fused' if fused else 'multi'}_us_per_step"] = round(e0.elapsed_time(e1) * 1e3 / iters, 2)
         res[f"b{b}_{'fused' if fused else 'multi'}_timeouts"] = dec.barrier_timeouts()
         assert torch.isfinite(y.float()).all()
-decode.FUSED_STACK_STEP = True
+decode.FUSED_STACK_STEP = default
 res["cache_len"] = n0
 print(json.dumps(res))

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Exactly N C3 training steps exactly as bench.py times them (CoarseTransformerWrapper.forward with its key mask + FCM
-mask, loss, backward) with no other GPU work - the target of the ncu launch lists under profiles/."""
+mask, loss, backward) with no other GPU work - a clean target for a profiler."""
 import sys
 from pathlib import Path
 

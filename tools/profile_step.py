@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Per-kernel-class / per-GEMM-shape device time of one C3 training step (CUDA events on the launching stream).
-Writes a markdown table to stdout; run on a B200:  python tools/profile_step.py > profiles/rNN_step_breakdown.md"""
+Writes a markdown table to stdout; run on the GPU:  python tools/profile_step.py > step_breakdown.md"""
 import json
 import sys
 from pathlib import Path
@@ -52,7 +52,7 @@ tot = 0.0
 for cls, (ms, work, n) in sorted(prof.items(), key=lambda kv: -kv[1][0]):
     rate = work / (ms * 1e-3) if ms else 0
     tot += ms
-    if ops.CLASS_UNIT.get(cls) == "byte":  # HBM-bound classes: GB/s of algorithmic bytes vs the measured copy peak
+    if ops.CLASS_UNIT.get(cls) == "byte":  # HBM-bound classes: GB/s of algorithmic bytes vs the HBM peak
         print(f"| {cls} | {n} | {ms:.3f} | {rate / 1e9:.0f} GB/s | {100 * rate / 1e9 / pk['hbm']:.0f}% of HBM |")
     else:
         print(f"| {cls} | {n} | {ms:.3f} | {rate / 1e12:.0f} | {100 * rate / 1e12 / pk['tf_sustained']:.0f}% |")
