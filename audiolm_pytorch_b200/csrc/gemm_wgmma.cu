@@ -1,7 +1,9 @@
 // Persistent, warp-specialised bf16 GEMM for sm_90a (H100).
 //   warpgroup 0 : TMA producer (one elected lane of warp 0) — cp.async.bulk.tensor into a STAGES-deep SW128 smem ring
 //   warpgroups 1, 2 : consumers — wgmma m64nBNk16 on rows [0, 64) / [64, 128) of the 128-row tile, fp32 accumulators
-//                     in registers, then the epilogue straight from those registers (alpha / bias / CE -> global)
+//                     in registers, then the epilogue: bf16 outputs that TMA can address go through a swizzled smem
+//                     staging buffer and a TMA tensor store (the warpgroup goes on to the next tile while it drains),
+//                     everything else (fp32 / accumulating / CE / misaligned C) is stored straight from the registers
 // Operands may be K-major or MN-major (wgmma transpose bits), which covers forward (x W^T), dgrad (dy W) and
 // wgrad (dy^T x) without materialising any transpose.
 #include "alm_common.cuh"
@@ -16,6 +18,7 @@ struct GemmParams {
   int M, N, K, batch;
   int m_blocks, n_blocks, k_blocks, split_k;
   int c_fp32, acc_mode;
+  int tma_store;  // bf16 C, acc_mode 0, 16-B aligned base and pitches: epilogue through smem + tmC
   float alpha;
   // fused logit head + cross entropy (CE kernel variant only; alm_gemm_head_ce):
   //   ce_mode 1: nothing is stored; every (row, n tile) emits its soft-max partial {max, sum 2^(t - max)} of
@@ -40,20 +43,26 @@ struct GemmCfg {
   static constexpr int STAGES = BLOCK_N == 256 ? 4 : (BLOCK_N == 128 ? 6 : 8);
   static constexpr int A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
   static constexpr int B_BYTES = BLOCK_N * GEMM_BLOCK_K * 2;
-  static constexpr int SMEM_BYTES = STAGES * (A_BYTES + B_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/;
+  // epilogue staging: 2 consumer warpgroups x 2 buffers x [64 rows][64 bf16] (SW128, one TMA store box each)
+  static constexpr int C_SUB_BYTES = 64 * 64 * 2;
+  static constexpr int C_STAGE_BYTES = 4 * C_SUB_BYTES;
+  static constexpr int SMEM_BYTES =
+      STAGES * (A_BYTES + B_BYTES) + C_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(SMEM_BYTES <= 227 * 1024, "exceeds the sm_90 dynamic shared memory limit");
 };
 
 template <int BLOCK_N, bool A_MN, bool B_MN, bool CE = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                       const GemmParams p) {
+                       const __grid_constant__ CUtensorMap tmC, const GemmParams p) {
   using Cfg = GemmCfg<BLOCK_N>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * Cfg::A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * (Cfg::A_BYTES + Cfg::B_BYTES));
+  uint8_t* stage_c = smem + STAGES * (Cfg::A_BYTES + Cfg::B_BYTES);  // 1024-B aligned (SW128 TMA box)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stage_c + Cfg::C_STAGE_BYTES);
   uint64_t* full_bar = bars;                  // [STAGES]  TMA -> MMA
   uint64_t* empty_bar = bars + STAGES;        // [STAGES]  consumers -> TMA (one arrive per consumer warp)
 
@@ -64,6 +73,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (p.tma_store) tma_prefetch_desc(&tmC);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);
@@ -170,8 +180,49 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     wgmma_fence_acc(acc);
     if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
 
-    // ===================== epilogue from the accumulator fragment =====================
     const int n0 = nb * BLOCK_N;
+    if constexpr (!CE) {
+      if (p.tma_store) {
+        // ============ epilogue through smem: 64-column sub-tiles of this warpgroup's 64 rows, one TMA store each ====
+        // same values and bf16 rounding as the register path; TMA clips rows >= M and columns >= N
+        // (thread 0 of the warpgroup issues and waits for its stores; an even sub-tile count alternates the two
+        // buffers, a single sub-tile (BLOCK_N 64) reuses one)
+        constexpr int SUBS = BLOCK_N / 64, NBUF = SUBS % 2 == 0 ? 2 : 1;
+        // this thread's staging rows: wq * 16 + lane / 4 and + 8, whose (row & 7) = lane / 4 picks the swizzle
+        const uint32_t st_base =
+            smem_u32(stage_c) + cw * 2 * Cfg::C_SUB_BYTES + (wq * 16 + (lane >> 2)) * 128 + (lane & 3) * 4;
+#pragma unroll
+        for (int sub = 0; sub < SUBS; ++sub) {
+          uint8_t* buf = stage_c + (cw * 2 + sub % NBUF) * Cfg::C_SUB_BYTES;
+          if ((threadIdx.x & 127) == 0) bulk_wait_group_read<NBUF - 1>();  // last store from this buffer read it
+          named_bar_sync(1 + cw, 128);
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = sub * 8 + jj;
+              const int col = n0 + 8 * j + c_lane;
+              float v0 = acc[4 * j + 2 * h] * p.alpha, v1 = acc[4 * j + 2 * h + 1] * p.alpha;
+              if (p.bias != nullptr) {
+                if (col < p.N) v0 += __ldg(p.bias + col);
+                if (col + 1 < p.N) v1 += __ldg(p.bias + col + 1);
+              }
+              // 128-B swizzle: 16-B chunk jj of row r sits at chunk jj ^ (r & 7) -> conflict-free 4-B stores
+              st_shared_u32(st_base + (sub % NBUF) * Cfg::C_SUB_BYTES + h * 1024 + ((jj ^ (lane >> 2)) << 4),
+                            pack_bf16x2(v0, v1));
+            }
+          fence_proxy_async_smem();
+          named_bar_sync(1 + cw, 128);
+          if ((threadIdx.x & 127) == 0) {
+            tma_store_3d(&tmC, buf, n0 + sub * 64, mb * GEMM_BLOCK_M + cw * 64, b);
+            bulk_commit_group();
+          }
+        }
+        continue;
+      }
+    }
+
+    // ===================== epilogue from the accumulator fragment =====================
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int gm = mb * GEMM_BLOCK_M + r_base + 8 * h;
@@ -272,10 +323,12 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       }
     }
   }
+  if ((threadIdx.x & 127) == 0) bulk_wait_group<0>();  // the CTA's smem must outlive its pending TMA stores
 }
 
 template <int BLOCK_N, bool A_MN, bool B_MN, bool CE = false>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const GemmParams& p,
+                       cudaStream_t stream) {
   using Cfg = GemmCfg<BLOCK_N>;
   auto kfn = gemm_bf16_wgmma_kernel<BLOCK_N, A_MN, B_MN, CE>;
   static bool attr_set = false;
@@ -285,7 +338,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
   }
   const int total = p.m_blocks * p.n_blocks * p.split_k * p.batch;
   const int grid = total < num_sms() ? total : num_sms();
-  kfn<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
+  kfn<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, tmC, p);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);
   return ALM_OK;
@@ -390,15 +443,28 @@ static int gemm_common(const void* A, int a_mn, int64_t lda, int64_t strideA, co
     if (rc != ALM_OK) return rc;
   }
 
+  // bf16 stores through TMA where a tensor map can describe C (16-B aligned base and pitches); the rest keeps the
+  // register epilogue (fp32 C, read-modify-write accumulation, the CE variant, e.g. a pitch of 10,920 B)
+  CUtensorMap tmC = {};
+  p.tma_store = ce == nullptr && !c_fp32 && acc_mode == 0 && (reinterpret_cast<uintptr_t>(C) & 15u) == 0 &&
+                (ldc * 2) % 16 == 0 && (batch == 1 || (strideC * 2) % 16 == 0);
+  if (p.tma_store) {
+    const uint64_t dims[3] = {(uint64_t)N, (uint64_t)M, (uint64_t)batch};
+    const uint64_t strides[3] = {2, (uint64_t)ldc * 2, batch > 1 ? (uint64_t)strideC * 2 : (uint64_t)M * ldc * 2};
+    const uint32_t box[3] = {64, 64, 1};
+    int rc = make_tensor_map(&tmC, C, 2, 3, dims, strides, box, true);
+    if (rc != ALM_OK) return rc;
+  }
+
   if (ce != nullptr) {   // (row-major x, row-major head weight: the only layout the fused head needs)
-    if (BN == 256) return launch_gemm<256, false, false, true>(tmA, tmB, p, stream);
-    if (BN == 128) return launch_gemm<128, false, false, true>(tmA, tmB, p, stream);
-    return launch_gemm<64, false, false, true>(tmA, tmB, p, stream);
+    if (BN == 256) return launch_gemm<256, false, false, true>(tmA, tmB, tmC, p, stream);
+    if (BN == 128) return launch_gemm<128, false, false, true>(tmA, tmB, tmC, p, stream);
+    return launch_gemm<64, false, false, true>(tmA, tmB, tmC, p, stream);
   }
 #define ALM_GEMM_DISPATCH(BN_)                                                             \
-  if (!a_mn && !b_mn) return launch_gemm<BN_, false, false>(tmA, tmB, p, stream);     \
-  if (!a_mn && b_mn) return launch_gemm<BN_, false, true>(tmA, tmB, p, stream);       \
-  return launch_gemm<BN_, true, true>(tmA, tmB, p, stream);
+  if (!a_mn && !b_mn) return launch_gemm<BN_, false, false>(tmA, tmB, tmC, p, stream);     \
+  if (!a_mn && b_mn) return launch_gemm<BN_, false, true>(tmA, tmB, tmC, p, stream);       \
+  return launch_gemm<BN_, true, true>(tmA, tmB, tmC, p, stream);
   if (BN == 256) { ALM_GEMM_DISPATCH(256) }
   if (BN == 128) { ALM_GEMM_DISPATCH(128) }
   { ALM_GEMM_DISPATCH(64) }

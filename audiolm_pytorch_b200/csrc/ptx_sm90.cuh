@@ -100,6 +100,31 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// tensor store shared -> global (elements outside the tensor map's dims are not written); completion is tracked per
+// thread in bulk groups: commit after issuing, wait_read before the smem source is rewritten
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* smem_src, int32_t c0, int32_t c1,
+                                             int32_t c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's committed bulk groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t smem_addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(smem_addr), "r"(v) : "memory");
+}
+// barrier over `nthreads` threads (a multiple of 32) on hardware barrier `id` (0 is __syncthreads')
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
 // ---------------------------------------------------------------------------------------------
 // wgmma (warpgroup MMA): bf16 x bf16 -> fp32 accumulators in registers, issued by all 128 threads of a warpgroup
 // ---------------------------------------------------------------------------------------------

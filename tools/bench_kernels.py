@@ -1,6 +1,7 @@
 #!/usr/bin/env python
-"""Stand-alone timings of the HBM-bound row kernels at C3 sizes (CUDA events, L2 flushed between iterations).
-usage: python tools/bench_kernels.py [geglu] [hc] [attn] ..."""
+"""Stand-alone timings of the HBM-bound row kernels, attention and every wgmma GEMM shape at C3 sizes (CUDA events,
+L2 flushed between iterations).
+usage: python tools/bench_kernels.py [geglu] [hc] [attn] [gemm] ..."""
 import sys
 from pathlib import Path
 
@@ -79,3 +80,29 @@ if "attn" in which:
     o, lse = ops.mqa_attn_fwd(q, k, v, heads=8)
     do = rnd(16, 2048, 512)
     timeit("attn bwd (delta + dkv + dq)", lambda: ops.mqa_attn_bwd(q, k, v, o, do, lse, heads=8), flops=2.5 * fl)
+
+if "gemm" in which:
+    from audiolm_pytorch_b200.transformer import best_split_k
+
+    # every distinct wgmma GEMM shape of one C3 layer (inner 2730, padded 2736): (name, M, N, K)
+    fwd = [("fwd to_q", M, 512, d), ("fwd to_kv", M, 128, d), ("fwd to_out", M, d, 512), ("fwd w1", M, 5472, d),
+           ("fwd w2", M, d, 2736)]
+    dgrad = [("dgrad w2", M, 2736, d), ("dgrad w1", M, d, 5472), ("dgrad to_out", M, 512, d), ("dgrad to_q", M, d, 512),
+             ("dgrad to_kv", M, d, 128)]
+    wgrads = [("wgrad w2", d, 2730, M), ("wgrad w1 (half)", 2730, d, M), ("wgrad to_out", d, 512, M),
+              ("wgrad to_q", 512, d, M), ("wgrad to_kv", 128, d, M)]
+    for name, m, n, k in fwd:
+        a, b = rnd(m, k), rnd(n, k)
+        timeit(f"gemm {name} M{m} N{n} K{k}", lambda a=a, b=b: ops.gemm(a, b), flops=2.0 * m * n * k)
+    for name, m, n, k in dgrad:
+        a, b = rnd(m, k), rnd(k, n)  # b: the layer's weight read MN-major
+        timeit(f"gemm {name} M{m} N{n} K{k}", lambda a=a, b=b: ops.gemm(a, b, b_mn=True), flops=2.0 * m * n * k)
+    for name, m, n, k in wgrads:
+        s = best_split_k(m, n, k)
+        # 2730-wide operands are column slices of wider tensors in the step, which keeps their rows 16-B aligned
+        a, b = rnd(k, -(-m // 8) * 8)[:, :m], rnd(k, -(-n // 8) * 8)[:, :n]
+        out = torch.zeros(m, n, dtype=f32, device=dev)
+        timeit(f"gemm {name} M{m} N{n} K{k} s{s}",
+               lambda a=a, b=b, out=out, s=s: ops.gemm(a, b, a_mn=True, b_mn=True, out=out,
+                                                        acc_mode=2 if s > 1 else 1, split_k=s),
+               flops=2.0 * m * n * k)
