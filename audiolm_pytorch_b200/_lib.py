@@ -23,11 +23,11 @@ F = C.c_float
 SIGNATURES: dict[str, list] = {
     "alm_gemm_bf16": [P, I, L, L, P, I, L, L, P, I, L, L, I, I, I, I, F, P, I, I, P],
     "alm_mqa_attn_fwd": [P, L, P, L, L, P, L, L, P, P, L, P, L, P, L, L, I, I, I, I, I, F, P],
-    "alm_mqa_attn_bwd": [P, L, P, L, L, P, L, L, P, L, P, P, P, I, P, L, P, L, P, L, P, P, L, L, I, I, I, I, I, F, P],
+    "alm_mqa_attn_bwd": [P, L, P, L, L, P, L, L, P, L, P, P, P, I, P, L, P, P, L, P, L, P, P, L, L, I, I, I, I, I, F, P],
     "alm_pack_key_mask": [P, P, I, I, P],
     "alm_embed_gather": [P, I, P, P, I, I, P],
     "alm_embed_scatter": [P, I, P, P, I, I, P],
-    "alm_attn_delta": [P, L, P, L, P, L, I, I, I, P],
+    "alm_attn_delta": [P, L, P, L, P, L, P, I, I, I, P],
     "alm_kv_append": [P, L, P, P, L, P, I, I, P],
     "alm_gemv_bf16": [P, L, P, L, P, I, L, P, I, I, I, P],
     "alm_gemm_head_ce": [P, L, P, L, P, P, L, I, P, P, P, P, P, P, L, I, I, I, P],

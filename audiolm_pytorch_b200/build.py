@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import hashlib
 import os
+import re
 import shutil
 import subprocess
 import sys
@@ -43,6 +44,16 @@ def _digest(path: Path, headers: list[Path]) -> str:
     return h.hexdigest()[:16]
 
 
+def _wgmma_serialised(ptxas_log: str) -> list[str]:
+    """Kernels for which ptxas reports C7510 (wgmma.mma_async serialised by a call in the wgmma pipeline)."""
+    found = []
+    for line in ptxas_log.splitlines():
+        if "C7510" in line:
+            m = re.search(r"in the function '([^']+)'", line)
+            found.append(m.group(1) if m else line.strip())
+    return found
+
+
 def sources() -> list[Path]:
     return sorted(CSRC.glob("*.cu"))
 
@@ -66,9 +77,16 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         src, obj = job
         cmd = [nvcc, *NVCC_FLAGS, "-c", str(src), "-o", str(obj)]
         r = subprocess.run(cmd, capture_output=True, text=True)
-        (OBJ_DIR / f"{src.stem}.ptxas.log").write_text(r.stderr)
+        log = OBJ_DIR / f"{src.stem}.ptxas.log"
+        log.write_text(r.stderr)
         if r.returncode != 0:
             raise RuntimeError(f"nvcc failed for {src.name}:\n{r.stdout}\n{r.stderr}")
+        serialised = _wgmma_serialised(r.stderr)
+        if serialised:
+            obj.unlink()
+            raise RuntimeError(
+                f"{src.name}: ptxas serialises wgmma (C7510) in {', '.join(serialised)}; a function call (printf, a "
+                f"non-inlined helper) inside a wgmma kernel costs every mma_async a wait. See {log}.")
         if verbose:
             print(f"[build] {src.name} ok", file=sys.stderr)
         return obj

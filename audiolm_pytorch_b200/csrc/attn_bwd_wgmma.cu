@@ -1,18 +1,23 @@
-// Multi-query causal attention backward for sm_90a (autograd of attend.py:69-146), two kernels:
+// Multi-query causal attention backward for sm_90a (autograd of attend.py:69-146), one kernel.
 //
-//  dKV kernel: one CTA = (batch, 128 keys).  It walks every (head, query block) that can see these keys
-//      S^T = K Q^T,  dP^T = V dO^T                       (wgmma, both operands in smem)
-//      P^T = exp(S^T*scale - lse),  dS^T = scale * P^T (dP^T - delta)   (on the accumulator fragments)
-//      dV += P^T dO,  dK += dS^T Q                       (wgmma with P^T / dS^T as register A operands; accumulated
-//                                                          in registers over all heads: MQA shares k/v, so no atomics)
-//  dQ kernel: one CTA = (batch, head, 128 queries), walks the key tiles:
-//      S = Q K^T, dP = dO V^T, dS = scale * P (dP - delta), dQ += dS K.
+// One CTA = (batch, 128 keys).  It walks every (head, query block) that can see these keys and computes, once each,
+//     S^T = K Q^T,  dP^T = V dO^T                                      (wgmma, both operands in smem)
+//     P^T = exp(S^T*scale - lse),  dS^T = scale * P^T (dP^T - delta)   (on the accumulator fragments)
+//     dV += P^T dO   (P^T as register A operand)
+//     dK += dS^T Q,  dQ_partial = dS K   (dS^T stored as bf16 in smem, read K-major for dK and MN-major for dQ)
+// dV / dK accumulate in registers over all heads (MQA shares k/v: no atomics).  The partial dQ of each tile is
+// reduced into an fp32 workspace [b, n_q, h*64] with red.global.add; the host zeroes it beforehand (alm_attn_delta)
+// and converts it to bf16 dq afterwards.
 //
 // Q/K/V/dO tiles arrive by TMA (SWIZZLE_128B); the SAME smem tile serves as a K-major operand
 // (contraction over the 64-wide head dim) and as an MN-major operand (contraction over its 128 rows).
-// Warps 0-3 / 4-7 are the two consumer warpgroups (tile rows [0, 64) / [64, 128)).  There is no producer warp: a
-// separate one would cap every thread at 168 registers, and the dQ / dK / dV products need more.  Warp 0 refills a
-// pipeline slot as soon as both warpgroups have released it; STAGES - 1 loads stay in flight.
+// Warps 0-3 / 4-7 are the two consumer warpgroups (key rows [0, 64) / [64, 128) and dQ query rows [0, 64) /
+// [64, 128)); each thread needs ~250 registers.  A separate producer warpgroup with a setmaxnreg hand-off does not
+// help: ptxas allocates for the 384-thread launch bound (168 registers) and spills ~850 B.  Warp 0 issues the loads
+// instead.  Inside a warpgroup S^T and dP^T are separate commit groups, so the exponentials overlap dP^T and dV
+// overlaps the dS arithmetic.  The two warpgroups meet once per iteration, on a named barrier, when both halves of
+// dS^T are in shared memory; dS^T is double-buffered so that barrier also orders its reuse.  Past that barrier both
+// have released the previous iteration's slot, so warp 0 refills it without waiting: STAGES - 1 loads stay ahead.
 #include "alm_common.cuh"
 #include "ptx_sm90.cuh"
 
@@ -33,10 +38,10 @@ struct AttnBwdParams {
   const float* bias;     // [h, n_q, bias_rs] additive score bias (as given to the forward) or null
   float* dbias;          // same layout, fp32: d(bias) is ACCUMULATED (red.add) over batches / calls; or null
   long long bias_hs, bias_rs;
-  __nv_bfloat16* dq;     // [b, n_q, h*64], row stride lddq
+  float* dq_acc;         // [b, n_q, h*64] fp32, zeroed; partial dQ products are reduced into it
   __nv_bfloat16* dk;     // [b, n_k, 64], row stride lddk
   __nv_bfloat16* dv;
-  long long lddq, lddk, lddv;
+  long long lddk, lddv;
   int b, h, n_q, n_k, n_q_pad;
   int causal;
   float scale, scale_log2;
@@ -72,23 +77,26 @@ __device__ __forceinline__ void store_d64(const float (&acc)[32], __nv_bfloat16*
 }
 
 // ================================================================================================
-// dK / dV
+// fused dK / dV / dQ
 // ================================================================================================
-constexpr int DKV_SMEM = AB_TILE * (2 + 2 * AB_STAGES) + AB_STAGES * 2 * 512 + 256;
+constexpr int AB_DS_TILE = AB_T * AB_T * 2;   // dS^T tile [128 keys][128 queries] bf16 = 32 KB
+constexpr int AB_SMEM = AB_TILE * (2 + 2 * AB_STAGES) + 2 * AB_DS_TILE + AB_STAGES * 2 * 512 + 256;
+constexpr uint32_t AB_DS_BAR = 1;             // named barrier of the two consumer warpgroups (0 is __syncthreads)
 
 template <bool HAS_BIAS>
 __global__ void __launch_bounds__(AB_THREADS, 1)
-mqa_attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                        const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
-                        const AttnBwdParams p) {
+mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
+                    const AttnBwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* sK = smem;
   uint8_t* sV = sK + AB_TILE;
   uint8_t* sQ = sV + AB_TILE;                    // [stages]
   uint8_t* sdO = sQ + AB_STAGES * AB_TILE;       // [stages]
-  float* sLse = reinterpret_cast<float*>(sdO + AB_STAGES * AB_TILE);  // [stages][128]
-  float* sDelta = sLse + AB_STAGES * AB_T;                            // [stages][128]
+  uint8_t* sDS = sdO + AB_STAGES * AB_TILE;      // [2] dS^T, double-buffered across iterations
+  float* sLse = reinterpret_cast<float*>(sDS + 2 * AB_DS_TILE);  // [stages][128]
+  float* sDelta = sLse + AB_STAGES * AB_T;                       // [stages][128]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sDelta + AB_STAGES * AB_T);
   uint64_t* kv_full = bars;
   uint64_t* qdo_full = bars + 1;              // [stages]
@@ -137,9 +145,11 @@ mqa_attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
     for (int it = 0; it < min(n_iter, AB_STAGES); ++it) issue_qdo(it);
   }
 
-  // consumers: warpgroup cw owns key rows [64 cw, 64 cw + 64); fragment rows r_base + 8 h, columns 8 g + c_lane + c
+  // consumers: warpgroup cw owns key rows [64 cw, 64 cw + 64) of S^T / dP^T / dK / dV and query rows
+  // [64 cw, 64 cw + 64) of dQ; fragment rows r_base + 8 h, columns 8 g + c_lane + c
   const int cw = warp >> 2;
-  const int r_base = cw * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int wl = warp & 3;
+  const int r_base = cw * 64 + wl * 16 + (lane >> 2);
   const int c_lane = 2 * (lane & 3);
   int kj[2];
   bool key_ok[2];
@@ -153,80 +163,134 @@ mqa_attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
   float dv[32], dk[32];
 #pragma unroll
   for (int e = 0; e < 32; ++e) { dv[e] = 0.f; dk[e] = 0.f; }
-  const uint32_t k_addr = smem_u32(sK) + cw * 8192, v_addr = smem_u32(sV) + cw * 8192;
+  const uint32_t k_all = smem_u32(sK);
+  const uint32_t k_addr = k_all + cw * 8192, v_addr = smem_u32(sV) + cw * 8192;
+  const long long dq_ld = (long long)p.h * AB_D;
   if (n_iter > 0) mbar_wait(kv_full, 0);
   int stage = 0;
   uint32_t phase = 0;
   for (int it = 0; it < n_iter; ++it) {
-    const int qb = qb_min + it % q_per_head;
-    const int q0 = qb * AB_T;
-    [[maybe_unused]] const long long bias_head = HAS_BIAS ? (long long)(it / q_per_head) * p.bias_hs : 0;
+    const int head = it / q_per_head;
+    const int q0 = (qb_min + it % q_per_head) * AB_T;
+    [[maybe_unused]] const long long bias_head = HAS_BIAS ? (long long)head * p.bias_hs : 0;
     mbar_wait(&qdo_full[stage], phase);
     const uint32_t q_addr = smem_u32(sQ + stage * AB_TILE), do_addr = smem_u32(sdO + stage * AB_TILE);
+    const uint32_t ds_addr = smem_u32(sDS + (it & 1) * AB_DS_TILE);
+    // S^T = K Q^T and dP^T = V dO^T as two commit groups: the exponentials run while dP^T is computed
     float st[64], dpt[64];
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < AB_D / 16; ++k)
       wgmma_ss<AB_T>(st, wgmma_desc_sw128(k_addr + k * 32, 1024, 16), wgmma_desc_sw128(q_addr + k * 32, 1024, 16),
                      k > 0 ? 1u : 0u);
+    wgmma_commit();
 #pragma unroll
     for (int k = 0; k < AB_D / 16; ++k)
       wgmma_ss<AB_T>(dpt, wgmma_desc_sw128(v_addr + k * 32, 1024, 16), wgmma_desc_sw128(do_addr + k * 32, 1024, 16),
                      k > 0 ? 1u : 0u);
     wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_acc(st);
-    wgmma_fence_acc(dpt);
     const float* lse_s = sLse + stage * AB_T;
     const float* del_s = sDelta + stage * AB_T;
     // whole tile below the causal diagonal and inside n_q: only the per-row key flag matters
     const bool tile_full = (q0 + AB_T <= p.n_q) && (!p.causal || k0 + AB_T - 1 <= q0 + off);
+    auto visible = [&](int h, int qi) {
+      return key_ok[h] && (tile_full || (qi < p.n_q && (!p.causal || kj[h] <= qi + off)));
+    };
+    auto bias_index = [&](int h, int qi) {
+      return bias_head + (long long)min(qi, p.n_q - 1) * p.bias_rs + min(kj[h], p.n_k - 1);
+    };
+    wgmma_wait<1>();
+    wgmma_fence_acc(st);
+    // P^T = exp(S^T * scale - lse), kept in fp32 for dS
 #pragma unroll
     for (int g = 0; g < AB_T / 8; ++g)
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
         const int col = 8 * g + c_lane + c;
         const int qi = q0 + col;
-        const float lv = lse_s[col], dl = del_s[col];
+        const float lv = lse_s[col];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int e = 4 * g + 2 * h + c;
-          const bool ok = key_ok[h] && (tile_full || (qi < p.n_q && (!p.causal || kj[h] <= qi + off)));
           float shift = -lv;
-          [[maybe_unused]] long long bidx = 0;
-          if constexpr (HAS_BIAS) {
-            bidx = bias_head + (long long)min(qi, p.n_q - 1) * p.bias_rs + min(kj[h], p.n_k - 1);
-            shift = fmaf(__ldg(p.bias + bidx), LOG2E, shift);
-          }
-          const float pe = ok ? ex2_approx(fmaf(st[e], p.scale_log2, shift)) : 0.f;
-          const float ds = ok ? pe * (dpt[e] - dl) : 0.f;
-          if constexpr (HAS_BIAS) {
-            if (ok && p.dbias != nullptr) atomicAdd(p.dbias + bidx, ds);
-          }
-          st[e] = pe;
-          dpt[e] = ds * p.scale;
+          if constexpr (HAS_BIAS) shift = fmaf(__ldg(p.bias + bias_index(h, qi)), LOG2E, shift);
+          st[e] = visible(h, qi) ? ex2_approx(fmaf(st[e], p.scale_log2, shift)) : 0.f;
         }
       }
-    uint32_t pa[8][4], da[8][4];
+    // dV += P^T dO runs under the dS arithmetic
+    uint32_t pa[8][4];
     pack_a_frags(st, pa);
-    pack_a_frags(dpt, da);
     wgmma_fence_acc(dv);
-    wgmma_fence_acc(dk);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < AB_T / 16; ++kk)
       wgmma_rs<AB_D, 1>(dv, pa[kk], wgmma_desc_sw128(do_addr + kk * 2048, 1024, 8192), 1u);
+    wgmma_commit();
+    wgmma_wait<1>();
+    wgmma_fence_acc(dpt);
+    // dS^T = scale * P^T (dP^T - delta), stored as bf16 into the 128-B-swizzled dS^T tile: two 16-KB halves of
+    // [128 keys][64 queries]; one half is the K-major A operand of dK (contraction over queries) and, read MN-major,
+    // the A operand of dQ (contraction over keys)
+#pragma unroll
+    for (int g = 0; g < AB_T / 8; ++g) {
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const int col = 8 * g + c_lane + c;
+        const int qi = q0 + col;
+        const float dl = del_s[col];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int e = 4 * g + 2 * h + c;
+          const bool ok = visible(h, qi);
+          const float ds = ok ? st[e] * (dpt[e] - dl) : 0.f;
+          if constexpr (HAS_BIAS) {
+            if (ok && p.dbias != nullptr) atomicAdd(p.dbias + bias_index(h, qi), ds);
+          }
+          dpt[e] = ds * p.scale;
+        }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = r_base + 8 * h;
+        const uint32_t a = ds_addr + (g >> 3) * (AB_DS_TILE / 2) + row * 128 + (((g & 7) ^ (row & 7)) << 4) + 2 * c_lane;
+        st_shared_u32(a, pack_bf16x2(dpt[4 * g + 2 * h], dpt[4 * g + 2 * h + 1]));
+      }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(AB_DS_BAR, 2 * 128);  // both halves of dS^T written before either warpgroup reads them for dQ
+    // both warpgroups are past iteration it - 1 and have released its slot, so this wait does not block: refill it
+    if (warp == 0 && it >= 1 && it - 1 + AB_STAGES < n_iter) {
+      const int prev = stage == 0 ? AB_STAGES - 1 : stage - 1;
+      mbar_wait(&qdo_empty[prev], stage == 0 ? phase ^ 1u : phase);
+      issue_qdo(it - 1 + AB_STAGES);
+    }
+    // dK += dS^T Q (own 64 keys x all queries) and dQ = dS K (own 64 queries x all keys), both from shared memory
+    float dq[32];
+    wgmma_fence_acc(dk);
+    wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < AB_T / 16; ++kk)
-      wgmma_rs<AB_D, 1>(dk, da[kk], wgmma_desc_sw128(q_addr + kk * 2048, 1024, 8192), 1u);
+      wgmma_ss<AB_D, 0, 1>(dk, wgmma_desc_sw128(ds_addr + (kk >> 2) * (AB_DS_TILE / 2) + cw * 8192 + (kk & 3) * 32, 1024, 16),
+                           wgmma_desc_sw128(q_addr + kk * 2048, 1024, 8192), 1u);
+#pragma unroll
+    for (int kk = 0; kk < AB_T / 16; ++kk)
+      wgmma_ss<AB_D, 1, 1>(dq, wgmma_desc_sw128(ds_addr + cw * (AB_DS_TILE / 2) + kk * 2048, 1024, 8192),
+                           wgmma_desc_sw128(k_all + kk * 2048, 1024, 8192), kk > 0 ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_acc(dv);
     wgmma_fence_acc(dk);
+    wgmma_fence_acc(dq);
     if (lane == 0) mbar_arrive(&qdo_empty[stage]);
-    if (warp == 0 && it + AB_STAGES < n_iter) {  // refill this slot once both warpgroups are done with it
-      mbar_wait(&qdo_empty[stage], phase);
-      issue_qdo(it + AB_STAGES);
+    // partial dQ -> fp32 workspace (fire-and-forget reductions in L2)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int qi = q0 + cw * 64 + wl * 16 + (lane >> 2) + 8 * h;
+      if (qi < p.n_q) {
+        float* row = p.dq_acc + ((size_t)batch * p.n_q + qi) * dq_ld + head * AB_D + c_lane;
+#pragma unroll
+        for (int g = 0; g < AB_D / 8; ++g) red_add_f32x2(row + 8 * g, dq[4 * g + 2 * h], dq[4 * g + 2 * h + 1]);
+      }
     }
     if (++stage == AB_STAGES) { stage = 0; phase ^= 1u; }
   }
@@ -243,157 +307,15 @@ mqa_attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
   store_d64(dk, rk[0], rk[1], c_lane);
 }
 
-// ================================================================================================
-// dQ
-// ================================================================================================
-constexpr int DQ_STAGES = 4;
-constexpr int DQ_SMEM = AB_TILE * (2 + 2 * DQ_STAGES) + 256;
-
-template <bool HAS_BIAS>
-__global__ void __launch_bounds__(AB_THREADS, 1)
-mqa_attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                       const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
-                       const AttnBwdParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  if ((smem_u32(smem) & 1023u) != 0) __trap();
-  uint8_t* sQ = smem;
-  uint8_t* sdO = sQ + AB_TILE;
-  uint8_t* sK = sdO + AB_TILE;                 // [stages]
-  uint8_t* sV = sK + DQ_STAGES * AB_TILE;      // [stages]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + DQ_STAGES * AB_TILE);
-  uint64_t* q_full = bars;
-  uint64_t* kv_full = bars + 1;
-  uint64_t* kv_empty = kv_full + DQ_STAGES;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_qblocks = (p.n_q + AB_T - 1) / AB_T;
-  const int qb = n_qblocks - 1 - (int)blockIdx.x;
-  const int head = blockIdx.y, batch = blockIdx.z;
-  const int q0 = qb * AB_T;
-  const int off = p.n_k - p.n_q;
-  int kv_end = p.n_k;
-  if (p.causal) kv_end = min(p.n_k, q0 + AB_T + off);
-  const int n_tiles = kv_end > 0 ? (kv_end + AB_T - 1) / AB_T : 0;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmdO);
-    mbar_init(q_full, 1);
-    for (int i = 0; i < DQ_STAGES; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 8); }
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  // TMA issue (warp 0, one elected lane): Q / dO once, then the K / V tile j into slot j % STAGES
-  auto issue_kv = [&](int j) {
-    const int st = j % DQ_STAGES;
-    if (elect_one_sync()) {
-      mbar_arrive_expect_tx(&kv_full[st], 2 * AB_TILE);
-      tma_load_3d(sK + st * AB_TILE, &tmK, &kv_full[st], 0, j * AB_T, batch);
-      tma_load_3d(sV + st * AB_TILE, &tmV, &kv_full[st], 0, j * AB_T, batch);
-    }
-    __syncwarp();
-  };
-  if (warp == 0 && n_tiles > 0) {
-    if (elect_one_sync()) {
-      mbar_arrive_expect_tx(q_full, 2 * AB_TILE);
-      tma_load_3d(sQ, &tmQ, q_full, head * AB_D, q0, batch);
-      tma_load_3d(sdO, &tmdO, q_full, head * AB_D, q0, batch);
-    }
-    __syncwarp();
-    for (int j = 0; j < min(n_tiles, DQ_STAGES); ++j) issue_kv(j);
-  }
-
-  // consumers: warpgroup cw owns query rows [64 cw, 64 cw + 64)
-  const int cw = warp >> 2;
-  const int r_base = cw * 64 + (warp & 3) * 16 + (lane >> 2);
-  const int c_lane = 2 * (lane & 3);
-  int qi[2], q_limit[2];
-  float lse[2], delta[2];
-  [[maybe_unused]] const float* brow[2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    qi[h] = q0 + r_base + 8 * h;
-    const size_t roff = ((size_t)batch * p.h + head) * p.n_q_pad + qi[h];
-    lse[h] = p.lse[roff];          // log2-domain; n_q_pad >= n_qblocks*128: always in bounds
-    delta[h] = p.delta[roff];
-    q_limit[h] = p.causal ? qi[h] + off : p.n_k - 1;
-    if constexpr (HAS_BIAS) brow[h] = p.bias + (long long)head * p.bias_hs + (long long)min(qi[h], p.n_q - 1) * p.bias_rs;
-  }
-  const uint32_t* mrow = p.kmask ? p.kmask + (size_t)batch * p.kb_stride : nullptr;
-  const uint32_t q_addr = smem_u32(sQ) + cw * 8192, do_addr = smem_u32(sdO) + cw * 8192;
-  float dq[32];
-#pragma unroll
-  for (int e = 0; e < 32; ++e) dq[e] = 0.f;
-  if (n_tiles > 0) mbar_wait(q_full, 0);
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int j = 0; j < n_tiles; ++j) {
-    mbar_wait(&kv_full[stage], phase);
-    const uint32_t k_addr = smem_u32(sK + stage * AB_TILE), v_addr = smem_u32(sV + stage * AB_TILE);
-    float sc[64], dp[64];
-    wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < AB_D / 16; ++k)
-      wgmma_ss<AB_T>(sc, wgmma_desc_sw128(q_addr + k * 32, 1024, 16), wgmma_desc_sw128(k_addr + k * 32, 1024, 16),
-                     k > 0 ? 1u : 0u);
-#pragma unroll
-    for (int k = 0; k < AB_D / 16; ++k)
-      wgmma_ss<AB_T>(dp, wgmma_desc_sw128(do_addr + k * 32, 1024, 16), wgmma_desc_sw128(v_addr + k * 32, 1024, 16),
-                     k > 0 ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_acc(sc);
-    wgmma_fence_acc(dp);
-    const int kbase = j * AB_T;
-    const bool tile_full = mrow == nullptr && (q0 + AB_T <= p.n_q) && (kbase + AB_T <= p.n_k) &&
-                           (!p.causal || kbase + AB_T - 1 <= q0 + off);
-    uint32_t mbits[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
-    if (mrow != nullptr) {
-      const uint4 mv = __ldg(reinterpret_cast<const uint4*>(mrow + j * 4));
-      mbits[0] = mv.x; mbits[1] = mv.y; mbits[2] = mv.z; mbits[3] = mv.w;
-    }
-#pragma unroll
-    for (int g = 0; g < AB_T / 8; ++g)
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        const int col = 8 * g + c_lane + c;
-        const int kj = kbase + col;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int e = 4 * g + 2 * h + c;
-          bool ok = tile_full;
-          if (!tile_full) ok = qi[h] < p.n_q && kj < p.n_k && kj <= q_limit[h] && ((mbits[col >> 5] >> (col & 31)) & 1u);
-          float shift = -lse[h];
-          if constexpr (HAS_BIAS) {
-            // bias_rs is a multiple of 4 and >= n_k: columns past the padded row read 0
-            if (kj < p.bias_rs) shift = fmaf(__ldg(brow[h] + kj), LOG2E, shift);
-          }
-          const float pe = ok ? ex2_approx(fmaf(sc[e], p.scale_log2, shift)) : 0.f;
-          sc[e] = ok ? pe * (dp[e] - delta[h]) * p.scale : 0.f;
-        }
-      }
-    uint32_t da[8][4];
-    pack_a_frags(sc, da);
-    wgmma_fence_acc(dq);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < AB_T / 16; ++kk)
-      wgmma_rs<AB_D, 1>(dq, da[kk], wgmma_desc_sw128(k_addr + kk * 2048, 1024, 8192), 1u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_acc(dq);
-    if (lane == 0) mbar_arrive(&kv_empty[stage]);
-    if (warp == 0 && j + DQ_STAGES < n_tiles) {  // refill this slot once both warpgroups are done with it
-      mbar_wait(&kv_empty[stage], phase);
-      issue_kv(j + DQ_STAGES);
-    }
-    if (++stage == DQ_STAGES) { stage = 0; phase ^= 1u; }
-  }
-  __nv_bfloat16* rq[2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-    rq[h] = qi[h] < p.n_q ? p.dq + ((size_t)batch * p.n_q + qi[h]) * p.lddq + head * AB_D : nullptr;
-  store_d64(dq, rq[0], rq[1], c_lane);
+// dq [b, n_q, h*64] bf16 (row stride lddq) <- the fp32 workspace [b, n_q, h*64] (contiguous); 4 columns per thread
+__global__ void attn_dq_convert_kernel(const float4* __restrict__ acc, __nv_bfloat16* __restrict__ dq, long long lddq,
+                                       long long rows, int cols4) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= rows * cols4) return;
+  const long long r = i / cols4;
+  const int c = (int)(i - r * cols4);
+  const float4 v = acc[i];
+  *reinterpret_cast<uint2*>(dq + r * lddq + 4 * c) = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
 }
 
 }  // namespace alm
@@ -401,12 +323,12 @@ mqa_attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
 extern "C" int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int64_t k_bstride,
                                 const void* v, int64_t ldv, int64_t v_bstride, const void* d_o, int64_t lddo,
                                 const void* key_mask, const float* lse, const float* delta, int n_q_pad, void* dq,
-                                int64_t lddq, void* dk, int64_t lddk, void* dv, int64_t lddv, const float* bias,
+                                int64_t lddq, float* dq_acc, void* dk, int64_t lddk, void* dv, int64_t lddv, const float* bias,
                                 float* dbias, int64_t bias_hstride, int64_t bias_rstride, int b, int h, int n_q,
                                 int n_k, int causal, float scale, alm_stream_t stream_) {
   using namespace alm;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  ALM_REQUIRE(q && k && v && d_o && lse && delta && dq && dk && dv, ALM_ERR_ARG);
+  ALM_REQUIRE(q && k && v && d_o && lse && delta && dq && dq_acc && dk && dv, ALM_ERR_ARG);
   ALM_REQUIRE(b > 0 && h > 0 && n_q > 0 && n_k >= n_q, ALM_ERR_ARG);
   ALM_REQUIRE(n_q_pad % AB_T == 0 && n_q_pad >= n_q, ALM_ERR_ARG);
   if (bias != nullptr) {
@@ -445,8 +367,8 @@ extern "C" int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64
   p.lse = lse; p.delta = delta;
   p.kmask = reinterpret_cast<const uint32_t*>(key_mask);
   p.kb_stride = (n_k + 127) / 128 * 4;
-  p.dq = (__nv_bfloat16*)dq; p.dk = (__nv_bfloat16*)dk; p.dv = (__nv_bfloat16*)dv;
-  p.lddq = lddq; p.lddk = lddk; p.lddv = lddv;
+  p.dq_acc = dq_acc; p.dk = (__nv_bfloat16*)dk; p.dv = (__nv_bfloat16*)dv;
+  p.lddk = lddk; p.lddv = lddv;
   p.bias = bias; p.dbias = dbias; p.bias_hs = bias_hstride; p.bias_rs = bias_rstride;
   p.b = b; p.h = h; p.n_q = n_q; p.n_k = n_k; p.n_q_pad = n_q_pad;
   p.causal = causal;
@@ -454,23 +376,20 @@ extern "C" int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64
   p.scale_log2 = scale * LOG2E;
   static bool attr_set = false;
   if (!attr_set) {
-    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_bwd_dkv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DKV_SMEM));
-    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_bwd_dq_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, DQ_SMEM));
-    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_bwd_dkv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DKV_SMEM));
-    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_bwd_dq_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DQ_SMEM));
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
     attr_set = true;
   }
-  dim3 grid_kv(((n_k + AB_T - 1) / AB_T) * b);
+  dim3 grid(((n_k + AB_T - 1) / AB_T) * b);
   if (bias != nullptr)
-    mqa_attn_bwd_dkv_kernel<true><<<grid_kv, AB_THREADS, DKV_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p);
+    mqa_attn_bwd_kernel<true><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p);
   else
-    mqa_attn_bwd_dkv_kernel<false><<<grid_kv, AB_THREADS, DKV_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p);
+    mqa_attn_bwd_kernel<false><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p);
   ALM_CHECK_LAUNCH();
-  dim3 grid_q((n_q + AB_T - 1) / AB_T, h, b);
-  if (bias != nullptr)
-    mqa_attn_bwd_dq_kernel<true><<<grid_q, AB_THREADS, DQ_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p);
-  else
-    mqa_attn_bwd_dq_kernel<false><<<grid_q, AB_THREADS, DQ_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p);
+  const long long rows = (long long)b * n_q;
+  const int cols4 = h * AB_D / 4;
+  attn_dq_convert_kernel<<<(unsigned)ceil_div(rows * cols4, 256LL), 256, 0, stream>>>(
+      reinterpret_cast<const float4*>(dq_acc), (__nv_bfloat16*)dq, lddq, rows, cols4);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(2);
   return ALM_OK;

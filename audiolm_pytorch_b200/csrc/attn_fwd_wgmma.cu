@@ -47,10 +47,7 @@ mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
                     const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw;
-  if ((smem_u32(smem) & 1023u) != 0) {  // SW128 tiles need 1024-B alignment
-    if (threadIdx.x == 0) printf("[alm] attn fwd: dynamic smem base not 1024-B aligned\n");
-    __trap();
-  }
+  if ((smem_u32(smem) & 1023u) != 0) __trap();  // SW128 tiles need 1024-B alignment
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + ATT_TILE_BYTES;                   // [stages]
   uint8_t* sV = sK + ATT_KV_STAGES * ATT_TILE_BYTES;   // [stages]

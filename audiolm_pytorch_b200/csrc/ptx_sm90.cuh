@@ -55,6 +55,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 // Blocking wait with a hang guard: a protocol bug traps (kernel fails with an error) instead of
 // wedging the GPU. 4 s is far beyond any legitimate wait in this library.
+// No diagnostic printf here: it compiles to a CALL, and any call in a wgmma kernel makes ptxas serialise every
+// wgmma (C7510, a wait after each mma_async).  build.py rejects a ptxas log that reports C7510.
 #ifndef ALM_MBAR_TIMEOUT_NS
 #define ALM_MBAR_TIMEOUT_NS 4000000000ull
 #endif
@@ -66,11 +68,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if ((++spins & 0x3FFu) == 0) {
       uint64_t now = global_timer_ns();
       if (t0 == 0) t0 = now;
-      else if (now - t0 > ALM_MBAR_TIMEOUT_NS) {
-        printf("[alm] mbarrier timeout: block (%d,%d,%d) thread %d bar@%u parity %u\n", blockIdx.x, blockIdx.y,
-               blockIdx.z, threadIdx.x, smem_u32(bar), parity);
-        __trap();
-      }
+      else if (now - t0 > ALM_MBAR_TIMEOUT_NS) __trap();
     }
   }
 }
@@ -120,6 +118,10 @@ __device__ __forceinline__ void bulk_wait_group() {
 }
 __device__ __forceinline__ void st_shared_u32(uint32_t smem_addr, uint32_t v) {
   asm volatile("st.shared.u32 [%0], %1;" ::"r"(smem_addr), "r"(v) : "memory");
+}
+// global fp32 reduction of two consecutive floats (8-B aligned), performed in L2 without a return value
+__device__ __forceinline__ void red_add_f32x2(float* gaddr, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(gaddr), "f"(a), "f"(b) : "memory");
 }
 // barrier over `nthreads` threads (a multiple of 32) on hardware barrier `id` (0 is __syncthreads')
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {

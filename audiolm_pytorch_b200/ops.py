@@ -230,8 +230,6 @@ def mqa_attn_bwd(q, k, v, o, d_o, lse, *, heads, key_mask=None, causal=True, sca
     n_q_pad = lse.shape[-1]
     assert d_o.dtype == bf16 and d_o.stride(-1) == 1 and o.stride(-1) == 1
     assert d_o.stride(0) == n_q * d_o.stride(1)
-    delta = torch.empty(b, heads, n_q_pad, device=q.device, dtype=f32)
-    _lib.call("alm_attn_delta", o, o.stride(1), d_o, d_o.stride(1), delta, n_q_pad, b, heads, n_q)
     key_mask = pack_key_mask(key_mask)
     if key_mask is not None:
         assert key_mask.n_k == n_k
@@ -239,17 +237,21 @@ def mqa_attn_bwd(q, k, v, o, d_o, lse, *, heads, key_mask=None, causal=True, sca
     if scale is None:
         scale = 64 ** -0.5
     dq = torch.empty(b, n_q, hd, device=q.device, dtype=bf16)
+    delta = torch.empty(b, heads, n_q_pad, device=q.device, dtype=f32)
+    dq_acc = torch.empty(b, n_q, hd, device=q.device, dtype=f32)  # fp32 dQ workspace, zeroed by alm_attn_delta
     dk = torch.empty(b, n_k, 64, device=q.device, dtype=bf16)
     dv = torch.empty(b, n_k, 64, device=q.device, dtype=bf16)
     bhs, brs = _check_bias(bias, heads, n_q, n_k) if bias is not None else (0, 0)
     if dbias is not None:
         assert bias is not None and dbias.dtype == f32 and dbias.shape == bias.shape and dbias.stride() == bias.stride()
     vis = (n_q * n_k - n_q * (n_q - 1) / 2) if causal else n_q * n_k
-    with _timed("mqa_attn_bwd_wgmma", 10.0 * b * heads * 64 * vis):  # 5 matmuls (algorithmic; 7 executed)
+    # 5 matmuls, each executed once; the timed region also covers delta + workspace zeroing and the dq conversion
+    with _timed("mqa_attn_bwd_wgmma", 10.0 * b * heads * 64 * vis):
+        _lib.call("alm_attn_delta", o, o.stride(1), d_o, d_o.stride(1), delta, n_q_pad, dq_acc, b, heads, n_q)
         _lib.call(
             "alm_mqa_attn_bwd",
             q, q.stride(1), k, k.stride(1), k.stride(0), v, v.stride(1), v.stride(0), d_o, d_o.stride(1), key_mask,
-            lse, delta, n_q_pad, dq, dq.stride(1), dk, dk.stride(1), dv, dv.stride(1),
+            lse, delta, n_q_pad, dq, dq.stride(1), dq_acc, dk, dk.stride(1), dv, dv.stride(1),
             bias, dbias, bhs, brs, b, heads, n_q, n_k, int(causal), float(scale),
         )
     return dq, dk, dv

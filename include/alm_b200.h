@@ -94,18 +94,22 @@ int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int
                      int n_q, int n_k, int causal, float scale, alm_stream_t stream);
 
 /*
- * Backward of alm_mqa_attn_fwd (two wgmma kernels: dK/dV per key block accumulating over all heads
- * in registers, then dQ per query block).  lse/delta are [b, h, n_q_pad] with n_q_pad a multiple of 128;
- * delta = rowsum(dO * O) from alm_attn_delta.  Autograd of attend.py:69-146.
+ * Backward of alm_mqa_attn_fwd (one wgmma kernel per (batch, 128-key block): dK/dV accumulate over all heads in
+ * registers, partial dQ products are reduced into dq_acc; a second kernel converts dq_acc to bf16 dq).
+ * lse/delta are [b, h, n_q_pad] with n_q_pad a multiple of 128; delta = rowsum(dO * O) from alm_attn_delta.
+ * dq_acc is an fp32 [b, n_q, h*64] contiguous workspace that must be zero on entry (alm_attn_delta zeroes it).
+ * dq is summed with fp32 atomics, so it is not bitwise reproducible from run to run; dk and dv are.
+ * Autograd of attend.py:69-146.
  */
 int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int64_t k_bstride, const void* v,
                      int64_t ldv, int64_t v_bstride, const void* d_o, int64_t lddo, const void* key_mask,
-                     const float* lse, const float* delta, int n_q_pad, void* dq, int64_t lddq, void* dk,
-                     int64_t lddk, void* dv, int64_t lddv, const float* bias, float* dbias, int64_t bias_hstride,
-                     int64_t bias_rstride, int b, int h, int n_q, int n_k, int causal, float scale,
-                     alm_stream_t stream);
+                     const float* lse, const float* delta, int n_q_pad, void* dq, int64_t lddq, float* dq_acc,
+                     void* dk, int64_t lddk, void* dv, int64_t lddv, const float* bias, float* dbias,
+                     int64_t bias_hstride, int64_t bias_rstride, int b, int h, int n_q, int n_k, int causal,
+                     float scale, alm_stream_t stream);
+/* delta[b, h, i] = rowsum(dO * O); also zeroes dq_acc ([b, n, h*64] fp32, contiguous) unless it is null */
 int alm_attn_delta(const void* o, int64_t ldo, const void* d_o, int64_t lddo, float* delta /* [b,h,stride] */,
-                   int64_t delta_stride, int b, int h, int n, alm_stream_t stream);
+                   int64_t delta_stride, float* dq_acc, int b, int h, int n, alm_stream_t stream);
 
 /*
  * Dense attention bias from a learned table (HBM-bound gather, scatter-add backward):

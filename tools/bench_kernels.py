@@ -79,7 +79,7 @@ if "attn" in which:
     timeit("attn fwd", lambda: ops.mqa_attn_fwd(q, k, v, heads=8), flops=fl)
     o, lse = ops.mqa_attn_fwd(q, k, v, heads=8)
     do = rnd(16, 2048, 512)
-    timeit("attn bwd (delta + dkv + dq)", lambda: ops.mqa_attn_bwd(q, k, v, o, do, lse, heads=8), flops=2.5 * fl)
+    timeit("attn bwd (delta + fused + dq convert)", lambda: ops.mqa_attn_bwd(q, k, v, o, do, lse, heads=8), flops=2.5 * fl)
 
 if "gemm" in which:
     from audiolm_pytorch_b200.transformer import best_split_k

@@ -1,5 +1,8 @@
 #!/usr/bin/env python
-"""Run-to-run bitwise determinism of the forward kernels at C3 sizes (races show up as mismatches)."""
+"""Run-to-run bitwise determinism of the forward kernels at C3 sizes (races show up as mismatches).
+
+The attention backward sums dq with fp32 atomics across key blocks, so dq is checked against a tolerance instead;
+dk and dv must stay bitwise reproducible."""
 import sys
 from pathlib import Path
 
@@ -18,20 +21,34 @@ def rnd(*s, dt=bf16, k=1.0):
     return (torch.randn(*s, device=dev) * k).to(dt)
 
 
-def check(name, fn, n=6):
+def check(name, fn, n=6, rtol=None):
+    """rtol: {output index: relative tolerance} for outputs summed by atomics (bitwise equality not expected)"""
+    rtol = rtol or {}
     ref = fn()
     ref = [t.clone() for t in (ref if isinstance(ref, (tuple, list)) else [ref]) if torch.is_tensor(t)]
-    bad = 0
+    bad, worst = 0, {i: 0.0 for i in rtol}
     for _ in range(n):
         out = fn()
         out = [t for t in (out if isinstance(out, (tuple, list)) else [out]) if torch.is_tensor(t)]
-        for a, b in zip(ref, out):
-            if not torch.equal(a, b):
-                bad += 1
-                diff = (a.float() - b.float()).abs()
-                print(f"   {name}: mismatch, max abs {diff.max().item():.4g}, count {(diff > 0).sum().item()} of {a.numel()}")
-                break
-    print(f"{name}: {'DETERMINISTIC' if bad == 0 else f'{bad}/{n} runs differ'}")
+        for i, (a, b) in enumerate(zip(ref, out)):
+            if i in rtol:
+                rel = ((a.float() - b.float()).abs().max() / a.float().abs().max().clamp_min(1e-30)).item()
+                worst[i] = max(worst[i], rel)
+                if rel <= rtol[i]:
+                    continue
+            elif torch.equal(a, b):
+                continue
+            bad += 1
+            diff = (a.float() - b.float()).abs()
+            print(f"   {name}: output {i} mismatch, max abs {diff.max().item():.4g}, count {(diff > 0).sum().item()} of {a.numel()}")
+            break
+    exact = [i for i in range(len(ref)) if i not in rtol]
+    verdict = "DETERMINISTIC" if bad == 0 else f"{bad}/{n} runs differ"
+    if rtol:
+        verdict += f" (outputs {exact} bitwise; " + ", ".join(
+            f"output {i} atomically summed: max diff {worst[i]:.2g} of its max |value|, tolerance {rtol[i]:.0g}"
+            for i in rtol) + ")"
+    print(f"{name}: {verdict}")
 
 
 a, w1 = rnd(M, d), rnd(5472, d, k=0.03)
@@ -52,7 +69,7 @@ check("attn fwd", lambda: ops.mqa_attn_fwd(q, k, v, heads=8))
 check("attn fwd masked", lambda: ops.mqa_attn_fwd(q, k, v, heads=8, key_mask=mask))
 o, lse = ops.mqa_attn_fwd(q, k, v, heads=8)
 do = rnd(16, 2048, 512)
-check("attn bwd", lambda: ops.mqa_attn_bwd(q, k, v, o, do, lse, heads=8))
+check("attn bwd (dq, dk, dv)", lambda: ops.mqa_attn_bwd(q, k, v, o, do, lse, heads=8), rtol={0: 1e-2})
 q1 = rnd(16, 1, 512)
 check("attn fwd decode n_q=1", lambda: ops.mqa_attn_fwd(q1, k, v, heads=8)[0])  # lse pad rows are unwritten
 hc = dict(gamma=rnd(d, dt=torch.float32, k=0.1), dyn_alpha=rnd(d, 5, dt=torch.float32, k=0.05),
