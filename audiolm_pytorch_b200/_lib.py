@@ -18,12 +18,16 @@ P = C.c_void_p
 I = C.c_int
 L = C.c_int64
 F = C.c_float
+U32 = C.c_uint32
+U64 = C.c_uint64
+DROP = [F, U64, U32]  # dropout_p, seed, site
 
 # name -> argtypes (stream is always last and always a void*)
 SIGNATURES: dict[str, list] = {
     "alm_gemm_bf16": [P, I, L, L, P, I, L, L, P, I, L, L, I, I, I, I, F, P, I, I, P],
-    "alm_mqa_attn_fwd": [P, L, P, L, L, P, L, L, P, P, L, P, L, P, L, L, I, I, I, I, I, F, P],
-    "alm_mqa_attn_bwd": [P, L, P, L, L, P, L, L, P, L, P, P, P, I, P, L, P, P, L, P, L, P, P, L, L, I, I, I, I, I, F, P],
+    "alm_mqa_attn_fwd": [P, L, P, L, L, P, L, L, P, P, L, P, L, P, L, L, I, I, I, I, I, F, *DROP, P],
+    "alm_mqa_attn_bwd": [P, L, P, L, L, P, L, L, P, L, P, P, P, I, P, L, P, P, L, P, L, P, P, L, L, I, I, I, I, I, F, *DROP,
+                         P],
     "alm_pack_key_mask": [P, P, I, I, P],
     "alm_embed_gather": [P, I, P, P, I, I, P],
     "alm_embed_scatter": [P, I, P, P, I, I, P],
@@ -41,8 +45,9 @@ SIGNATURES: dict[str, list] = {
     "alm_hc_param_finish": [P, P, P, P, P, P, P, I, P],
     "alm_hc_post_fwd": [P, P, P, P, P, P, I, I, I, P],
     "alm_hc_post_bwd": [P, P, P, P, P, P, P, P, P, P, I, I, I, P],
-    "alm_geglu_ln_fwd": [P, L, I, P, P, L, P, I, I, I, P],
-    "alm_geglu_ln_bwd": [P, L, I, P, P, P, L, P, P, I, I, I, P],
+    "alm_geglu_ln_fwd": [P, L, I, P, P, L, P, I, I, I, *DROP, P],
+    "alm_geglu_ln_bwd": [P, L, I, P, P, P, L, P, P, I, I, I, *DROP, P],
+    "alm_dropout_bf16": [P, L, L, I, *DROP, P],
     "alm_ce_fwd_bwd": [P, L, P, L, P, P, L, P, P, I, I, I, P],
     "alm_axpby_bf16": [P, L, F, P, L, F, P, L, L, I, P],
     "alm_cast_pad_bf16": [P, L, P, L, L, I, I, P],

@@ -87,4 +87,70 @@ __device__ __forceinline__ void gelu_parts(float x, float& cdf, float& xpdf) {
   xpdf = 0.3989422804014327f * x * e;
 }
 
+// ---- dropout mask ------------------------------------------------------------------------------
+// Every dropout decision of the library is keep(seed, site, row, col): a pure function of its arguments, so the
+// backward regenerates the forward's mask instead of storing it.  Coordinates: elementwise sites on an [M, C]
+// activation use (token b*n + i, channel); attention probabilities use ((b*H + h) * n_q_pad + i, key j), with
+// n_q_pad = n_q rounded up to 128 (the LSE row stride), so that 16-row groups never straddle two heads.
+//
+// Generator: Philox4x32-10 (Salmon et al., SC'11; the generator of torch's CUDA RNG), key = the 64-bit seed.
+// One draw gives four 32-bit words = eight 16-bit uniforms.  They decide the 8 elements
+//     rows {i0, i0+1, i0+8, i0+9} x cols {j0, j0+8},   i0 % 16 in {0, 2, 4, 6},  j0 % 16 < 8,
+// counter = (row / 16, col / 16, site, 8 * ((row % 8) / 2) + col % 8); row i0 + r1 + 8 r8 takes word r1 + 2 r8
+// and col j0 + 8 c8 takes its low (c8 = 0) or high half.  This group lies inside what one thread of the attention
+// backward holds of dP^T / P^T (two key rows j0, j0 + 8 by query columns {2c, 2c+1} mod 8), so there every draw
+// is used in full.  The attention forward holds rows {r, r+8} by the same columns: a lane pair (r, r^1) splits
+// the draws and swaps halves with one shuffle per word.  Keep iff the 16-bit uniform < thr, thr = round(65536 (1-p)),
+// so the keep probability is exact to 2^-17.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+    const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+    k0 += 0x9E3779B9u;
+    k1 += 0xBB67AE85u;
+  }
+  return c;
+}
+
+struct DropoutArgs {
+  uint64_t seed;
+  uint32_t site;
+  uint32_t thr;   // keep iff the 16-bit uniform < thr (65536: keep all)
+  float scale;    // 1 / (1 - p)
+};
+
+// the draw of the 8-element group that holds (row, col)
+__device__ __forceinline__ uint4 dropout_draw(const DropoutArgs& d, uint32_t row, uint32_t col) {
+  const uint4 ctr = make_uint4(row >> 4, col >> 4, d.site, ((row & 7u) >> 1) * 8u + (col & 7u));
+  return philox4x32_10(ctr, (uint32_t)d.seed, (uint32_t)(d.seed >> 32));
+}
+
+// the word of a draw that holds `row`'s two elements
+__device__ __forceinline__ uint32_t dropout_word(const uint4& draw, uint32_t row) {
+  return (row & 1u) ? ((row & 8u) ? draw.w : draw.y) : ((row & 8u) ? draw.z : draw.x);
+}
+
+// the decision for (row, col) inside its group's draw (only the word of `row` is read)
+__device__ __forceinline__ bool dropout_pick(const DropoutArgs& d, const uint4& draw, uint32_t row, uint32_t col) {
+  const uint32_t w = dropout_word(draw, row);
+  const uint32_t u = (col & 8u) ? (w >> 16) : (w & 0xFFFFu);
+  return u < d.thr;
+}
+
+__device__ __forceinline__ bool dropout_keep(const DropoutArgs& d, uint32_t row, uint32_t col) {
+  return dropout_pick(d, dropout_draw(d, row, col), row, col);
+}
+
+inline DropoutArgs make_dropout_args(float p, uint64_t seed, uint32_t site) {
+  DropoutArgs a;
+  a.seed = seed;
+  a.site = site;
+  const double keep = 1.0 - (double)p;
+  a.thr = (uint32_t)(keep * 65536.0 + 0.5);
+  a.scale = (float)(1.0 / keep);
+  return a;
+}
+
 }  // namespace alm

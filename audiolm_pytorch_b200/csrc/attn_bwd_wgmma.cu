@@ -18,6 +18,11 @@
 // overlaps the dS arithmetic.  The two warpgroups meet once per iteration, on a named barrier, when both halves of
 // dS^T are in shared memory; dS^T is double-buffered so that barrier also orders its reuse.  Past that barrier both
 // have released the previous iteration's slot, so warp 0 refills it without waiting: STAGES - 1 loads stay ahead.
+// With DROPOUT (keep mask Z from alm_common.cuh: dropout_keep, regenerated here, never stored):
+//     dV += (P^T o Z / (1-p)) dO,   dP^T <- dP^T o Z / (1-p),   dS^T = P^T (dP^T - delta)
+// delta = rowsum(dO o O) needs no change because O is the dropped output.  One thread's two key rows by its query
+// columns {2c, 2c+1} mod 8 are exactly whole 8-element groups of the generator, so 8 draws per tile cover its 64
+// elements; they run while S^T and dP^T are computed.
 #include "alm_common.cuh"
 #include "ptx_sm90.cuh"
 
@@ -76,6 +81,25 @@ __device__ __forceinline__ void store_d64(const float (&acc)[32], __nv_bfloat16*
   }
 }
 
+// keep bits of one (128 keys x 128 queries) tile for this thread: key rows key0, key0 + 8, query columns
+// qrow0 + 8 g + c (qrow0 = counter row of column 0 of this thread); bit 4 g + 2 h + c, the index of st / dpt
+__device__ __forceinline__ uint64_t attn_bwd_keep_bits(const DropoutArgs& d, uint32_t qrow0, uint32_t key0) {
+  uint64_t bits = 0;
+#pragma unroll
+  for (int cc = 0; cc < AB_T / 16; ++cc) {
+    const uint32_t i0 = qrow0 + 16 * cc;
+    const uint4 dr = dropout_draw(d, i0, key0);
+#pragma unroll
+    for (int gh = 0; gh < 2; ++gh)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int c = 0; c < 2; ++c)
+          if (dropout_pick(d, dr, i0 + 8 * gh + c, key0 + 8 * h)) bits |= 1ull << (8 * cc + 4 * gh + 2 * h + c);
+  }
+  return bits;
+}
+
 // ================================================================================================
 // fused dK / dV / dQ
 // ================================================================================================
@@ -83,11 +107,11 @@ constexpr int AB_DS_TILE = AB_T * AB_T * 2;   // dS^T tile [128 keys][128 querie
 constexpr int AB_SMEM = AB_TILE * (2 + 2 * AB_STAGES) + 2 * AB_DS_TILE + AB_STAGES * 2 * 512 + 256;
 constexpr uint32_t AB_DS_BAR = 1;             // named barrier of the two consumer warpgroups (0 is __syncthreads)
 
-template <bool HAS_BIAS>
+template <bool HAS_BIAS, bool DROPOUT>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
-                    const AttnBwdParams p) {
+                    const AttnBwdParams p, const DropoutArgs drop) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* sK = smem;
@@ -189,6 +213,9 @@ mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       wgmma_ss<AB_T>(dpt, wgmma_desc_sw128(v_addr + k * 32, 1024, 16), wgmma_desc_sw128(do_addr + k * 32, 1024, 16),
                      k > 0 ? 1u : 0u);
     wgmma_commit();
+    [[maybe_unused]] uint64_t keep = 0;
+    if constexpr (DROPOUT)
+      keep = attn_bwd_keep_bits(drop, ((uint32_t)batch * p.h + head) * (uint32_t)p.n_q_pad + q0 + c_lane, kj[0]);
     const float* lse_s = sLse + stage * AB_T;
     const float* del_s = sDelta + stage * AB_T;
     // whole tile below the causal diagonal and inside n_q: only the per-row key flag matters
@@ -219,7 +246,14 @@ mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       }
     // dV += P^T dO runs under the dS arithmetic
     uint32_t pa[8][4];
-    pack_a_frags(st, pa);
+    if constexpr (DROPOUT) {
+      float pz[64];
+#pragma unroll
+      for (int e = 0; e < 64; ++e) pz[e] = ((keep >> e) & 1u) ? st[e] * drop.scale : 0.f;
+      pack_a_frags(pz, pa);
+    } else {
+      pack_a_frags(st, pa);
+    }
     wgmma_fence_acc(dv);
     wgmma_fence();
 #pragma unroll
@@ -242,7 +276,11 @@ mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         for (int h = 0; h < 2; ++h) {
           const int e = 4 * g + 2 * h + c;
           const bool ok = visible(h, qi);
-          const float ds = ok ? st[e] * (dpt[e] - dl) : 0.f;
+          float ds;
+          if constexpr (DROPOUT)
+            ds = ok ? st[e] * ((((keep >> e) & 1u) ? dpt[e] * drop.scale : 0.f) - dl) : 0.f;
+          else
+            ds = ok ? st[e] * (dpt[e] - dl) : 0.f;
           if constexpr (HAS_BIAS) {
             if (ok && p.dbias != nullptr) atomicAdd(p.dbias + bias_index(h, qi), ds);
           }
@@ -325,12 +363,17 @@ extern "C" int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64
                                 const void* key_mask, const float* lse, const float* delta, int n_q_pad, void* dq,
                                 int64_t lddq, float* dq_acc, void* dk, int64_t lddk, void* dv, int64_t lddv, const float* bias,
                                 float* dbias, int64_t bias_hstride, int64_t bias_rstride, int b, int h, int n_q,
-                                int n_k, int causal, float scale, alm_stream_t stream_) {
+                                int n_k, int causal, float scale, float dropout_p, uint64_t seed, uint32_t site,
+                                alm_stream_t stream_) {
   using namespace alm;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ALM_REQUIRE(q && k && v && d_o && lse && delta && dq && dq_acc && dk && dv, ALM_ERR_ARG);
   ALM_REQUIRE(b > 0 && h > 0 && n_q > 0 && n_k >= n_q, ALM_ERR_ARG);
   ALM_REQUIRE(n_q_pad % AB_T == 0 && n_q_pad >= n_q, ALM_ERR_ARG);
+  ALM_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, ALM_ERR_ARG);
+  // the dropout counter rows are (b*h + head) * (n_q rounded up to 128) + i, as in the forward
+  ALM_REQUIRE(dropout_p == 0.f || n_q_pad == (n_q + AB_T - 1) / AB_T * AB_T, ALM_ERR_ARG);
+  ALM_REQUIRE((long long)b * h * n_q_pad < (1ll << 32), ALM_ERR_UNSUPPORTED);
   if (bias != nullptr) {
     ALM_REQUIRE(bias_rstride >= n_k && bias_rstride % 4 == 0 && bias_hstride % 4 == 0, ALM_ERR_ALIGN);
     ALM_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15u) == 0, ALM_ERR_ALIGN);
@@ -374,17 +417,26 @@ extern "C" int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64
   p.causal = causal;
   p.scale = scale;
   p.scale_log2 = scale * LOG2E;
+  // counter rows (b*h + head) * n_q_pad + i, columns = key index
+  const DropoutArgs dargs = make_dropout_args(dropout_p, seed, site);
   static bool attr_set = false;
   if (!attr_set) {
-    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
-    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_bwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_bwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_bwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_bwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, AB_SMEM));
     attr_set = true;
   }
   dim3 grid(((n_k + AB_T - 1) / AB_T) * b);
-  if (bias != nullptr)
-    mqa_attn_bwd_kernel<true><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p);
+  const bool drop = dropout_p > 0.f;
+  if (bias != nullptr && drop)
+    mqa_attn_bwd_kernel<true, true><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p, dargs);
+  else if (bias != nullptr)
+    mqa_attn_bwd_kernel<true, false><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p, dargs);
+  else if (drop)
+    mqa_attn_bwd_kernel<false, true><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p, dargs);
   else
-    mqa_attn_bwd_kernel<false><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p);
+    mqa_attn_bwd_kernel<false, false><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p, dargs);
   ALM_CHECK_LAUNCH();
   const long long rows = (long long)b * n_q;
   const int cols4 = h * AB_D / 4;

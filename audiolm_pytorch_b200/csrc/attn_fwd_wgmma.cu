@@ -9,6 +9,8 @@
 //   warpgroup 0 : TMA producer (warp 0)      warpgroups 1, 2 : softmax + MMA, query rows [0, 64) / [64, 128)
 // An optional additive score bias [h, n_q, n_k] (flash_attn=False path, attend.py:122-124) is added to the scores;
 // tiles that lie fully below the causal diagonal take a predicate-free path.
+// With DROPOUT, P is multiplied by the keep mask (alm_common.cuh: dropout_keep) times 1/(1-p) when it is packed into
+// the A operand of P V; the row max, the row sum and the stored LSE use the un-dropped P.
 #include "alm_common.cuh"
 #include "ptx_sm90.cuh"
 
@@ -33,6 +35,8 @@ struct AttnFwdParams {
   int b, h, n_q, n_k;
   int causal;
   float scale_log2;       // d^-1/2 * log2(e)
+  int n_q_pad;            // n_q rounded up to 128: query rows of the dropout counter are (b*h + head) * n_q_pad + i
+  DropoutArgs drop;
 };
 
 __device__ __forceinline__ float att_ex2(float x) {
@@ -41,7 +45,33 @@ __device__ __forceinline__ float att_ex2(float x) {
   return y;
 }
 
-template <bool HAS_BIAS>
+// Dropout keep bits of one 128-key tile for this thread's fragment: rows qrow, qrow + 8 (counter rows), columns
+// kbase + 8 g + c_lane + c; bit 4 g + 2 h + c. The lane pair (lane, lane ^ 4) holds rows (qrow, qrow ^ 1): for each
+// 16-key step each of the two draws the group of its own c and hands the partner the words of the partner's rows.
+__device__ __forceinline__ uint64_t attn_fwd_keep_bits(const DropoutArgs& d, uint32_t qrow, uint32_t kbase, int c_lane) {
+  const uint32_t odd = qrow & 1u;
+  uint64_t bits = 0;
+#pragma unroll
+  for (int kk = 0; kk < ATT_BN / 16; ++kk) {
+    const uint32_t j0 = kbase + 16 * kk + c_lane;
+    const uint4 own = dropout_draw(d, qrow, j0 + odd);
+    const uint32_t ra = __shfl_xor_sync(0xffffffffu, odd ? own.x : own.y, 4);
+    const uint32_t rb = __shfl_xor_sync(0xffffffffu, odd ? own.z : own.w, 4);
+    const uint4 other = odd ? make_uint4(0u, ra, 0u, rb) : make_uint4(ra, 0u, rb, 0u);
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      const uint4 dr = (uint32_t)c == odd ? own : other;
+#pragma unroll
+      for (int half = 0; half < 2; ++half)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (dropout_pick(d, dr, qrow + 8 * h, j0 + 8 * half + c)) bits |= 1ull << (8 * kk + 4 * half + 2 * h + c);
+    }
+  }
+  return bits;
+}
+
+template <bool HAS_BIAS, bool DROPOUT>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p) {
@@ -127,6 +157,7 @@ mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   }
   const uint32_t* mrow = p.kmask ? p.kmask + (long long)batch * p.kb_stride : nullptr;
   const uint32_t q_addr = smem_u32(sQ) + cw * 8192;
+  [[maybe_unused]] const uint32_t drop_row = ((uint32_t)batch * p.h + head) * (uint32_t)p.n_q_pad + q0 + r_base;
 
   if (n_tiles > 0) mbar_wait(q_full, 0);
   int stage = 0;
@@ -142,6 +173,8 @@ mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       wgmma_ss<ATT_BN>(s, wgmma_desc_sw128(q_addr + k * 32, 1024, 16), wgmma_desc_sw128(k_addr + k * 32, 1024, 16),
                        k > 0 ? 1u : 0u);
     wgmma_commit();
+    [[maybe_unused]] uint64_t keep = 0;  // drawn while S = Q K^T runs
+    if constexpr (DROPOUT) keep = attn_fwd_keep_bits(p.drop, drop_row, j * ATT_BN, c_lane);
     wgmma_wait<0>();
     wgmma_fence_acc(s);
 
@@ -196,6 +229,10 @@ mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         o_acc[4 * g + 2 * h] *= alpha;
         o_acc[4 * g + 2 * h + 1] *= alpha;
       }
+    }
+    if constexpr (DROPOUT) {
+#pragma unroll
+      for (int e = 0; e < ATT_BN / 2; ++e) s[e] = ((keep >> e) & 1u) ? s[e] * p.drop.scale : 0.f;
     }
 #pragma unroll
     for (int kk = 0; kk < ATT_BN / 16; ++kk) {
@@ -269,11 +306,13 @@ extern "C" int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64
                                 const void* v, int64_t ldv, int64_t v_bstride, const void* key_mask, void* o,
                                 int64_t ldo, float* lse, int64_t lse_stride, const float* bias, int64_t bias_hstride,
                                 int64_t bias_rstride, int b, int h, int n_q, int n_k, int causal, float scale,
-                                alm_stream_t stream_) {
+                                float dropout_p, uint64_t seed, uint32_t site, alm_stream_t stream_) {
   using namespace alm;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ALM_REQUIRE(q && k && v && o, ALM_ERR_ARG);
   ALM_REQUIRE(b > 0 && h > 0 && n_q > 0 && n_k > 0 && n_k >= n_q, ALM_ERR_ARG);
+  ALM_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, ALM_ERR_ARG);
+  ALM_REQUIRE((long long)b * h * ((n_q + 127) / 128 * 128) < (1ll << 32), ALM_ERR_UNSUPPORTED);  // 32-bit counter rows
   ALM_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0, ALM_ERR_ALIGN);
   ALM_REQUIRE(k_bstride % 8 == 0 && v_bstride % 8 == 0, ALM_ERR_ALIGN);
   ALM_REQUIRE((reinterpret_cast<uintptr_t>(o) & 15u) == 0, ALM_ERR_ALIGN);
@@ -314,19 +353,30 @@ extern "C" int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64
   p.b = b; p.h = h; p.n_q = n_q; p.n_k = n_k;
   p.causal = causal;
   p.scale_log2 = scale * 1.4426950408889634f;
+  p.n_q_pad = (n_q + 127) / 128 * 128;
+  p.drop = make_dropout_args(dropout_p, seed, site);
   static bool attr_set = false;
   if (!attr_set) {
-    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      ATT_SMEM_BYTES));
-    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     ATT_SMEM_BYTES));
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     ATT_SMEM_BYTES));
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      ATT_SMEM_BYTES));
     attr_set = true;
   }
   dim3 grid((n_q + ATT_BM - 1) / ATT_BM, h, b);
-  if (bias != nullptr)
-    mqa_attn_fwd_kernel<true><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
+  const bool drop = dropout_p > 0.f;
+  if (bias != nullptr && drop)
+    mqa_attn_fwd_kernel<true, true><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
+  else if (bias != nullptr)
+    mqa_attn_fwd_kernel<true, false><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
+  else if (drop)
+    mqa_attn_fwd_kernel<false, true><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
   else
-    mqa_attn_fwd_kernel<false><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
+    mqa_attn_fwd_kernel<false, false><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);
   return ALM_OK;

@@ -5,6 +5,7 @@
 //   attn_delta : rowsum(dO * O) for the attention backward
 //   axpby      : value-residual mix v = 0.5 (v + v_first) (audiolm_pytorch.py:355-358) and its backward
 //   cast_pad   : fp32 master weights -> zero-padded bf16 operand copies for the TMA/wgmma GEMMs
+//   dropout    : in-place bf16 dropout (attention-branch output and its gradient)
 #include <stdlib.h>
 
 #include "alm_common.cuh"
@@ -67,6 +68,28 @@ __device__ __forceinline__ void block_sum_nt(float (&v)[N], float* buf /*[N][NT/
   }
 }
 
+// Dropout keep bits of row m, columns c0 .. c0 + 7 (bit e: column c0 + e) for a row-per-CTA kernel whose lanes hold
+// 8 consecutive columns each, lane pairs (2t, 2t+1) a 16-column group.  Column c0 + e belongs to the draw of group
+// column (c0 & ~15) + e, whose word for row m also decides column c0 + e ^ 8 of the partner lane: each lane of the
+// pair draws 4 of the 8 groups and passes the word of row m to the other.  Every lane of the warp must call this.
+__device__ __forceinline__ uint32_t row_keep_bits8(const DropoutArgs& d, uint32_t m, uint32_t c0) {
+  const uint32_t hi = (c0 >> 3) & 1u;
+  const uint32_t jb = c0 & ~15u;
+  uint32_t own[4], other[4];
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    own[t] = dropout_word(dropout_draw(d, m, jb + 4 * hi + t), m);
+    other[t] = __shfl_xor_sync(0xffffffffu, own[t], 1);
+  }
+  uint32_t bits = 0;
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    const uint32_t w = ((uint32_t)e >> 2) == hi ? own[e & 3] : other[e & 3];
+    if (dropout_pick(d, make_uint4(w, w, w, w), m, c0 + e)) bits |= 1u << e;
+  }
+  return bits;
+}
+
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.7071067811865476f)); }
 
 __device__ __forceinline__ float gelu_erf_grad(float x) {
@@ -76,11 +99,12 @@ __device__ __forceinline__ float gelu_erf_grad(float x) {
 }
 
 // h [M, ldh]: a = h[:, 0:inner], gate = h[:, gate_off : gate_off+inner]   ->  gn [M, ldg] (cols >= inner are 0)
-template <int NCH, int NT>
+// DROPOUT: gn = LN(...) * gamma * keep(row, channel) / (1 - p)
+template <int NCH, int NT, bool DROPOUT>
 __global__ void __launch_bounds__(NT)
 geglu_ln_fwd_kernel(const __nv_bfloat16* __restrict__ h, long long ldh, int gate_off,
                     const float* __restrict__ gamma, __nv_bfloat16* __restrict__ gn, long long ldg,
-                    float* __restrict__ stats, int M, int inner, int inner_pad) {
+                    float* __restrict__ stats, int M, int inner, int inner_pad, const DropoutArgs drop) {
   __shared__ float buf[2 * (NT / 32)];
   // software pipeline: the NEXT row's operands are loaded into registers before this row is reduced, so the
   // load latency overlaps the erf / reduction / store phases of the current row (the row after that is pulled
@@ -139,6 +163,8 @@ geglu_ln_fwd_kernel(const __nv_bfloat16* __restrict__ h, long long ldh, int gate
 #pragma unroll
     for (int k = 0; k < NCH; ++k) {
       const int c0 = (threadIdx.x + k * NT) * 8;
+      [[maybe_unused]] uint32_t keep = 0;
+      if constexpr (DROPOUT) keep = row_keep_bits8(drop, m, c0);
       if (c0 < inner_pad) {
         const int nv = min(8, inner - c0);
         float gm[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -154,6 +180,10 @@ geglu_ln_fwd_kernel(const __nv_bfloat16* __restrict__ h, long long ldh, int gate
         float o[8];
 #pragma unroll
         for (int e = 0; e < 8; ++e) o[e] = e < nv ? (g[k][e] - mean) * rstd * gm[e] : 0.f;
+        if constexpr (DROPOUT) {
+#pragma unroll
+          for (int e = 0; e < 8; ++e) o[e] = ((keep >> e) & 1u) ? o[e] * drop.scale : 0.f;
+        }
         *reinterpret_cast<uint4*>(gn + (size_t)m * ldg + c0) = pack8b(o);
       }
     }
@@ -166,12 +196,13 @@ geglu_ln_fwd_kernel(const __nv_bfloat16* __restrict__ h, long long ldh, int gate
   }
 }
 
-template <int NCH, int NT>
+// DROPOUT: the incoming dgn is multiplied by the forward's mask / (1 - p) first
+template <int NCH, int NT, bool DROPOUT>
 __global__ void __launch_bounds__(NT, NT == 512 ? 2 : 1)
 geglu_ln_bwd_kernel(const __nv_bfloat16* __restrict__ h, long long ldh, int gate_off,
                     const float* __restrict__ gamma, const float* __restrict__ stats,
                     const __nv_bfloat16* __restrict__ dgn, long long ldg, __nv_bfloat16* __restrict__ dh,
-                    float* __restrict__ g_gamma, int M, int inner, int inner_pad) {
+                    float* __restrict__ g_gamma, int M, int inner, int inner_pad, const DropoutArgs drop) {
   __shared__ float buf[2 * (NT / 32)];
   float gacc[NCH][8];
 #pragma unroll
@@ -199,11 +230,17 @@ geglu_ln_bwd_kernel(const __nv_bfloat16* __restrict__ h, long long ldh, int gate
       const int c0 = (threadIdx.x + k * NT) * 8;
 #pragma unroll
       for (int e = 0; e < 8; ++e) { a[k][e] = gp[k][e] = gl[k][e] = ge[k][e] = 0.f; }
+      [[maybe_unused]] uint32_t keep = 0;
+      if constexpr (DROPOUT) keep = row_keep_bits8(drop, m, c0);
       if (c0 < inner_pad) {
         float dv[8], gt[8];
         unpack8b(*reinterpret_cast<const uint4*>(h + (size_t)m * ldh + c0), a[k]);
         unpack8b(*reinterpret_cast<const uint4*>(h + (size_t)m * ldh + gate_off + c0), gt);
         unpack8b(*reinterpret_cast<const uint4*>(dgn + (size_t)m * ldg + c0), dv);
+        if constexpr (DROPOUT) {
+#pragma unroll
+          for (int e = 0; e < 8; ++e) dv[e] = ((keep >> e) & 1u) ? dv[e] * drop.scale : 0.f;
+        }
         const int nv = min(8, inner - c0);
         float gm[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         if (nv == 8) {
@@ -537,33 +574,103 @@ __global__ void resid_ln_bwd_kernel(const float* __restrict__ r_new, const float
   }
 }
 
+// ---- in-place dropout: one thread per rows {i0, i0+1, i0+8, i0+9} x 16 columns (8 draws, all used) ------------
+__global__ void __launch_bounds__(256)
+dropout_bf16_kernel(__nv_bfloat16* __restrict__ x, long long ld, long long M, int C, const DropoutArgs d) {
+  const int ncb = (C + 15) / 16;
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long rest = t / ncb;
+  const int cb = (int)(t - rest * ncb);
+  const long long rb = rest >> 2;
+  if (rb * 16 >= M) return;
+  const uint32_t i0 = (uint32_t)(rb * 16 + 2 * (rest & 3));
+  const uint32_t j0 = (uint32_t)cb * 16;
+  uint4 dr[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) dr[e] = dropout_draw(d, i0, j0 + e);
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    const uint32_t row = i0 + (r & 1) + 8 * (r >> 1);
+    if (row >= M) continue;
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      const uint32_t c = j0 + 8 * half;
+      if ((int)c >= C) continue;
+      uint4* ptr = reinterpret_cast<uint4*>(x + (size_t)row * ld + c);
+      float f[8];
+      unpack8b(*ptr, f);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) f[e] = dropout_pick(d, dr[e], row, c + e) ? f[e] * d.scale : 0.f;
+      *ptr = pack8b(f);
+    }
+  }
+}
+
 }  // namespace alm
 
 using namespace alm;
 
+extern "C" int alm_dropout_bf16(void* x, int64_t ld, int64_t M, int C, float p, uint64_t seed, uint32_t site,
+                                alm_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ALM_REQUIRE(x && M >= 0 && C >= 0 && p >= 0.f && p < 1.f, ALM_ERR_ARG);
+  ALM_REQUIRE(C % 8 == 0 && ld % 8 == 0 && ld >= C && (reinterpret_cast<uintptr_t>(x) & 15u) == 0, ALM_ERR_ALIGN);
+  ALM_REQUIRE(M < (1ll << 32), ALM_ERR_UNSUPPORTED);  // 32-bit counter rows
+  if (M == 0 || C == 0 || p == 0.f) return ALM_OK;
+  const long long threads = (M + 15) / 16 * 4 * ((C + 15) / 16);
+  dropout_bf16_kernel<<<(unsigned)ceil_div(threads, 256LL), 256, 0, stream>>>(
+      reinterpret_cast<__nv_bfloat16*>(x), ld, M, C, make_dropout_args(p, seed, site));
+  ALM_CHECK_LAUNCH();
+  ALM_LAUNCHED(1);
+  return ALM_OK;
+}
+
+template <bool DROPOUT>
+static void launch_geglu_ln_fwd(int nch, int grid, cudaStream_t stream, const __nv_bfloat16* hp, int64_t ldh,
+                                int gate_off, const float* gamma, __nv_bfloat16* gp, int64_t ldg, float* stats, int M,
+                                int inner, int inner_pad, const DropoutArgs& d) {
+  if (nch <= 1) geglu_ln_fwd_kernel<1, 256, DROPOUT><<<grid, FF_THREADS, 0, stream>>>(hp, ldh, gate_off, gamma, gp, ldg, stats, M, inner, inner_pad, d);
+  else if (nch == 2) geglu_ln_fwd_kernel<2, 256, DROPOUT><<<grid, FF_THREADS, 0, stream>>>(hp, ldh, gate_off, gamma, gp, ldg, stats, M, inner, inner_pad, d);
+  else geglu_ln_fwd_kernel<4, 256, DROPOUT><<<grid, FF_THREADS, 0, stream>>>(hp, ldh, gate_off, gamma, gp, ldg, stats, M, inner, inner_pad, d);
+}
+
 extern "C" int alm_geglu_ln_fwd(const void* h, int64_t ldh, int gate_off, const float* gamma, void* gn, int64_t ldg,
-                                float* stats, int M, int inner, int inner_pad, alm_stream_t stream_) {
+                                float* stats, int M, int inner, int inner_pad, float dropout_p, uint64_t seed,
+                                uint32_t site, alm_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ALM_REQUIRE(M > 0 && inner > 0 && inner_pad >= inner && inner_pad % 8 == 0, ALM_ERR_ARG);
+  ALM_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, ALM_ERR_ARG);
   ALM_REQUIRE(ldh % 8 == 0 && ldg % 8 == 0 && gate_off % 8 == 0, ALM_ERR_ALIGN);
   const int nch = ceil_div(inner_pad / 8, FF_THREADS);
   ALM_REQUIRE(nch <= FF_MAX_CHUNKS, ALM_ERR_UNSUPPORTED);
   const int grid = min(M, num_sms() * 8);
   auto* hp = (const __nv_bfloat16*)h;
   auto* gp = (__nv_bfloat16*)gn;
-  if (nch <= 1) geglu_ln_fwd_kernel<1, 256><<<grid, FF_THREADS, 0, stream>>>(hp, ldh, gate_off, gamma, gp, ldg, stats, M, inner, inner_pad);
-  else if (nch == 2) geglu_ln_fwd_kernel<2, 256><<<grid, FF_THREADS, 0, stream>>>(hp, ldh, gate_off, gamma, gp, ldg, stats, M, inner, inner_pad);
-  else geglu_ln_fwd_kernel<4, 256><<<grid, FF_THREADS, 0, stream>>>(hp, ldh, gate_off, gamma, gp, ldg, stats, M, inner, inner_pad);
+  const DropoutArgs d = make_dropout_args(dropout_p, seed, site);
+  if (dropout_p > 0.f) launch_geglu_ln_fwd<true>(nch, grid, stream, hp, ldh, gate_off, gamma, gp, ldg, stats, M, inner, inner_pad, d);
+  else launch_geglu_ln_fwd<false>(nch, grid, stream, hp, ldh, gate_off, gamma, gp, ldg, stats, M, inner, inner_pad, d);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);
   return ALM_OK;
 }
 
+template <bool DROPOUT>
+static void launch_geglu_ln_bwd(int nch, int threads, int grid, cudaStream_t stream, const __nv_bfloat16* hp,
+                                int64_t ldh, int gate_off, const float* gamma, const float* stats,
+                                const __nv_bfloat16* dg, int64_t ldg, __nv_bfloat16* dhp, float* g_gamma, int M,
+                                int inner, int inner_pad, const DropoutArgs& d) {
+  if (threads == 512) geglu_ln_bwd_kernel<1, 512, DROPOUT><<<grid, 512, 0, stream>>>(hp, ldh, gate_off, gamma, stats, dg, ldg, dhp, g_gamma, M, inner, inner_pad, d);
+  else if (nch <= 1) geglu_ln_bwd_kernel<1, 256, DROPOUT><<<grid, FF_THREADS, 0, stream>>>(hp, ldh, gate_off, gamma, stats, dg, ldg, dhp, g_gamma, M, inner, inner_pad, d);
+  else if (nch == 2) geglu_ln_bwd_kernel<2, 256, DROPOUT><<<grid, FF_THREADS, 0, stream>>>(hp, ldh, gate_off, gamma, stats, dg, ldg, dhp, g_gamma, M, inner, inner_pad, d);
+  else geglu_ln_bwd_kernel<4, 256, DROPOUT><<<grid, FF_THREADS, 0, stream>>>(hp, ldh, gate_off, gamma, stats, dg, ldg, dhp, g_gamma, M, inner, inner_pad, d);
+}
+
 extern "C" int alm_geglu_ln_bwd(const void* h, int64_t ldh, int gate_off, const float* gamma, const float* stats,
                                 const void* dgn, int64_t ldg, void* dh, float* g_gamma, int M, int inner,
-                                int inner_pad, alm_stream_t stream_) {
+                                int inner_pad, float dropout_p, uint64_t seed, uint32_t site, alm_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ALM_REQUIRE(M > 0 && inner > 0 && inner_pad >= inner && inner_pad % 8 == 0, ALM_ERR_ARG);
+  ALM_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, ALM_ERR_ARG);
   ALM_REQUIRE(ldh % 8 == 0 && ldg % 8 == 0 && gate_off % 8 == 0, ALM_ERR_ALIGN);
   const int nch = ceil_div(inner_pad / 8, FF_THREADS);
   ALM_REQUIRE(nch <= FF_MAX_CHUNKS, ALM_ERR_UNSUPPORTED);
@@ -571,18 +678,12 @@ extern "C" int alm_geglu_ln_bwd(const void* h, int64_t ldh, int gate_off, const 
   auto* dg = (const __nv_bfloat16*)dgn;
   auto* dhp = (__nv_bfloat16*)dh;
   static const int bwd_threads = getenv("ALM_GEGLU_BWD_THREADS") ? atoi(getenv("ALM_GEGLU_BWD_THREADS")) : 512;
-  if (bwd_threads == 512 && inner_pad > 2048 && inner_pad <= 4096) {
-    // one 8-column chunk per thread: half the registers of the 256-thread layout -> 2 x 512 threads per SM
-    const int grid = min(M, num_sms() * 2);
-    geglu_ln_bwd_kernel<1, 512><<<grid, 512, 0, stream>>>(hp, ldh, gate_off, gamma, stats, dg, ldg, dhp, g_gamma, M, inner, inner_pad);
-    ALM_CHECK_LAUNCH();
-    ALM_LAUNCHED(1);
-    return ALM_OK;
-  }
-  const int grid = min(M, num_sms() * 4);
-  if (nch <= 1) geglu_ln_bwd_kernel<1, 256><<<grid, FF_THREADS, 0, stream>>>(hp, ldh, gate_off, gamma, stats, dg, ldg, dhp, g_gamma, M, inner, inner_pad);
-  else if (nch == 2) geglu_ln_bwd_kernel<2, 256><<<grid, FF_THREADS, 0, stream>>>(hp, ldh, gate_off, gamma, stats, dg, ldg, dhp, g_gamma, M, inner, inner_pad);
-  else geglu_ln_bwd_kernel<4, 256><<<grid, FF_THREADS, 0, stream>>>(hp, ldh, gate_off, gamma, stats, dg, ldg, dhp, g_gamma, M, inner, inner_pad);
+  // 512 threads: one 8-column chunk per thread: half the registers of the 256-thread layout -> 2 x 512 threads per SM
+  const int threads = bwd_threads == 512 && inner_pad > 2048 && inner_pad <= 4096 ? 512 : 256;
+  const int grid = min(M, num_sms() * (threads == 512 ? 2 : 4));
+  const DropoutArgs d = make_dropout_args(dropout_p, seed, site);
+  if (dropout_p > 0.f) launch_geglu_ln_bwd<true>(nch, threads, grid, stream, hp, ldh, gate_off, gamma, stats, dg, ldg, dhp, g_gamma, M, inner, inner_pad, d);
+  else launch_geglu_ln_bwd<false>(nch, threads, grid, stream, hp, ldh, gate_off, gamma, stats, dg, ldg, dhp, g_gamma, M, inner, inner_pad, d);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);
   return ALM_OK;

@@ -181,13 +181,39 @@ def pack_key_mask(key_mask):
     return PackedKeyMask(bits, n_k)
 
 
-def mqa_attn_fwd(q, k, v, *, heads, key_mask=None, causal=True, scale=None, return_lse=True, bias=None):
+def _drop_args(dropout):
+    """(p, seed, site) or None -> the (dropout_p, seed, site) C arguments; p == 0 selects the dropout-free kernels."""
+    if dropout is None:
+        return 0.0, 0, 0
+    p, seed, site = dropout
+    if not 0.0 <= p < 1.0:
+        raise ValueError(f"dropout probability must be in [0, 1), got {p}")
+    return float(p), int(seed) & 0xFFFFFFFFFFFFFFFF, int(site) & 0xFFFFFFFF
+
+
+def dropout_(x, p, seed, site):
+    """In place: x[r, c] = keep(seed, site, r, c) ? x[r, c] / (1 - p) : 0 for a bf16 [M, C] tensor (C % 8 == 0,
+    unit column stride).  The mask is a pure function of (seed, site, r, c), so calling it again on the gradient with
+    the same arguments is the backward."""
+    _check_cuda(x)
+    assert x.dtype == bf16 and x.dim() == 2 and x.stride(1) == 1
+    M, C = x.shape
+    with _timed("dropout_bf16", M * C * 4, "byte"):
+        _lib.call("alm_dropout_bf16", x, x.stride(0), M, C, *_drop_args((p, seed, site)))
+    return x
+
+
+def mqa_attn_fwd(q, k, v, *, heads, key_mask=None, causal=True, scale=None, return_lse=True, bias=None,
+                 dropout=None):
     """Multi-query attention forward (attend.py:69-146).
 
     q: [b, n_q, heads*64] bf16 (last dim contiguous; may be a column slice of a wider buffer)
     k, v: [b, n_k, 64] bf16 (one shared head);  key_mask: [b, n_k] bool/uint8 (True = attend) or None.
     Queries are right-aligned against keys (query i sees keys <= i + n_k - n_q) when causal.
     bias: optional fp32 [heads, n_q, >=n_k] additive score bias shared by the batch (attend.py:122-124).
+    dropout: optional (p, seed, site): dropout on the attention probabilities (attend.py:139-140); the mask element
+    of (batch, head, query i, key j) is keep(seed, site, (batch*heads + head) * n_q_pad + i, j), n_q_pad = n_q
+    rounded up to 128.  The returned lse is that of the un-dropped probabilities.
     Returns o [b, n_q, heads*64] bf16 and lse [b, heads, n_q] fp32.
     """
     _check_cuda(q, k, v, bias)
@@ -214,12 +240,15 @@ def mqa_attn_fwd(q, k, v, *, heads, key_mask=None, causal=True, scale=None, retu
             "alm_mqa_attn_fwd",
             q, q.stride(1), k, k.stride(1), k.stride(0), v, v.stride(1), v.stride(0), key_mask,
             o, o.stride(1), lse, n_q_pad, bias, bhs, brs, b, heads, n_q, n_k, int(causal), float(scale),
+            *_drop_args(dropout),
         )
     return o, lse
 
 
-def mqa_attn_bwd(q, k, v, o, d_o, lse, *, heads, key_mask=None, causal=True, scale=None, bias=None, dbias=None):
+def mqa_attn_bwd(q, k, v, o, d_o, lse, *, heads, key_mask=None, causal=True, scale=None, bias=None, dbias=None,
+                 dropout=None):
     """Backward of mqa_attn_fwd: returns dq [b,n_q,h*64], dk [b,n_k,64], dv [b,n_k,64] (bf16).
+    dropout: the (p, seed, site) of the forward call; its mask is regenerated.
 
     lse is the padded [b, heads, n_q_pad] tensor returned by the forward.  With a bias, d(bias) is ACCUMULATED
     into `dbias` (fp32, same shape/strides as `bias`; the caller zeroes it once per step).
@@ -252,7 +281,7 @@ def mqa_attn_bwd(q, k, v, o, d_o, lse, *, heads, key_mask=None, causal=True, sca
             "alm_mqa_attn_bwd",
             q, q.stride(1), k, k.stride(1), k.stride(0), v, v.stride(1), v.stride(0), d_o, d_o.stride(1), key_mask,
             lse, delta, n_q_pad, dq, dq.stride(1), dq_acc, dk, dk.stride(1), dv, dv.stride(1),
-            bias, dbias, bhs, brs, b, heads, n_q, n_k, int(causal), float(scale),
+            bias, dbias, bhs, brs, b, heads, n_q, n_k, int(causal), float(scale), *_drop_args(dropout),
         )
     return dq, dk, dv
 
@@ -482,23 +511,26 @@ def hc_post_bwd(R_in, Y, beta_prev, ln_gamma, stats, dout, g_ln_gamma, *, M, d, 
     return dR_in, dY, dbp
 
 
-def geglu_ln_fwd(h, gamma, *, inner, inner_pad):
-    """h [M, 2*inner_pad] bf16 (a | gate) -> gn [M, inner_pad] bf16 = LN(gelu(gate)*a)*gamma, stats [M,2]."""
+def geglu_ln_fwd(h, gamma, *, inner, inner_pad, dropout=None):
+    """h [M, 2*inner_pad] bf16 (a | gate) -> gn [M, inner_pad] bf16 = LN(gelu(gate)*a)*gamma, stats [M,2].
+    dropout: optional (p, seed, site): gn is returned dropped, mask keep(seed, site, row, channel)."""
     M = h.shape[0]
     gn = torch.empty(M, inner_pad, device=h.device, dtype=bf16)
     stats = torch.empty(M, 2, device=h.device, dtype=f32)
     with _timed("geglu_ln_fwd", M * inner_pad * 6, "byte"):
-        _lib.call("alm_geglu_ln_fwd", h, h.stride(0), inner_pad, gamma, gn, gn.stride(0), stats, M, inner, inner_pad)
+        _lib.call("alm_geglu_ln_fwd", h, h.stride(0), inner_pad, gamma, gn, gn.stride(0), stats, M, inner, inner_pad,
+                  *_drop_args(dropout))
     return gn, stats
 
 
-def geglu_ln_bwd(h, gamma, stats, dgn, g_gamma, *, inner, inner_pad):
+def geglu_ln_bwd(h, gamma, stats, dgn, g_gamma, *, inner, inner_pad, dropout=None):
+    """dropout: the (p, seed, site) of the forward; the mask is applied to dgn first."""
     M = h.shape[0]
     dh = torch.empty_like(h)
     assert dh.stride(0) == h.stride(0)
     with _timed("geglu_ln_bwd", M * inner_pad * 10, "byte"):
         _lib.call("alm_geglu_ln_bwd", h, h.stride(0), inner_pad, gamma, stats, dgn, dgn.stride(0), dh, g_gamma, M,
-                  inner, inner_pad)
+                  inner, inner_pad, *_drop_args(dropout))
     return dh
 
 

@@ -33,6 +33,17 @@ def _pad8(n: int) -> int:
     return (n + 7) // 8 * 8
 
 
+def _check_dropout(p, name="dropout"):
+    if not 0.0 <= float(p) < 1.0:
+        raise ValueError(f"{name} must be in [0, 1), got {p}")
+
+
+def _draw_dropout_seed() -> int:
+    """one 63-bit seed from torch's default CPU generator: `torch.manual_seed` reproduces a step, and drawing it
+    needs no device synchronisation."""
+    return int(torch.randint(0, 2 ** 63 - 1, (), dtype=torch.int64))
+
+
 # ----------------------------------------------------------------------------------------------
 # parameter containers (same attribute names -> same state_dict keys as the reference)
 # ----------------------------------------------------------------------------------------------
@@ -50,6 +61,7 @@ class Attend(nn.Module):
 
     def __init__(self, dropout=0.0, causal=False, flash=False):
         super().__init__()
+        _check_dropout(dropout)
         self.dropout = dropout
         self.causal = causal
         self.flash = flash
@@ -62,8 +74,9 @@ class Attend(nn.Module):
             from .rel_pos import as_kernel_bias
             attn_bias = as_kernel_bias(attn_bias.detach())
         qf = q.permute(0, 2, 1, 3).reshape(b, n, h * d).to(bf16).contiguous()
+        drop = (self.dropout, _draw_dropout_seed(), 0) if self.training and self.dropout > 0 else None
         o, _ = ops.mqa_attn_fwd(qf, k.to(bf16).contiguous(), v.to(bf16).contiguous(), heads=h, key_mask=mask,
-                                causal=self.causal, return_lse=False, bias=attn_bias)
+                                causal=self.causal, return_lse=False, bias=attn_bias, dropout=drop)
         return o.reshape(b, n, h, d).permute(0, 2, 1, 3)
 
 
@@ -89,15 +102,17 @@ class Attention(nn.Module):
 
 class FeedForward(nn.Module):
     """audiolm_pytorch.py:251-260 with the reference's Sequential indices as attribute names
-    (0: LayerNorm, 1: Linear(d, 2*inner), 3: LayerNorm(inner), 5: Linear(inner, d))."""
+    (0: LayerNorm, 1: Linear(d, 2*inner), 3: LayerNorm(inner), 4: Dropout, 5: Linear(inner, d))."""
 
     def __init__(self, dim, mult=4, dropout=0.1):
         super().__init__()
+        _check_dropout(dropout)
         inner = int(dim * 2 * mult / 3)
         self.inner = inner
         self.add_module("0", LayerNorm(dim))
         self.add_module("1", nn.Linear(dim, inner * 2, bias=False))
         self.add_module("3", LayerNorm(inner))
+        self.add_module("4", nn.Dropout(dropout))
         self.add_module("5", nn.Linear(inner, dim, bias=False))
 
 
@@ -214,8 +229,8 @@ class _StackFn(torch.autograd.Function):
     """Whole Transformer stack as one autograd node: explicit forward + backward over C-ABI kernels."""
 
     @staticmethod
-    def forward(ctx, tr, x, mask, bias, *params):
-        out, saved = tr._run_forward(x, mask, bias, save=any(ctx.needs_input_grad))
+    def forward(ctx, tr, x, mask, bias, drop, *params):
+        out, saved = tr._run_forward(x, mask, bias, save=any(ctx.needs_input_grad), drop=drop)
         ctx.tr = tr
         ctx.saved = saved
         ctx.bias_grad = bias is not None and ctx.needs_input_grad[3]
@@ -232,7 +247,7 @@ class _StackFn(torch.autograd.Function):
         dx, grads = tr._run_backward(S, dout)
         dbias = S["dbias"]
         ctx.saved = None
-        return (None, dx, None, dbias, *grads)
+        return (None, dx, None, dbias, None, *grads)
 
 
 def _grad_targets(params, direct_ok=False):
@@ -270,8 +285,8 @@ class Transformer(nn.Module):
             raise NotImplementedError("text / audio conditioning is outside the accelerated hot path")
         if num_residual_streams not in (1, 4):
             raise NotImplementedError("residual-stream kernels are built for num_residual_streams in (1, 4)")
-        if attn_dropout != 0.0 or ff_dropout != 0.0:
-            raise NotImplementedError("dropout > 0 is not built (reference default is 0)")
+        _check_dropout(attn_dropout, "attn_dropout")
+        _check_dropout(ff_dropout, "ff_dropout")
         if dim % 8 != 0:
             raise ValueError("dim must be a multiple of 8")
         self.dim = dim
@@ -393,6 +408,20 @@ class Transformer(nn.Module):
             w2=pk.get((i, "w2"), [w2], lambda: pack_plain(w2)),
         )
 
+    # ---- dropout ---------------------------------------------------------------------------------
+    def _dropout_plan(self):
+        """Per layer: (attention probabilities, attention output, feed-forward) dropout as (p, seed, site) or None.
+        None overall in eval mode or when every p is 0: then no seed is drawn and the dropout-free kernels run.
+        One seed per forward; site 3 i + k names layer i's k-th dropout, so every mask is independent."""
+        if not self.training:
+            return None
+        ps = [(a.branch.attend.dropout, a.branch.to_out[1].p, getattr(f.branch, "4").p) for a, _, f in self.layers]
+        if not any(p > 0 for layer in ps for p in layer):
+            return None
+        seed = _draw_dropout_seed()
+        return [tuple((p, seed, 3 * i + k) if p > 0 else None for k, p in enumerate(layer))
+                for i, layer in enumerate(ps)]
+
     # ---- forward -------------------------------------------------------------------------------
     def forward(self, x, self_attn_mask=None, context=None, context_mask=None, attn_bias=None,
                 return_kv_cache=False, kv_cache=None):
@@ -406,22 +435,23 @@ class Transformer(nn.Module):
         if exists(bias):
             from .rel_pos import as_kernel_bias
             bias = as_kernel_bias(bias)
+        drop = self._dropout_plan()
         if exists(kv_cache):
             if exists(bias):
                 bias = bias[:, kv_cache.shape[-2]:, :]
-            out, kv = self._forward_cached(x, self_attn_mask, kv_cache, bias)
+            out, kv = self._forward_cached(x, self_attn_mask, kv_cache, bias, drop)
         else:
             # the [depth, 2, b, n, 64] cache tensor is only materialised when the caller asks for it (a training
             # step does not: stacking it costs six strided copies per forward)
             self._want_kv = bool(return_kv_cache)
-            out, kv = _StackFn.apply(self, x, self_attn_mask, bias, *self._param_list())
+            out, kv = _StackFn.apply(self, x, self_attn_mask, bias, drop, *self._param_list())
         if not return_kv_cache:
             return out
         return out, kv
 
-    def _run_forward(self, x, mask, bias, save):
+    def _run_forward(self, x, mask, bias, save, drop=None):
         if self.num_residual_streams == 1:
-            return self._run_forward_plain(x, mask, bias, save)
+            return self._run_forward_plain(x, mask, bias, save, drop=drop)
         b, n, d = x.shape
         M = b * n
         H = self.heads
@@ -436,6 +466,7 @@ class Transformer(nn.Module):
             W = self._weights(i)
             f = ff_hc.branch
             inner, ip = f.inner, _pad8(f.inner)
+            d_attn, d_out, d_ff = drop[i] if drop else (None, None, None)
             rec = dict(R_a=R, bin_a=bin_, xn_a=xn, beta_a=beta, aux_a=aux)
             q = ops.gemm(xn, W["wq"])                      # [M, H*64]
             kv = ops.gemm(bin_, W["wkv"])                  # [M, 128]  (k | v) from the UN-normalised input
@@ -445,15 +476,18 @@ class Transformer(nn.Module):
                 v_first = kv[:, 64:].clone()               # layer-0 values before any mixing (:355-358)
             k3 = kv[:, :64].unflatten(0, (b, n))
             v3 = kv[:, 64:].unflatten(0, (b, n))
-            o, lse = ops.mqa_attn_fwd(q.view(b, n, H * 64), k3, v3, heads=H, key_mask=mask_u8, causal=True, bias=bias)
+            o, lse = ops.mqa_attn_fwd(q.view(b, n, H * 64), k3, v3, heads=H, key_mask=mask_u8, causal=True, bias=bias,
+                                      dropout=d_attn)
             o2 = o.view(M, H * 64)
             Y = ops.gemm(o2, W["wo"])
+            if d_out:
+                ops.dropout_(Y, *d_out)
             rec.update(q=q, kv=kv, o=o2, lse=lse, Y_a=Y)
             kvs.append(kv)
             R2, bin2, xn2, beta2, aux2 = ops.hc_pre_fwd(ff_hc.kernel_params(), getattr(f, "0").gamma, R_in=R, Y=Y,
                                                         beta_prev=beta, M=M, d=d)
             h = ops.gemm(xn2, W["w1"])                     # [M, 2*ip]
-            gn, st = ops.geglu_ln_fwd(h, getattr(f, "3").gamma, inner=inner, inner_pad=ip)
+            gn, st = ops.geglu_ln_fwd(h, getattr(f, "3").gamma, inner=inner, inner_pad=ip, dropout=d_ff)
             Y2 = ops.gemm(gn, W["w2"])
             rec.update(R_f=R2, xn_f=xn2, beta_f=beta2, aux_f=aux2, h=h, gn=gn, st=st, Y_f=Y2)
             L.append(rec)
@@ -470,7 +504,7 @@ class Transformer(nn.Module):
             kv_t = torch.empty(0, device=x.device, dtype=bf16)
         saved = dict(kv=kv_t)
         if save:
-            saved.update(L=L, x2=x2, mask=mask_u8, bias=bias, stats=stats, shape=(b, n, d), x_dtype=x.dtype)
+            saved.update(L=L, x2=x2, mask=mask_u8, bias=bias, stats=stats, shape=(b, n, d), x_dtype=x.dtype, drop=drop)
         return out.view(b, n, d), saved
 
     # ---- backward ------------------------------------------------------------------------------
@@ -508,10 +542,12 @@ class Transformer(nn.Module):
             W = self._weights(i)
             rec = L[i]
             a_hc, g_ln_a, g_wq, g_wkv, g_wo, f_hc, g_ln_f, g_w1, g_ln2, g_w2 = slot(i)
+            d_attn, d_out, d_ff = S["drop"][i] if S["drop"] else (None, None, None)
             # ---- feed-forward branch ----
             dgn = ops.gemm(dY, W["w2"], b_mn=True)                       # [M, ip]
             _wgrad_cols(dY, rec["gn"], g_w2, inner)
-            dh = ops.geglu_ln_bwd(rec["h"], getattr(f, "3").gamma, rec["st"], dgn, g_ln2, inner=inner, inner_pad=ip)
+            dh = ops.geglu_ln_bwd(rec["h"], getattr(f, "3").gamma, rec["st"], dgn, g_ln2, inner=inner, inner_pad=ip,
+                                  dropout=d_ff)
             dxn_f = ops.gemm(dh, W["w1"], b_mn=True)                     # [M, d]
             wgrad(dh[:, :inner], rec["xn_f"], g_w1[:inner])
             wgrad(dh[:, ip:ip + inner], rec["xn_f"], g_w1[inner:])
@@ -519,6 +555,8 @@ class Transformer(nn.Module):
                                                  rec["aux_f"], dR, dxn_f, dbeta, R_in=rec["R_a"], Y=rec["Y_a"],
                                                  beta_prev=rec["beta_a"], M=M, d=d)
             # ---- attention branch ----
+            if d_out:
+                ops.dropout_(dY_a, *d_out)
             dO = ops.gemm(dY_a, W["wo"], b_mn=True)                      # [M, H*64]
             wgrad(dY_a, rec["o"], g_wo)
             kv = rec["kv"]
@@ -526,7 +564,7 @@ class Transformer(nn.Module):
             v3 = kv[:, 64:].unflatten(0, (b, n))
             dq, dk, dv = ops.mqa_attn_bwd(rec["q"].view(b, n, H * 64), k3, v3, rec["o"].view(b, n, H * 64),
                                           dO.view(b, n, H * 64), rec["lse"], heads=H, key_mask=S["mask"], causal=True,
-                                          bias=S["bias"], dbias=S["dbias"])
+                                          bias=S["bias"], dbias=S["dbias"], dropout=d_attn)
             dkv = torch.empty(M, 128, device=dev, dtype=bf16)
             ops.axpby(dk.view(M, 64), 1.0, None, 0.0, out=dkv[:, :64])
             dv2 = dv.view(M, 64)
@@ -557,8 +595,8 @@ class Transformer(nn.Module):
 
 
     # ---- num_residual_streams == 1: plain residual stream (fp32) ---------------------------------
-    def _attn_branch_fwd(self, i, xn, raw, b, n, mask_u8, v_first, cache=None, bias=None):
-        """q/kv projections, value residual, (optional KV cache), attention, output projection."""
+    def _attn_branch_fwd(self, i, xn, raw, b, n, mask_u8, v_first, cache=None, bias=None, d_attn=None, d_out=None):
+        """q/kv projections, value residual, (optional KV cache), attention, output projection (+ their dropout)."""
         H = self.heads
         W = self._weights(i)
         M = b * n
@@ -573,12 +611,15 @@ class Transformer(nn.Module):
         if cache is not None:
             k3 = torch.cat((cache[0].to(bf16), k3), dim=1).contiguous()
             v3 = torch.cat((cache[1].to(bf16), v3), dim=1).contiguous()
-        o, lse = ops.mqa_attn_fwd(q.view(b, n, H * 64), k3, v3, heads=H, key_mask=mask_u8, causal=True, bias=bias)
+        o, lse = ops.mqa_attn_fwd(q.view(b, n, H * 64), k3, v3, heads=H, key_mask=mask_u8, causal=True, bias=bias,
+                                  dropout=d_attn)
         o2 = o.view(M, H * 64)
         Y = ops.gemm(o2, W["wo"])
+        if d_out:
+            ops.dropout_(Y, *d_out)
         return q, kv, o2, lse, Y, v_first, torch.stack((k3, v3))
 
-    def _run_forward_plain(self, x, mask, bias, save, kv_cache=None):
+    def _run_forward_plain(self, x, mask, bias, save, kv_cache=None, drop=None):
         b, n, d = x.shape
         M = b * n
         r = x.detach().reshape(M, d).to(f32).contiguous()
@@ -592,12 +633,13 @@ class Transformer(nn.Module):
             a, f = attn_w.branch, ff_w.branch
             W = self._weights(i)
             inner, ip = f.inner, _pad8(f.inner)
+            d_attn, d_out, d_ff = drop[i] if drop else (None, None, None)
             q, kv, o2, lse, Y, v_first, kv_t = self._attn_branch_fwd(
-                i, xn, raw, b, n, mask_u8, v_first, None if kv_cache is None else kv_cache[i], bias)
+                i, xn, raw, b, n, mask_u8, v_first, None if kv_cache is None else kv_cache[i], bias, d_attn, d_out)
             kvs.append(kv_t)
             r_f, xn_f, _, st_f = ops.resid_ln_fwd(r, Y, getattr(f, "0").gamma)
             h = ops.gemm(xn_f, W["w1"])
-            gn, stg = ops.geglu_ln_fwd(h, getattr(f, "3").gamma, inner=inner, inner_pad=ip)
+            gn, stg = ops.geglu_ln_fwd(h, getattr(f, "3").gamma, inner=inner, inner_pad=ip, dropout=d_ff)
             Y2 = ops.gemm(gn, W["w2"])
             L.append(dict(r_a=r, st_a=st, xn_a=xn, raw_a=raw, q=q, kv=kv, o=o2, lse=lse, r_f=r_f, st_f=st_f, xn_f=xn_f,
                           h=h, gn=gn, stg=stg))
@@ -608,7 +650,7 @@ class Transformer(nn.Module):
         saved = dict(kv=torch.stack(kvs))
         if save:
             saved.update(L=L, mask=mask_u8, bias=bias, r_last=r_last, st_last=st_last, shape=(b, n, d),
-                         x_dtype=x.dtype)
+                         x_dtype=x.dtype, drop=drop)
         return out.view(b, n, d), saved
 
     def _run_backward_plain(self, S, dout):
@@ -629,15 +671,19 @@ class Transformer(nn.Module):
             W = self._weights(i)
             rec = L[i]
             g_ln_a, g_wq, g_wkv, g_wo, g_ln_f, g_w1, g_ln2, g_w2 = grads[i * 8:(i + 1) * 8]
+            d_attn, d_out, d_ff = S["drop"][i] if S["drop"] else (None, None, None)
             # feed-forward branch (its output gradient is the residual-stream gradient)
             dgn = ops.gemm(dr_b, W["w2"], b_mn=True)
             _wgrad_cols(dr_b, rec["gn"], g_w2, inner)
-            dh = ops.geglu_ln_bwd(rec["h"], getattr(f, "3").gamma, rec["stg"], dgn, g_ln2, inner=inner, inner_pad=ip)
+            dh = ops.geglu_ln_bwd(rec["h"], getattr(f, "3").gamma, rec["stg"], dgn, g_ln2, inner=inner, inner_pad=ip,
+                                  dropout=d_ff)
             dxn_f = ops.gemm(dh, W["w1"], b_mn=True)
             wgrad(dh[:, :inner], rec["xn_f"], g_w1[:inner])
             wgrad(dh[:, ip:ip + inner], rec["xn_f"], g_w1[inner:])
             dr, dr_b = ops.resid_ln_bwd(rec["r_f"], getattr(f, "0").gamma, rec["st_f"], dr, dxn_f, None, g_ln_f)
             # attention branch
+            if d_out:
+                ops.dropout_(dr_b, *d_out)  # dr_b is read by nothing else
             dO = ops.gemm(dr_b, W["wo"], b_mn=True)
             wgrad(dr_b, rec["o"], g_wo)
             kv = rec["kv"]
@@ -645,7 +691,7 @@ class Transformer(nn.Module):
             v3 = kv[:, 64:].unflatten(0, (b, n))
             dq, dk, dv = ops.mqa_attn_bwd(rec["q"].view(b, n, H * 64), k3, v3, rec["o"].view(b, n, H * 64),
                                           dO.view(b, n, H * 64), rec["lse"], heads=H, key_mask=S["mask"], causal=True,
-                                          bias=S["bias"], dbias=S["dbias"])
+                                          bias=S["bias"], dbias=S["dbias"], dropout=d_attn)
             dkv = torch.empty(M, 128, device=dev, dtype=bf16)
             ops.axpby(dk.view(M, 64), 1.0, None, 0.0, out=dkv[:, :64])
             dv2 = dv.view(M, 64)
@@ -667,12 +713,12 @@ class Transformer(nn.Module):
 
     # ---- incremental (KV-cache) inference ------------------------------------------------------
     @torch.no_grad()
-    def _forward_cached(self, x, mask, kv_cache, bias=None):
+    def _forward_cached(self, x, mask, kv_cache, bias=None, drop=None):
         """x is the FULL sequence; only x[:, cache_len:] is processed (audiolm_pytorch.py:489-496)."""
         cache_len = kv_cache.shape[-2]
         x = x[:, cache_len:]
         if self.num_residual_streams == 1:
-            out, saved = self._run_forward_plain(x, mask, bias, save=False, kv_cache=kv_cache)
+            out, saved = self._run_forward_plain(x, mask, bias, save=False, kv_cache=kv_cache, drop=drop)
             return out, saved["kv"]
         b, n, d = x.shape
         M = b * n
@@ -687,6 +733,7 @@ class Transformer(nn.Module):
             W = self._weights(i)
             f = ff_hc.branch
             inner, ip = f.inner, _pad8(f.inner)
+            d_attn, d_out, d_ff = drop[i] if drop else (None, None, None)
             q = ops.gemm(xn, W["wq"])
             kv = ops.gemm(bin_, W["wkv"])
             if self.add_value_residual and v_first is not None:
@@ -698,12 +745,14 @@ class Transformer(nn.Module):
             v_all = torch.cat((cv, kv[:, 64:].unflatten(0, (b, n))), dim=1).contiguous()
             new_cache.append(torch.stack((k_all, v_all)))
             o, _ = ops.mqa_attn_fwd(q.view(b, n, H * 64), k_all, v_all, heads=H, key_mask=mask_u8, causal=True,
-                                    return_lse=False, bias=bias)
+                                    return_lse=False, bias=bias, dropout=d_attn)
             Y = ops.gemm(o.view(M, H * 64), W["wo"])
+            if d_out:
+                ops.dropout_(Y, *d_out)
             R2, _, xn2, beta2, _ = ops.hc_pre_fwd(ff_hc.kernel_params(), getattr(f, "0").gamma, R_in=R, Y=Y,
                                                   beta_prev=beta, M=M, d=d)
             h = ops.gemm(xn2, W["w1"])
-            gn, _ = ops.geglu_ln_fwd(h, getattr(f, "3").gamma, inner=inner, inner_pad=ip)
+            gn, _ = ops.geglu_ln_fwd(h, getattr(f, "3").gamma, inner=inner, inner_pad=ip, dropout=d_ff)
             Y2 = ops.gemm(gn, W["w2"])
             if i + 1 < self.depth:
                 nxt = self.layers[i + 1][0]

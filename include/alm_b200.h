@@ -87,11 +87,15 @@ int alm_pack_key_mask(const void* key_mask, void* bits, int b, int n_k, alm_stre
  * RelativePositionBias / cross_attn_bias / pos_bias_mlp (audiolm_pytorch.py:202-242, 926-936, 1229-1298).
  * bias_rstride >= n_k and a multiple of 4; the backward accumulates d(bias) into dbias (same layout) with
  * atomic adds - zero it once per step, every layer / batch adds into it.
+ * dropout_p in [0, 1): dropout on the attention probabilities (attend.py:139-140), applied to P before P V with the
+ * mask keep(seed, site, (b*h + head) * n_q_pad + i, j), n_q_pad = n_q rounded up to 128 (see alm_dropout_bf16).
+ * The LSE is that of the un-dropped probabilities.  dropout_p == 0 runs the dropout-free kernels.
  */
 int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int64_t k_bstride, const void* v,
                      int64_t ldv, int64_t v_bstride, const void* key_mask, void* o, int64_t ldo, float* lse,
                      int64_t lse_stride, const float* bias, int64_t bias_hstride, int64_t bias_rstride, int b, int h,
-                     int n_q, int n_k, int causal, float scale, alm_stream_t stream);
+                     int n_q, int n_k, int causal, float scale, float dropout_p, uint64_t seed, uint32_t site,
+                     alm_stream_t stream);
 
 /*
  * Backward of alm_mqa_attn_fwd (one wgmma kernel per (batch, 128-key block): dK/dV accumulate over all heads in
@@ -99,6 +103,8 @@ int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int
  * lse/delta are [b, h, n_q_pad] with n_q_pad a multiple of 128; delta = rowsum(dO * O) from alm_attn_delta.
  * dq_acc is an fp32 [b, n_q, h*64] contiguous workspace that must be zero on entry (alm_attn_delta zeroes it).
  * dq is summed with fp32 atomics, so it is not bitwise reproducible from run to run; dk and dv are.
+ * dropout_p / seed / site: those of the forward call (the mask is regenerated, not stored); with dropout_p > 0,
+ * n_q_pad must be n_q rounded up to 128.
  * Autograd of attend.py:69-146.
  */
 int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int64_t k_bstride, const void* v,
@@ -106,7 +112,7 @@ int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int
                      const float* lse, const float* delta, int n_q_pad, void* dq, int64_t lddq, float* dq_acc,
                      void* dk, int64_t lddk, void* dv, int64_t lddv, const float* bias, float* dbias,
                      int64_t bias_hstride, int64_t bias_rstride, int b, int h, int n_q, int n_k, int causal,
-                     float scale, alm_stream_t stream);
+                     float scale, float dropout_p, uint64_t seed, uint32_t site, alm_stream_t stream);
 /* delta[b, h, i] = rowsum(dO * O); also zeroes dq_acc ([b, n, h*64] fp32, contiguous) unless it is null */
 int alm_attn_delta(const void* o, int64_t ldo, const void* d_o, int64_t lddo, float* delta /* [b,h,stride] */,
                    int64_t delta_stride, float* dq_acc, int b, int h, int n, alm_stream_t stream);
@@ -240,11 +246,22 @@ int alm_resid_ln_bwd(const float* r_new, const float* gamma, const float* stats,
 
 /* ---- FeedForward inner part: GEGLU + LayerNorm(inner) (audiolm_pytorch.py:246-258) -------------- */
 /* h [M, ldh] bf16 holds a = h[:, 0:inner] and gate = h[:, gate_off:gate_off+inner];
- * gn[M, ldg] = LN(gelu(gate) * a) * gamma, columns [inner, inner_pad) are written as zeros. */
+ * gn[M, ldg] = LN(gelu(gate) * a) * gamma, columns [inner, inner_pad) are written as zeros.
+ * dropout_p in [0, 1): the FeedForward dropout after the inner LayerNorm (audiolm_pytorch.py:256), mask
+ * keep(seed, site, row, channel); gn holds the dropped values.  The backward applies the same mask to dgn. */
 int alm_geglu_ln_fwd(const void* h, int64_t ldh, int gate_off, const float* gamma, void* gn, int64_t ldg,
-                     float* stats, int M, int inner, int inner_pad, alm_stream_t stream);
+                     float* stats, int M, int inner, int inner_pad, float dropout_p, uint64_t seed, uint32_t site,
+                     alm_stream_t stream);
 int alm_geglu_ln_bwd(const void* h, int64_t ldh, int gate_off, const float* gamma, const float* stats,
                      const void* dgn, int64_t ldg, void* dh, float* g_gamma, int M, int inner, int inner_pad,
+                     float dropout_p, uint64_t seed, uint32_t site, alm_stream_t stream);
+
+/* In-place dropout of a bf16 [M, C] tensor (row stride ld; C, ld multiples of 8, x 16-B aligned):
+ * x[r, c] = keep(seed, site, r, c) ? x[r, c] / (1 - p) : 0, rounded to bf16.  keep() is the counter-based
+ * (Philox4x32-10) mask every dropout kernel of the library uses (csrc/alm_common.cuh), so the same call on the
+ * gradient is the backward, and on a tensor of ones of shape [b*h*n_q_pad, n_k] it yields the attention mask.
+ * Used for the attention-branch output (audiolm_pytorch.py:302-305).  0 <= p < 1. */
+int alm_dropout_bf16(void* x, int64_t ld, int64_t M, int C, float p, uint64_t seed, uint32_t site,
                      alm_stream_t stream);
 
 /* ---- cross entropy with ignore_index, fused forward + d(logits) --------------------------------- */

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Stand-alone timings of the HBM-bound row kernels, attention and every wgmma GEMM shape at C3 sizes (CUDA events,
 L2 flushed between iterations).
-usage: python tools/bench_kernels.py [geglu] [hc] [attn] [gemm] ..."""
+usage: python tools/bench_kernels.py [geglu] [hc] [attn] [gemm] [dropout] ..."""
 import sys
 from pathlib import Path
 
@@ -106,3 +106,44 @@ if "gemm" in which:
                lambda a=a, b=b, out=out, s=s: ops.gemm(a, b, a_mn=True, b_mn=True, out=out,
                                                         acc_mode=2 if s > 1 else 1, split_k=s),
                flops=2.0 * m * n * k)
+
+if "dropout" in which:
+    # every dropout site of a C3 layer with p = 0.1 against p = 0 (the dropout-free kernels), then a C3-shaped
+    # training step of the Transformer stack (dim 1024, depth 6, 8 heads, 4 streams, batch 16 x 2048)
+    from audiolm_pytorch_b200.transformer import Transformer
+
+    q, k, v = rnd(16, 2048, 512), rnd(16, 2048, 64), rnd(16, 2048, 64)
+    do = rnd(16, 2048, 512)
+    ip = 2736
+    h = rnd(M, 2 * ip)
+    g = rnd(2730, dt=f32)
+    dgn = rnd(M, ip)
+    gg = torch.zeros_like(g)
+    y = rnd(M, d)
+    for p in (0.0, 0.1):
+        drop = (p, 12345, 1) if p > 0 else None
+        timeit(f"p={p} attn fwd", lambda: ops.mqa_attn_fwd(q, k, v, heads=8, dropout=drop))
+        o, lse = ops.mqa_attn_fwd(q, k, v, heads=8, dropout=drop)
+        timeit(f"p={p} attn bwd (delta + fused + dq)", lambda: ops.mqa_attn_bwd(q, k, v, o, do, lse, heads=8, dropout=drop))
+        timeit(f"p={p} geglu_ln_fwd", lambda: ops.geglu_ln_fwd(h, g, inner=2730, inner_pad=ip, dropout=drop),
+               nbytes=M * ip * 6)
+        _, st = ops.geglu_ln_fwd(h, g, inner=2730, inner_pad=ip, dropout=drop)
+        timeit(f"p={p} geglu_ln_bwd", lambda: ops.geglu_ln_bwd(h, g, st, dgn, gg, inner=2730, inner_pad=ip, dropout=drop),
+               nbytes=M * ip * 10)
+        if p > 0:
+            timeit(f"p={p} output dropout [M, {d}] in place", lambda: ops.dropout_(y, p, 12345, 2), nbytes=M * d * 4)
+    del q, k, v, do, h, dgn, y
+    x = torch.randn(16, 2048, d, device=dev)
+    steps = {}
+    for p in (0.0, 0.1):
+        torch.manual_seed(0)
+        steps[p] = Transformer(dim=d, depth=6, heads=8, flash_attn=True, attn_dropout=p, ff_dropout=p).to(dev).train()
+
+    def step(tr):
+        for prm in tr.parameters():
+            prm.grad = None
+        tr(x).float().pow(2).mean().backward()
+
+    for rep in range(3):   # alternate the two models
+        for p, tr in steps.items():
+            timeit(f"p={p} C3 stack fwd+bwd (run {rep})", lambda tr=tr: step(tr), iters=5)
