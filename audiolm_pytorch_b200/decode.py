@@ -1,7 +1,7 @@
 """CUDA-graph decode engine for the KV-cache sampling loops (config C5; audiolm_pytorch.py:1406-1511,
 1608-1740, 1896-2039).
 
-The reference (and `Transformer._forward_cached`) re-concatenate the per-layer cache with `torch.cat` every step
+The reference (and `Transformer.forward` with a `kv_cache`) re-concatenate the per-layer cache with `torch.cat` every step
 and launch ~60 kernels + as many torch ops per token from Python, so a token costs host and launch overhead rather
 than GPU work.  Here one decode step
 

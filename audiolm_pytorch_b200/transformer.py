@@ -4,8 +4,13 @@ Class names, constructor kwargs and state_dict keys follow the reference
 (/root/reference/audiolm_pytorch/audiolm_pytorch.py:191-560, attend.py:35-146) so checkpoints load
 unchanged; the arithmetic is one hand-orchestrated forward/backward over the C-ABI kernels:
 
-    per branch:   [hc_pre: depth(prev) + width + LayerNorm]  ->  wgmma GEMMs / attention / GEGLU+LN
-    end of stack: [hc_post: depth + reduce_streams + final LayerNorm]
+    per branch:   [residual step + LayerNorm]  ->  wgmma GEMMs / attention / GEGLU+LN
+    end of stack: [residual exit + final LayerNorm]
+
+One forward walk (`Transformer._walk_forward`) serves training, the no-grad forward and KV-cache inference, and one
+backward walk serves both residual modes.  Only the residual step differs between them: hyper-connections
+(`_HyperStreams`: hc_pre = depth(prev) + width + LayerNorm over a bf16 [M, 4, d] stream, hc_post = depth +
+reduce_streams + final LayerNorm) or the plain residual (`_PlainStream`: resid_ln over an fp32 [M, d] stream).
 
 Activations are bf16 with fp32 accumulation (the reference's bf16-autocast numerics), parameters stay
 fp32 `nn.Parameter`s; padded bf16 operand copies are rebuilt only when a parameter's version changes.
@@ -154,8 +159,8 @@ class PlainResidual(nn.Module):
         super().__init__()
         self.branch = branch
 
-
-HC_KEYS = ("gamma", "dyn_alpha", "dyn_beta", "static_alpha", "static_beta", "alpha_scale", "beta_scale")
+    def kernel_params(self):
+        return {}
 
 
 # ----------------------------------------------------------------------------------------------
@@ -229,12 +234,11 @@ class _StackFn(torch.autograd.Function):
     """Whole Transformer stack as one autograd node: explicit forward + backward over C-ABI kernels."""
 
     @staticmethod
-    def forward(ctx, tr, x, mask, bias, drop, *params):
-        out, saved = tr._run_forward(x, mask, bias, save=any(ctx.needs_input_grad), drop=drop)
+    def forward(ctx, tr, x, mask, bias, drop, want_kv, *params):
+        out, kv, saved = tr._walk_forward(x, mask, bias, drop, save=any(ctx.needs_input_grad), want_kv=want_kv)
         ctx.tr = tr
         ctx.saved = saved
         ctx.bias_grad = bias is not None and ctx.needs_input_grad[3]
-        kv = saved["kv"]
         ctx.mark_non_differentiable(kv)
         return out, kv
 
@@ -244,10 +248,101 @@ class _StackFn(torch.autograd.Function):
         S = ctx.saved
         # d(bias) is accumulated by every layer's attention backward (atomic adds over batches and layers)
         S["dbias"] = torch.zeros_like(S["bias"]) if ctx.bias_grad else None
-        dx, grads = tr._run_backward(S, dout)
+        dx, grads = tr._walk_backward(S, dout)
         dbias = S["dbias"]
         ctx.saved = None
-        return (None, dx, None, dbias, None, *grads)
+        return (None, dx, None, dbias, None, None, *grads)
+
+
+# ----------------------------------------------------------------------------------------------
+# the residual stream: one step before every branch (`enter` before the first), `exit` after the last.  A step adds the
+# previous branch's output Y to the stream and returns the branch input LayerNorm(stream) as `xn` plus the
+# un-normalised input `bin`, which feeds to_kv.  The `*_bwd` methods run the steps backward in reverse order; each
+# returns the gradient of the previous branch's output (`enter_bwd`: of x).  `hc` / `g_hc` are the hyper-connection
+# parameters of the branch's wrapper and their gradient buffers (empty dicts for the plain residual).
+# ----------------------------------------------------------------------------------------------
+class _HyperStreams:
+    """num_residual_streams == 4: a bf16 [M, 4, d] stream; depth (of the previous branch), width and LayerNorm are one
+    hc_pre kernel, which always writes `bin`.  Saves per step its inputs (R, Y, beta) and the kernel's aux state; the
+    exit saves its LN stats."""
+
+    def __init__(self, save):
+        self.saved = [] if save else None
+
+    def _pre(self, inputs, hc, gamma):
+        self.R, bin_, xn, self.beta, aux = ops.hc_pre_fwd(hc, gamma, **inputs, M=self.M, d=self.d)
+        if self.saved is not None:
+            self.saved.append((inputs, aux))
+        return xn, bin_
+
+    def enter(self, x2, hc, gamma):
+        self.M, self.d = x2.shape
+        return self._pre(dict(x_expand=x2), hc, gamma)
+
+    def step(self, Y, hc, gamma, want_bin):
+        return self._pre(dict(R_in=self.R, Y=Y, beta_prev=self.beta), hc, gamma)
+
+    def exit(self, Y, gamma):
+        out, stats = ops.hc_post_fwd(self.R, Y, self.beta, gamma, M=self.M, d=self.d)
+        if self.saved is not None:
+            self.saved.append(((self.R, Y, self.beta), stats))
+        return out
+
+    def exit_bwd(self, gamma, dout, g_gamma):
+        (R, Y, beta), stats = self.saved.pop()
+        self.dR, dY, self.dbeta = ops.hc_post_bwd(R, Y, beta, gamma, stats, dout, g_gamma, M=self.M, d=self.d)
+        return dY
+
+    def _pre_bwd(self, hc, gamma, g_hc, g_gamma, dxn, dbin, **kw):
+        inputs, aux = self.saved.pop()
+        return ops.hc_pre_bwd(hc, gamma, g_hc, g_gamma, aux, self.dR, dxn, self.dbeta, dbin_extra=dbin, **inputs, **kw,
+                              M=self.M, d=self.d)
+
+    def step_bwd(self, hc, gamma, g_hc, g_gamma, dxn, dbin=None):
+        self.dR, dY, self.dbeta = self._pre_bwd(hc, gamma, g_hc, g_gamma, dxn, dbin)
+        return dY
+
+    def enter_bwd(self, hc, gamma, g_hc, g_gamma, dxn, dbin, scale):
+        return self._pre_bwd(hc, gamma, g_hc, g_gamma, dxn, dbin, dx_scale=scale)
+
+
+class _PlainStream:
+    """num_residual_streams == 1: an fp32 [M, d] stream r += Y, then LayerNorm (resid_ln); `bin` is a bf16 copy of r,
+    written only when the branch asks for it.  Saves per step the updated stream and its LN stats."""
+
+    def __init__(self, save):
+        self.saved = [] if save else None
+        self.dr = None
+
+    def _fwd(self, r, Y, gamma, **kw):
+        self.r, xn, raw, st = ops.resid_ln_fwd(r, Y, gamma, **kw)
+        if self.saved is not None:
+            self.saved.append((self.r, st))
+        return xn, raw
+
+    def enter(self, x2, hc, gamma):
+        return self._fwd(x2, None, gamma, want_raw=True)
+
+    def step(self, Y, hc, gamma, want_bin):
+        return self._fwd(self.r, Y, gamma, want_raw=want_bin)
+
+    def exit(self, Y, gamma):
+        return self._fwd(self.r, Y, gamma)[0]
+
+    def _bwd(self, gamma, g_gamma, dxn, dbin, **kw):
+        r, st = self.saved.pop()
+        self.dr, dr_b = ops.resid_ln_bwd(r, gamma, st, self.dr, dxn, dbin, g_gamma, **kw)
+        return dr_b
+
+    def exit_bwd(self, gamma, dout, g_gamma):
+        return self._bwd(gamma, g_gamma, dout, None)
+
+    def step_bwd(self, hc, gamma, g_hc, g_gamma, dxn, dbin=None):
+        return self._bwd(gamma, g_gamma, dxn, dbin)
+
+    def enter_bwd(self, hc, gamma, g_hc, g_gamma, dxn, dbin, scale):
+        self._bwd(gamma, g_gamma, dxn, dbin, out_scale=scale)
+        return self.dr
 
 
 def _grad_targets(params, direct_ok=False):
@@ -328,26 +423,22 @@ class Transformer(nn.Module):
         self._packed.clear()
 
     # ---- parameter plumbing ------------------------------------------------------------------
-    def _param_list(self):
-        if self.num_residual_streams == 1:
-            ps = []
-            for attn_w, _, ff_w in self.layers:
-                a, f = attn_w.branch, ff_w.branch
-                ps += [a.norm.gamma, a.to_q.weight, a.to_kv.weight, a.to_out[0].weight, getattr(f, "0").gamma,
-                       getattr(f, "1").weight, getattr(f, "3").gamma, getattr(f, "5").weight]
-            ps.append(self.norm.gamma)
-            return ps
-        ps = []
-        for attn_hc, _, ff_hc in self.layers:
-            a, f = attn_hc.branch, ff_hc.branch
-            ps += [*attn_hc.kernel_params().values(), a.norm.gamma, a.to_q.weight, a.to_kv.weight,
-                   a.to_out[0].weight]
-            ps += [*ff_hc.kernel_params().values(), getattr(f, "0").gamma, getattr(f, "1").weight,
-                   getattr(f, "3").gamma, getattr(f, "5").weight]
-        ps.append(self.norm.gamma)
-        return ps
+    def _layer_params(self):
+        """Per layer, the parameters the kernels read in four groups: (attention wrapper, attention, feed-forward
+        wrapper, feed-forward).  A wrapper group is its hyper-connection parameters (empty for the plain residual).
+        `_param_list` is these groups in order, then the final LayerNorm; the backward groups the gradients alike."""
+        layout = []
+        for attn_w, _, ff_w in self.layers:
+            a, f = attn_w.branch, ff_w.branch
+            layout.append((attn_w.kernel_params(),
+                           dict(ln=a.norm.gamma, wq=a.to_q.weight, wkv=a.to_kv.weight, wo=a.to_out[0].weight),
+                           ff_w.kernel_params(),
+                           dict(ln=getattr(f, "0").gamma, w1=getattr(f, "1").weight, ln2=getattr(f, "3").gamma,
+                                w2=getattr(f, "5").weight)))
+        return layout
 
-    PER_LAYER = 2 * len(HC_KEYS) + 4 + 4
+    def _param_list(self):
+        return [p for layer in self._layer_params() for group in layer for p in group.values()] + [self.norm.gamma]
 
     def _pack_all(self):
         """re-pack the bf16 operand copies of EVERY Linear of the stack in one launch (alm_cast_pad_multi) whenever a
@@ -437,329 +528,164 @@ class Transformer(nn.Module):
             bias = as_kernel_bias(bias)
         drop = self._dropout_plan()
         if exists(kv_cache):
+            # x is the FULL sequence; only the positions after the cache are processed (audiolm_pytorch.py:489-496)
+            cache_len = kv_cache.shape[-2]
             if exists(bias):
-                bias = bias[:, kv_cache.shape[-2]:, :]
-            out, kv = self._forward_cached(x, self_attn_mask, kv_cache, bias, drop)
+                bias = bias[:, cache_len:, :]
+            with torch.no_grad():
+                out, kv, _ = self._walk_forward(x[:, cache_len:], self_attn_mask, bias, drop, save=False,
+                                                want_kv=return_kv_cache, kv_cache=kv_cache)
         else:
-            # the [depth, 2, b, n, 64] cache tensor is only materialised when the caller asks for it (a training
-            # step does not: stacking it costs six strided copies per forward)
-            self._want_kv = bool(return_kv_cache)
-            out, kv = _StackFn.apply(self, x, self_attn_mask, bias, drop, *self._param_list())
+            out, kv = _StackFn.apply(self, x, self_attn_mask, bias, drop, bool(return_kv_cache), *self._param_list())
         if not return_kv_cache:
             return out
         return out, kv
 
-    def _run_forward(self, x, mask, bias, save, drop=None):
-        if self.num_residual_streams == 1:
-            return self._run_forward_plain(x, mask, bias, save, drop=drop)
+    def _walk_forward(self, x, mask, bias, drop, *, save, want_kv, kv_cache=None):
+        """The stack's forward over the kernels, for both residual modes.  Returns (out, kv, saved):
+        kv is the [depth, 2, b, cache_len + n, 64] cache tensor when `want_kv` (stacking it is a copy a training step
+        does not need), else an empty tensor; `saved` is what `_walk_backward` reads when `save`, else None.
+        `kv_cache`: keys / values of the positions before x."""
         b, n, d = x.shape
         M = b * n
-        H = self.heads
         x2 = x.detach().reshape(M, d).to(f32).contiguous()
-        mask_u8 = ops.pack_key_mask(mask)  # bits, packed once for every layer and the backward
-        L = []
-        hc0 = self.layers[0][0]
-        R, bin_, xn, beta, aux = ops.hc_pre_fwd(hc0.kernel_params(), hc0.branch.norm.gamma, x_expand=x2, M=M, d=d)
-        v_first = None
-        kvs = []
-        for i, (attn_hc, _, ff_hc) in enumerate(self.layers):
+        S = dict(shape=(b, n, d), x_dtype=x.dtype, mask=ops.pack_key_mask(mask),  # bits, packed once for every layer
+                 bias=bias, drop=drop)
+        P = self._layer_params()
+        res = _PlainStream(save) if self.num_residual_streams == 1 else _HyperStreams(save)
+        xn, bin_ = res.enter(x2, P[0][0], P[0][1]["ln"])
+        L, kvs, v_first = [], [], None
+        for i, (_, _, hc_f, p_f) in enumerate(P):
             W = self._weights(i)
-            f = ff_hc.branch
-            inner, ip = f.inner, _pad8(f.inner)
             d_attn, d_out, d_ff = drop[i] if drop else (None, None, None)
-            rec = dict(R_a=R, bin_a=bin_, xn_a=xn, beta_a=beta, aux_a=aux)
-            q = ops.gemm(xn, W["wq"])                      # [M, H*64]
-            kv = ops.gemm(bin_, W["wkv"])                  # [M, 128]  (k | v) from the UN-normalised input
-            if self.add_value_residual and v_first is not None:
-                ops.axpby(kv[:, 64:], 0.5, v_first, 0.5, out=kv[:, 64:])
-            elif self.add_value_residual:
-                v_first = kv[:, 64:].clone()               # layer-0 values before any mixing (:355-358)
-            k3 = kv[:, :64].unflatten(0, (b, n))
-            v3 = kv[:, 64:].unflatten(0, (b, n))
-            o, lse = ops.mqa_attn_fwd(q.view(b, n, H * 64), k3, v3, heads=H, key_mask=mask_u8, causal=True, bias=bias,
-                                      dropout=d_attn)
-            o2 = o.view(M, H * 64)
-            Y = ops.gemm(o2, W["wo"])
-            if d_out:
-                ops.dropout_(Y, *d_out)
-            rec.update(q=q, kv=kv, o=o2, lse=lse, Y_a=Y)
-            kvs.append(kv)
-            R2, bin2, xn2, beta2, aux2 = ops.hc_pre_fwd(ff_hc.kernel_params(), getattr(f, "0").gamma, R_in=R, Y=Y,
-                                                        beta_prev=beta, M=M, d=d)
-            h = ops.gemm(xn2, W["w1"])                     # [M, 2*ip]
-            gn, st = ops.geglu_ln_fwd(h, getattr(f, "3").gamma, inner=inner, inner_pad=ip, dropout=d_ff)
-            Y2 = ops.gemm(gn, W["w2"])
-            rec.update(R_f=R2, xn_f=xn2, beta_f=beta2, aux_f=aux2, h=h, gn=gn, st=st, Y_f=Y2)
-            L.append(rec)
+            rec = dict(xn_a=xn, bin_a=bin_)
+            Y, k, v, v_first = self._attn_fwd(S, W, rec, v_first, None if kv_cache is None else kv_cache[i], save,
+                                              d_attn, d_out)
+            if want_kv:
+                kvs += (k, v)
+            rec["xn_f"], _ = res.step(Y, hc_f, p_f["ln"], want_bin=False)
+            Y = self._ff_fwd(i, W, rec, d_ff)
+            if save:
+                L.append(rec)
             if i + 1 < self.depth:
-                nxt = self.layers[i + 1][0]
-                R, bin_, xn, beta, aux = ops.hc_pre_fwd(nxt.kernel_params(), nxt.branch.norm.gamma, R_in=R2, Y=Y2,
-                                                        beta_prev=beta2, M=M, d=d)
-        last = L[-1]
-        out, stats = ops.hc_post_fwd(last["R_f"], last["Y_f"], last["beta_f"], self.norm.gamma, M=M, d=d)
+                xn, bin_ = res.step(Y, P[i + 1][0], P[i + 1][1]["ln"], want_bin=True)
+        out = res.exit(Y, self.norm.gamma)
         # kv cache tensor [depth, 2, b, n, 64] as the reference returns it (audiolm_pytorch.py:370, 560)
-        if getattr(self, "_want_kv", True):
-            kv_t = torch.stack([kv.view(b, n, 2, 64).permute(2, 0, 1, 3) for kv in kvs])
-        else:
-            kv_t = torch.empty(0, device=x.device, dtype=bf16)
-        saved = dict(kv=kv_t)
-        if save:
-            saved.update(L=L, x2=x2, mask=mask_u8, bias=bias, stats=stats, shape=(b, n, d), x_dtype=x.dtype, drop=drop)
-        return out.view(b, n, d), saved
+        kv = torch.stack(kvs).unflatten(0, (self.depth, 2)) if want_kv else torch.empty(0, device=x.device, dtype=bf16)
+        if not save:
+            return out.view(b, n, d), kv, None
+        S.update(L=L, res=res)
+        return out.view(b, n, d), kv, S
+
+    def _attn_fwd(self, S, W, rec, v_first, cache, save, d_attn, d_out):
+        """q / kv projections, value residual, KV cache, attention, output projection (+ their dropout) from
+        rec["xn_a"] / rec["bin_a"]; records q, kv, o, lse in `rec`.  Returns (Y, k, v, v_first), k / v including
+        the cached positions."""
+        b, n, _ = S["shape"]
+        H = self.heads
+        q = ops.gemm(rec["xn_a"], W["wq"])                 # [M, H*64]
+        kv = ops.gemm(rec["bin_a"], W["wkv"])              # [M, 128]  (k | v) from the UN-normalised input
+        if self.add_value_residual and v_first is not None:
+            ops.axpby(kv[:, 64:], 0.5, v_first, 0.5, out=kv[:, 64:])
+        elif self.add_value_residual:
+            v_first = kv[:, 64:].clone()                   # layer-0 values before any mixing (:355-358)
+        k = kv[:, :64].unflatten(0, (b, n))
+        v = kv[:, 64:].unflatten(0, (b, n))
+        if cache is not None:
+            k = torch.cat((cache[0].to(bf16), k), dim=1).contiguous()
+            v = torch.cat((cache[1].to(bf16), v), dim=1).contiguous()
+        # without a backward to feed, the kernel skips writing the row LSE
+        o, lse = ops.mqa_attn_fwd(q.view(b, n, H * 64), k, v, heads=H, key_mask=S["mask"], causal=True,
+                                  return_lse=save, bias=S["bias"], dropout=d_attn)
+        o = o.view(b * n, H * 64)
+        Y = ops.gemm(o, W["wo"])
+        if d_out:
+            ops.dropout_(Y, *d_out)
+        rec.update(q=q, kv=kv, o=o, lse=lse)
+        return Y, k, v, v_first
+
+    def _ff_fwd(self, i, W, rec, d_ff):
+        """W1 -> GEGLU + LayerNorm (+ dropout) -> W2 from rec["xn_f"]; records h, gn, st in `rec`.  Returns Y."""
+        f = self.layers[i][2].branch
+        h = ops.gemm(rec["xn_f"], W["w1"])                 # [M, 2*ip]
+        gn, st = ops.geglu_ln_fwd(h, getattr(f, "3").gamma, inner=f.inner, inner_pad=_pad8(f.inner), dropout=d_ff)
+        rec.update(h=h, gn=gn, st=st)
+        return ops.gemm(gn, W["w2"])
 
     # ---- backward ------------------------------------------------------------------------------
-    def _run_backward(self, S, dout):
-        if self.num_residual_streams == 1:
-            return self._run_backward_plain(S, dout)
+    def _walk_backward(self, S, dout):
         b, n, d = S["shape"]
         M = b * n
-        H = self.heads
-        dev = dout.device
-        L = S["L"]
         dout = dout.reshape(M, d).to(bf16).contiguous()
-        params = self._param_list()
-        grads, returned = _grad_targets(params, self.accumulate_into_grad)
-        PL = self.PER_LAYER
-        nk = len(HC_KEYS)
-
-        def slot(i):
-            g = grads[i * PL:(i + 1) * PL]
-            a_hc = dict(zip(HC_KEYS, g[:nk]))
-            g_ln_a, g_wq, g_wkv, g_wo = g[nk:nk + 4]
-            f_hc = dict(zip(HC_KEYS, g[nk + 4:2 * nk + 4]))
-            g_ln_f, g_w1, g_ln2, g_w2 = g[2 * nk + 4:]
-            return a_hc, g_ln_a, g_wq, g_wkv, g_wo, f_hc, g_ln_f, g_w1, g_ln2, g_w2
-
-        last = L[-1]
-        dR, dY, dbeta = ops.hc_post_bwd(last["R_f"], last["Y_f"], last["beta_f"], self.norm.gamma, S["stats"], dout,
-                                        grads[-1], M=M, d=d)
+        P = self._layer_params()
+        grads, returned = _grad_targets(self._param_list(), self.accumulate_into_grad)
+        it = iter(grads)
+        G = [tuple({k: next(it) for k in group} for group in layer) for layer in P]  # grouped like P
+        res = S["res"]
+        dY = res.exit_bwd(self.norm.gamma, dout, grads[-1])
         dv_first = None
-        dx = None
         for i in reversed(range(self.depth)):
-            attn_hc, _, ff_hc = self.layers[i]
-            a, f = attn_hc.branch, ff_hc.branch
-            inner, ip = f.inner, _pad8(f.inner)
+            hc_a, p_a, hc_f, p_f = P[i]
+            g_hc_a, g_a, g_hc_f, g_f = G[i]
             W = self._weights(i)
-            rec = L[i]
-            a_hc, g_ln_a, g_wq, g_wkv, g_wo, f_hc, g_ln_f, g_w1, g_ln2, g_w2 = slot(i)
+            rec = S["L"][i]
             d_attn, d_out, d_ff = S["drop"][i] if S["drop"] else (None, None, None)
-            # ---- feed-forward branch ----
-            dgn = ops.gemm(dY, W["w2"], b_mn=True)                       # [M, ip]
-            _wgrad_cols(dY, rec["gn"], g_w2, inner)
-            dh = ops.geglu_ln_bwd(rec["h"], getattr(f, "3").gamma, rec["st"], dgn, g_ln2, inner=inner, inner_pad=ip,
-                                  dropout=d_ff)
-            dxn_f = ops.gemm(dh, W["w1"], b_mn=True)                     # [M, d]
-            wgrad(dh[:, :inner], rec["xn_f"], g_w1[:inner])
-            wgrad(dh[:, ip:ip + inner], rec["xn_f"], g_w1[inner:])
-            dR_a, dY_a, dbeta_a = ops.hc_pre_bwd(ff_hc.kernel_params(), getattr(f, "0").gamma, f_hc, g_ln_f,
-                                                 rec["aux_f"], dR, dxn_f, dbeta, R_in=rec["R_a"], Y=rec["Y_a"],
-                                                 beta_prev=rec["beta_a"], M=M, d=d)
-            # ---- attention branch ----
-            if d_out:
-                ops.dropout_(dY_a, *d_out)
-            dO = ops.gemm(dY_a, W["wo"], b_mn=True)                      # [M, H*64]
-            wgrad(dY_a, rec["o"], g_wo)
-            kv = rec["kv"]
-            k3 = kv[:, :64].unflatten(0, (b, n))
-            v3 = kv[:, 64:].unflatten(0, (b, n))
-            dq, dk, dv = ops.mqa_attn_bwd(rec["q"].view(b, n, H * 64), k3, v3, rec["o"].view(b, n, H * 64),
-                                          dO.view(b, n, H * 64), rec["lse"], heads=H, key_mask=S["mask"], causal=True,
-                                          bias=S["bias"], dbias=S["dbias"], dropout=d_attn)
-            dkv = torch.empty(M, 128, device=dev, dtype=bf16)
-            ops.axpby(dk.view(M, 64), 1.0, None, 0.0, out=dkv[:, :64])
-            dv2 = dv.view(M, 64)
-            if self.add_value_residual and i > 0:
-                ops.axpby(dv2, 0.5, None, 0.0, out=dkv[:, 64:])
-                dv_first = ops.axpby(dv2, 0.5, dv_first, 1.0) if dv_first is not None else ops.axpby(dv2, 0.5, None, 0.0)
-            elif self.add_value_residual and dv_first is not None:
-                ops.axpby(dv2, 1.0, dv_first, 1.0, out=dkv[:, 64:])
-            else:
-                ops.axpby(dv2, 1.0, None, 0.0, out=dkv[:, 64:])
-            dq2 = dq.view(M, H * 64)
-            dxn_a = ops.gemm(dq2, W["wq"], b_mn=True)
-            dbin_a = ops.gemm(dkv, W["wkv"], b_mn=True)
-            wgrad(dq2, rec["xn_a"], g_wq)
-            wgrad(dkv, rec["bin_a"], g_wkv)
+            dxn = self._ff_bwd(i, W, rec, dY, g_f, d_ff)
+            dY = res.step_bwd(hc_f, p_f["ln"], g_hc_f, g_f["ln"], dxn)
+            dxn, dbin, dv_first = self._attn_bwd(S, i, W, rec, dY, g_a, dv_first, d_attn, d_out)
             if i > 0:
-                prev = L[i - 1]
-                dR, dY, dbeta = ops.hc_pre_bwd(attn_hc.kernel_params(), a.norm.gamma, a_hc, g_ln_a, rec["aux_a"], dR_a,
-                                               dxn_a, dbeta_a, dbin_extra=dbin_a, R_in=prev["R_f"], Y=prev["Y_f"],
-                                               beta_prev=prev["beta_f"], M=M, d=d)
+                dY = res.step_bwd(hc_a, p_a["ln"], g_hc_a, g_a["ln"], dxn, dbin)
             else:
-                dx = ops.hc_pre_bwd(attn_hc.kernel_params(), a.norm.gamma, a_hc, g_ln_a, rec["aux_a"], dR_a, dxn_a,
-                                    dbeta_a, dbin_extra=dbin_a, x_expand=S["x2"], dx_scale=self.grad_shrink_alpha,
-                                    M=M, d=d)
+                dx = res.enter_bwd(hc_a, p_a["ln"], g_hc_a, g_a["ln"], dxn, dbin, self.grad_shrink_alpha)
             if self.grad_ready_hook is not None and returned[0] is None:
                 self.grad_ready_hook(i)  # layer i's gradients are final in their `.grad` buffers (direct accumulation)
         return dx.view(b, n, d).to(S["x_dtype"]), returned
 
+    def _ff_bwd(self, i, W, rec, dY, g, d_ff):
+        """backward of _ff_fwd: accumulates the W1 / LN / W2 gradients into `g`, returns d(xn_f)."""
+        f = self.layers[i][2].branch
+        inner, ip = f.inner, _pad8(f.inner)
+        dgn = ops.gemm(dY, W["w2"], b_mn=True)             # [M, ip]
+        _wgrad_cols(dY, rec["gn"], g["w2"], inner)
+        dh = ops.geglu_ln_bwd(rec["h"], getattr(f, "3").gamma, rec["st"], dgn, g["ln2"], inner=inner, inner_pad=ip,
+                              dropout=d_ff)
+        dxn = ops.gemm(dh, W["w1"], b_mn=True)             # [M, d]
+        wgrad(dh[:, :inner], rec["xn_f"], g["w1"][:inner])
+        wgrad(dh[:, ip:ip + inner], rec["xn_f"], g["w1"][inner:])
+        return dxn
 
-    # ---- num_residual_streams == 1: plain residual stream (fp32) ---------------------------------
-    def _attn_branch_fwd(self, i, xn, raw, b, n, mask_u8, v_first, cache=None, bias=None, d_attn=None, d_out=None):
-        """q/kv projections, value residual, (optional KV cache), attention, output projection (+ their dropout)."""
-        H = self.heads
-        W = self._weights(i)
+    def _attn_bwd(self, S, i, W, rec, dY, g, dv_first, d_attn, d_out):
+        """backward of _attn_fwd for layer i: accumulates the q / kv / out projection gradients into `g`.
+        dv_first: gradient of layer 0's values from the layers above (value residual).  Returns (dxn, dbin, dv_first)."""
+        b, n, _ = S["shape"]
         M = b * n
-        q = ops.gemm(xn, W["wq"])
-        kv = ops.gemm(raw, W["wkv"])
-        if self.add_value_residual and v_first is not None:
-            ops.axpby(kv[:, 64:], 0.5, v_first, 0.5, out=kv[:, 64:])
-        elif self.add_value_residual:
-            v_first = kv[:, 64:].clone()
+        H = self.heads
+        if d_out:
+            ops.dropout_(dY, *d_out)  # dY is read by nothing else
+        dO = ops.gemm(dY, W["wo"], b_mn=True)              # [M, H*64]
+        wgrad(dY, rec["o"], g["wo"])
+        kv = rec["kv"]
         k3 = kv[:, :64].unflatten(0, (b, n))
         v3 = kv[:, 64:].unflatten(0, (b, n))
-        if cache is not None:
-            k3 = torch.cat((cache[0].to(bf16), k3), dim=1).contiguous()
-            v3 = torch.cat((cache[1].to(bf16), v3), dim=1).contiguous()
-        o, lse = ops.mqa_attn_fwd(q.view(b, n, H * 64), k3, v3, heads=H, key_mask=mask_u8, causal=True, bias=bias,
-                                  dropout=d_attn)
-        o2 = o.view(M, H * 64)
-        Y = ops.gemm(o2, W["wo"])
-        if d_out:
-            ops.dropout_(Y, *d_out)
-        return q, kv, o2, lse, Y, v_first, torch.stack((k3, v3))
-
-    def _run_forward_plain(self, x, mask, bias, save, kv_cache=None, drop=None):
-        b, n, d = x.shape
-        M = b * n
-        r = x.detach().reshape(M, d).to(f32).contiguous()
-        x2 = r
-        mask_u8 = ops.pack_key_mask(mask)  # bits, packed once for every layer and the backward
-        L, kvs = [], []
-        a0 = self.layers[0][0].branch
-        r, xn, raw, st = ops.resid_ln_fwd(r, None, a0.norm.gamma, want_raw=True)
-        v_first = None
-        for i, (attn_w, _, ff_w) in enumerate(self.layers):
-            a, f = attn_w.branch, ff_w.branch
-            W = self._weights(i)
-            inner, ip = f.inner, _pad8(f.inner)
-            d_attn, d_out, d_ff = drop[i] if drop else (None, None, None)
-            q, kv, o2, lse, Y, v_first, kv_t = self._attn_branch_fwd(
-                i, xn, raw, b, n, mask_u8, v_first, None if kv_cache is None else kv_cache[i], bias, d_attn, d_out)
-            kvs.append(kv_t)
-            r_f, xn_f, _, st_f = ops.resid_ln_fwd(r, Y, getattr(f, "0").gamma)
-            h = ops.gemm(xn_f, W["w1"])
-            gn, stg = ops.geglu_ln_fwd(h, getattr(f, "3").gamma, inner=inner, inner_pad=ip, dropout=d_ff)
-            Y2 = ops.gemm(gn, W["w2"])
-            L.append(dict(r_a=r, st_a=st, xn_a=xn, raw_a=raw, q=q, kv=kv, o=o2, lse=lse, r_f=r_f, st_f=st_f, xn_f=xn_f,
-                          h=h, gn=gn, stg=stg))
-            if i + 1 < self.depth:
-                nxt = self.layers[i + 1][0].branch
-                r, xn, raw, st = ops.resid_ln_fwd(r_f, Y2, nxt.norm.gamma, want_raw=True)
-        r_last, out, _, st_last = ops.resid_ln_fwd(r_f, Y2, self.norm.gamma)
-        saved = dict(kv=torch.stack(kvs))
-        if save:
-            saved.update(L=L, mask=mask_u8, bias=bias, r_last=r_last, st_last=st_last, shape=(b, n, d),
-                         x_dtype=x.dtype, drop=drop)
-        return out.view(b, n, d), saved
-
-    def _run_backward_plain(self, S, dout):
-        b, n, d = S["shape"]
-        M = b * n
-        H = self.heads
-        dev = dout.device
-        L = S["L"]
-        dout = dout.reshape(M, d).to(bf16).contiguous()
-        params = self._param_list()
-        grads, returned = _grad_targets(params, self.accumulate_into_grad)
-        dr, dr_b = ops.resid_ln_bwd(S["r_last"], self.norm.gamma, S["st_last"], None, dout, None, grads[-1])
-        dv_first = None
-        for i in reversed(range(self.depth)):
-            attn_w, _, ff_w = self.layers[i]
-            a, f = attn_w.branch, ff_w.branch
-            inner, ip = f.inner, _pad8(f.inner)
-            W = self._weights(i)
-            rec = L[i]
-            g_ln_a, g_wq, g_wkv, g_wo, g_ln_f, g_w1, g_ln2, g_w2 = grads[i * 8:(i + 1) * 8]
-            d_attn, d_out, d_ff = S["drop"][i] if S["drop"] else (None, None, None)
-            # feed-forward branch (its output gradient is the residual-stream gradient)
-            dgn = ops.gemm(dr_b, W["w2"], b_mn=True)
-            _wgrad_cols(dr_b, rec["gn"], g_w2, inner)
-            dh = ops.geglu_ln_bwd(rec["h"], getattr(f, "3").gamma, rec["stg"], dgn, g_ln2, inner=inner, inner_pad=ip,
-                                  dropout=d_ff)
-            dxn_f = ops.gemm(dh, W["w1"], b_mn=True)
-            wgrad(dh[:, :inner], rec["xn_f"], g_w1[:inner])
-            wgrad(dh[:, ip:ip + inner], rec["xn_f"], g_w1[inner:])
-            dr, dr_b = ops.resid_ln_bwd(rec["r_f"], getattr(f, "0").gamma, rec["st_f"], dr, dxn_f, None, g_ln_f)
-            # attention branch
-            if d_out:
-                ops.dropout_(dr_b, *d_out)  # dr_b is read by nothing else
-            dO = ops.gemm(dr_b, W["wo"], b_mn=True)
-            wgrad(dr_b, rec["o"], g_wo)
-            kv = rec["kv"]
-            k3 = kv[:, :64].unflatten(0, (b, n))
-            v3 = kv[:, 64:].unflatten(0, (b, n))
-            dq, dk, dv = ops.mqa_attn_bwd(rec["q"].view(b, n, H * 64), k3, v3, rec["o"].view(b, n, H * 64),
-                                          dO.view(b, n, H * 64), rec["lse"], heads=H, key_mask=S["mask"], causal=True,
-                                          bias=S["bias"], dbias=S["dbias"], dropout=d_attn)
-            dkv = torch.empty(M, 128, device=dev, dtype=bf16)
-            ops.axpby(dk.view(M, 64), 1.0, None, 0.0, out=dkv[:, :64])
-            dv2 = dv.view(M, 64)
-            if self.add_value_residual and i > 0:
-                ops.axpby(dv2, 0.5, None, 0.0, out=dkv[:, 64:])
-                dv_first = ops.axpby(dv2, 0.5, dv_first, 1.0) if dv_first is not None else ops.axpby(dv2, 0.5, None, 0.0)
-            elif self.add_value_residual and dv_first is not None:
-                ops.axpby(dv2, 1.0, dv_first, 1.0, out=dkv[:, 64:])
-            else:
-                ops.axpby(dv2, 1.0, None, 0.0, out=dkv[:, 64:])
-            dq2 = dq.view(M, H * 64)
-            dxn_a = ops.gemm(dq2, W["wq"], b_mn=True)
-            dbin_a = ops.gemm(dkv, W["wkv"], b_mn=True)
-            wgrad(dq2, rec["xn_a"], g_wq)
-            wgrad(dkv, rec["raw_a"], g_wkv)
-            dr, dr_b = ops.resid_ln_bwd(rec["r_a"], a.norm.gamma, rec["st_a"], dr, dxn_a, dbin_a, g_ln_a,
-                                        out_scale=self.grad_shrink_alpha if i == 0 else 1.0)
-        return dr.view(b, n, d).to(S["x_dtype"]), returned
-
-    # ---- incremental (KV-cache) inference ------------------------------------------------------
-    @torch.no_grad()
-    def _forward_cached(self, x, mask, kv_cache, bias=None, drop=None):
-        """x is the FULL sequence; only x[:, cache_len:] is processed (audiolm_pytorch.py:489-496)."""
-        cache_len = kv_cache.shape[-2]
-        x = x[:, cache_len:]
-        if self.num_residual_streams == 1:
-            out, saved = self._run_forward_plain(x, mask, bias, save=False, kv_cache=kv_cache, drop=drop)
-            return out, saved["kv"]
-        b, n, d = x.shape
-        M = b * n
-        H = self.heads
-        x2 = x.reshape(M, d).to(f32).contiguous()
-        mask_u8 = ops.pack_key_mask(mask)  # bits, packed once for every layer and the backward
-        hc0 = self.layers[0][0]
-        R, bin_, xn, beta, _ = ops.hc_pre_fwd(hc0.kernel_params(), hc0.branch.norm.gamma, x_expand=x2, M=M, d=d)
-        v_first = None
-        new_cache = []
-        for i, (attn_hc, _, ff_hc) in enumerate(self.layers):
-            W = self._weights(i)
-            f = ff_hc.branch
-            inner, ip = f.inner, _pad8(f.inner)
-            d_attn, d_out, d_ff = drop[i] if drop else (None, None, None)
-            q = ops.gemm(xn, W["wq"])
-            kv = ops.gemm(bin_, W["wkv"])
-            if self.add_value_residual and v_first is not None:
-                ops.axpby(kv[:, 64:], 0.5, v_first, 0.5, out=kv[:, 64:])
-            elif self.add_value_residual:
-                v_first = kv[:, 64:].clone()
-            ck, cv = kv_cache[i][0].to(bf16), kv_cache[i][1].to(bf16)
-            k_all = torch.cat((ck, kv[:, :64].unflatten(0, (b, n))), dim=1).contiguous()
-            v_all = torch.cat((cv, kv[:, 64:].unflatten(0, (b, n))), dim=1).contiguous()
-            new_cache.append(torch.stack((k_all, v_all)))
-            o, _ = ops.mqa_attn_fwd(q.view(b, n, H * 64), k_all, v_all, heads=H, key_mask=mask_u8, causal=True,
-                                    return_lse=False, bias=bias, dropout=d_attn)
-            Y = ops.gemm(o.view(M, H * 64), W["wo"])
-            if d_out:
-                ops.dropout_(Y, *d_out)
-            R2, _, xn2, beta2, _ = ops.hc_pre_fwd(ff_hc.kernel_params(), getattr(f, "0").gamma, R_in=R, Y=Y,
-                                                  beta_prev=beta, M=M, d=d)
-            h = ops.gemm(xn2, W["w1"])
-            gn, _ = ops.geglu_ln_fwd(h, getattr(f, "3").gamma, inner=inner, inner_pad=ip, dropout=d_ff)
-            Y2 = ops.gemm(gn, W["w2"])
-            if i + 1 < self.depth:
-                nxt = self.layers[i + 1][0]
-                R, bin_, xn, beta, _ = ops.hc_pre_fwd(nxt.kernel_params(), nxt.branch.norm.gamma, R_in=R2, Y=Y2,
-                                                      beta_prev=beta2, M=M, d=d)
-        out, _ = ops.hc_post_fwd(R2, Y2, beta2, self.norm.gamma, M=M, d=d)
-        return out.view(b, n, d), torch.stack(new_cache)
+        dq, dk, dv = ops.mqa_attn_bwd(rec["q"].view(b, n, H * 64), k3, v3, rec["o"].view(b, n, H * 64),
+                                      dO.view(b, n, H * 64), rec["lse"], heads=H, key_mask=S["mask"], causal=True,
+                                      bias=S["bias"], dbias=S["dbias"], dropout=d_attn)
+        dkv = torch.empty(M, 128, device=dY.device, dtype=bf16)
+        ops.axpby(dk.view(M, 64), 1.0, None, 0.0, out=dkv[:, :64])
+        dv2 = dv.view(M, 64)
+        if self.add_value_residual and i > 0:
+            ops.axpby(dv2, 0.5, None, 0.0, out=dkv[:, 64:])
+            dv_first = ops.axpby(dv2, 0.5, dv_first, 1.0) if dv_first is not None else ops.axpby(dv2, 0.5, None, 0.0)
+        elif self.add_value_residual and dv_first is not None:
+            ops.axpby(dv2, 1.0, dv_first, 1.0, out=dkv[:, 64:])
+        else:
+            ops.axpby(dv2, 1.0, None, 0.0, out=dkv[:, 64:])
+        dq2 = dq.view(M, H * 64)
+        dxn = ops.gemm(dq2, W["wq"], b_mn=True)
+        dbin = ops.gemm(dkv, W["wkv"], b_mn=True)
+        wgrad(dq2, rec["xn_a"], g["wq"])
+        wgrad(dkv, rec["bin_a"], g["wkv"])
+        return dxn, dbin, dv_first
 
 
 def _wgrad_cols(dy, x_padded, out, cols):
