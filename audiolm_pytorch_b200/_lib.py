@@ -37,7 +37,8 @@ SIGNATURES: dict[str, list] = {
     "alm_gemm_head_ce": [P, L, P, L, P, P, L, I, P, P, P, P, P, P, L, I, I, I, P],
     "alm_ce_finish": [P, I, P, P, L, P, P, I, P],
     "alm_decode_stack_step": [P, I, P, P, P, P, I, L, P, L, P, L, I, I, I, I, I, F, I, P],
-    "alm_mqa_attn_decode": [P, L, P, P, L, P, I, P, L, P, L, P, I, I, I, F, P],
+    "alm_mqa_attn_decode": [P, L, P, P, L, P, I, P, L, P, L, P, L, P, I, I, I, F, P],
+    "alm_decode_bias_row": [P, I, P, P, P, I, P, I, P, L, I, P],
     "alm_bias_gather_fwd": [P, P, P, P, I, I, I, L, P],
     "alm_bias_gather_bwd": [P, P, P, P, I, I, I, L, P],
     "alm_hc_pre_fwd": [P] * 12 + [P, P, P, P, P, I, I, I, P],

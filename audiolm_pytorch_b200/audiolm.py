@@ -17,7 +17,7 @@ from torch import nn
 from . import heads as _heads_mod
 from .heads import (HeadCache, LazyLogits, cross_entropy, generate_mask_with_prob, gumbel_sample, mask_out_after_eos_id, top_k)
 from . import ops
-from .decode import StackDecoder, TokenDecoder, engine_supported
+from .decode import StackDecoder, TokenDecoder
 from .rel_pos import gather_bias, mlp_table
 from .transformer import Transformer, default, exists
 
@@ -68,6 +68,20 @@ def _tile_rows(weight, n):
     backward is a strided sum instead of an index_put scatter over batch x positions."""
     q = weight.shape[0]
     return weight.repeat(ceil_div(n, q), 1)[:n]
+
+
+def _rel_coords(cls):
+    """(u, cls, c) of a relative-position bias over cache positions 0..max_len-1 (max_len = cls.shape[0]): u = t and
+    c = max_len - 1, i.e. table row (L - j) + max_len - 1 of `RelativePositionBias.table(max_len)`."""
+    max_len = cls.shape[0]
+    return torch.arange(max_len, dtype=torch.int32, device=cls.device), cls, max_len - 1
+
+
+def _pos_mlp_in(max_seq, rel_off, dev):
+    """fp32 [(2 max_seq - 1) rel_off, 2] inputs of the fine transformer's pos_bias_mlp: (row // rel_off, row % rel_off)
+    of every table row (the reference feeds the shifted, non-negative coordinates, :1278-1290)."""
+    rows = torch.arange((2 * max_seq - 1) * rel_off, device=dev)
+    return torch.stack((rows // rel_off, rows % rel_off), dim=-1).float()
 
 
 def _quantizer_ids(n, q, device):
@@ -176,6 +190,21 @@ class SemanticTransformer(_TokenTransformer):
         logits, new_cache = self.forward(*args, cond_drop_prob=0.0, kv_cache=cache, return_kv_cache=True, **kwargs)
         return (logits, new_cache[None]) if return_kv_cache else logits
 
+    def decode_bias_coords(self, max_len, dev=None):
+        """(u, cls, c) of the decode engine's bias rule (decode.StackDecoder.set_bias) for cache positions
+        0..max_len-1: the relative-position bias of keys j <= L for the query at position L is table row
+        u[L] - u[j] + c of `rel_pos_bias.table(max_len)`, the row RelativePositionBias.index picks in the dense path."""
+        return _rel_coords(torch.zeros(max_len, dtype=torch.int32, device=dev))
+
+    def decode_bias(self, max_len):
+        """(table, override, u, cls, c) of the decode engine's bias for a cache of max_len positions, None without a
+        relative-position bias (flash_attn=True)."""
+        rp = self.transformer.rel_pos_bias
+        if not exists(rp):
+            return None
+        u, cls, c = self.decode_bias_coords(max_len, self.device)
+        return rp.table(max_len), None, u, cls, c
+
     def forward(self, *, ids=None, return_loss=False, text=None, text_embeds=None, self_attn_mask=None,
                 cond_drop_prob=None, unique_consecutive=None, kv_cache=None, return_kv_cache=False):
         self._no_text(text, text_embeds)
@@ -234,6 +263,21 @@ class CoarseTransformer(_TokenTransformer):
         logits, (new_kv, new_emb) = self.forward(*args, cond_drop_prob=0.0, return_cache=True, kv_cache=kv,
                                                  embed_cache=emb, **kwargs)
         return (logits, (new_kv[None], new_emb[None])) if return_kv_cache else logits
+
+    def decode_bias_coords(self, num_semantic, max_len, dev=None):
+        """(u, cls, c) of the decode engine's bias rule for the sequence [semantic start | num_semantic semantic
+        tokens | coarse start | coarse tokens ...] over cache positions 0..max_len-1: the relative-position row as
+        `_cross_index`, and `cross_attn_bias` between the semantic segment (class 1) and the coarse one (class 2)."""
+        t = torch.arange(max_len, device=dev)
+        return _rel_coords(torch.where(t <= num_semantic, 1, 2).to(torch.int32))
+
+    def decode_bias(self, num_semantic, max_len):
+        """(table, override, u, cls, c) of the decode engine's bias (see decode_bias_coords), None on the flash path."""
+        rp = self.transformer.rel_pos_bias
+        if not exists(rp):
+            return None
+        u, cls, c = self.decode_bias_coords(num_semantic, max_len, self.device)
+        return rp.table(max_len), self.cross_attn_bias.reshape(-1), u, cls, c
 
     def _cross_index(self, n, n_sem, dev):
         """table row per (i, j) as RelativePositionBias.index, -1 where exactly one of i, j is semantic."""
@@ -344,31 +388,66 @@ class FineTransformer(_TokenTransformer):
                                                  embed_cache=emb, **kwargs)
         return (logits, (new_kv[None], new_emb[None])) if return_kv_cache else logits
 
+    def _pos_coords(self, n, nf, dev):
+        """per token of [coarse start | n coarse | fine start | nf fine]: frame position (-1 for the two start tokens)
+        and quantizer offset (fine offsets follow the coarse ones); plus the frame count N = max_seq, the number of
+        offsets and the table row stride rel_off = 2 * num_off - 1."""
+        qc, qf = self.num_coarse_quantizers, self.num_fine_quantizers
+        max_seq = max(ceil_div(n, qc), ceil_div(nf, qf))
+        num_off = qc + qf
+        rel_off = 2 * num_off - 1
+        ar = lambda m: torch.arange(m, device=dev)  # noqa: E731
+        minus1 = torch.full((1,), -1, device=dev)
+        zero = torch.zeros(1, dtype=torch.long, device=dev)
+        pos = torch.cat((minus1, ar(n) // qc, minus1, ar(nf) // qf))
+        off = torch.cat((zero, ar(n) % qc, zero, ar(nf) % qf + qc))
+        return pos, off, max_seq, num_off, rel_off
+
     def _pos_bias_index(self, n, nf, dev):
         """(idx int32 [L, L], mlp inputs fp32 [P, 2]) of the engineered coarse/fine bias (:1229-1298).
 
-        Token t has a frame position and a quantizer offset (fine offsets follow the coarse ones); the bias of
-        (i, j) is the MLP at (frame_i - frame_j, offset_i - offset_j), shifted to non-negative table
-        coordinates; rows / columns of the two start tokens use `null_pos_bias` (idx -1)."""
+        Token t has a frame position and a quantizer offset (`_pos_coords`); the bias of (i, j) is the MLP at
+        (frame_i - frame_j, offset_i - offset_j), shifted to non-negative table coordinates; rows / columns of the
+        two start tokens use `null_pos_bias` (idx -1)."""
         key = (n, nf, str(dev))
         if self._bias_idx.get("key") != key:
-            qc, qf = self.num_coarse_quantizers, self.num_fine_quantizers
-            max_seq = max(ceil_div(n, qc), ceil_div(nf, qf))
-            num_off = qc + qf
-            rel_off = 2 * num_off - 1
-            ar = lambda m: torch.arange(m, device=dev)  # noqa: E731
-            minus1 = torch.full((1,), -1, device=dev)
-            zero = torch.zeros(1, dtype=torch.long, device=dev)
-            pos = torch.cat((minus1, ar(n) // qc, minus1, ar(nf) // qf))
-            off = torch.cat((zero, ar(n) % qc, zero, ar(nf) % qf + qc))
+            pos, off, max_seq, num_off, rel_off = self._pos_coords(n, nf, dev)
             pc = pos.clamp(min=0)
             idx = (pc[:, None] - pc[None, :] + max_seq - 1) * rel_off + (off[:, None] - off[None, :] + num_off - 1)
             start = pos == -1
             idx[start[:, None] | start[None, :]] = -1
-            rows = ar((2 * max_seq - 1) * rel_off)
-            mlp_in = torch.stack((rows // rel_off, rows % rel_off), dim=-1).float()
-            self._bias_idx = dict(key=key, val=(idx.to(torch.int32).contiguous(), mlp_in))
+            self._bias_idx = dict(key=key, val=(idx.to(torch.int32).contiguous(), _pos_mlp_in(max_seq, rel_off, dev)))
         return self._bias_idx["val"]
+
+    def decode_bias_coords(self, num_coarse, num_fine, max_len, dev=None):
+        """(u, cls, c) of the decode engine's bias rule for [coarse start | num_coarse coarse | fine start | fine
+        tokens] over cache positions 0..max_len-1, while the sequence holds at most num_fine fine tokens:
+        u = frame * rel_off + offset and c = (N - 1) * rel_off + num_off - 1, so u[L] - u[j] + c is the row
+        `_pos_bias_index` picks; the start tokens are class -1 (null_pos_bias).  The table (and N) of the dense path
+        depends on the fine length; it is the same at every length the sequence passes through only while the fine
+        frames do not outnumber the coarse ones, which is asserted."""
+        qc, qf = self.num_coarse_quantizers, self.num_fine_quantizers
+        assert ceil_div(num_fine, qf) <= ceil_div(num_coarse, qc), \
+            "the fine frames outnumber the coarse frames: the bias table would change during decoding"
+        pos, off, max_seq, num_off, rel_off = self._pos_coords(num_coarse, num_fine, dev)
+        n_all = pos.shape[0]
+        assert n_all <= max_len
+        u = torch.zeros(max_len, dtype=torch.int32, device=dev)
+        cls = torch.full((max_len,), -1, dtype=torch.int32, device=dev)
+        u[:n_all] = (pos.clamp(min=0) * rel_off + off).to(torch.int32)
+        cls[:n_all] = torch.where(pos < 0, -1, 0).to(torch.int32)
+        return u, cls, (max_seq - 1) * rel_off + num_off - 1
+
+    def decode_bias(self, num_coarse, num_fine, max_len):
+        """(table, override, u, cls, c) of the decode engine's bias (see decode_bias_coords), None on the flash path.
+        The table is the pos_bias_mlp over the dense path's table rows, so both paths read the same values."""
+        if not exists(self.pos_bias_mlp):
+            return None
+        u, cls, c = self.decode_bias_coords(num_coarse, num_fine, max_len, self.device)
+        _, _, max_seq, _, rel_off = self._pos_coords(num_coarse, num_fine, "cpu")
+        m = self.pos_bias_mlp
+        table = mlp_table(_pos_mlp_in(max_seq, rel_off, self.device), m[0], [m[2]], m[4], self._bias_cache, "pos")
+        return table, self.null_pos_bias.reshape(-1), u, cls, c
 
     def forward(self, coarse_token_ids, fine_token_ids, text=None, text_embeds=None, cond_drop_prob=None,
                 self_attn_mask=None, kv_cache=None, embed_cache=None, return_cache=False,
@@ -436,22 +515,31 @@ def _eval_no_grad(fn):
     return inner
 
 
-def _cached_engine(owner, stack, batch, max_len, filter_thres, temperature, *, embed_fn, logits_fn):
+def _cached_engine(owner, stack, batch, max_len, filter_thres, temperature, *, embed_fn, logits_fn, bias_fn=None):
     """one TokenDecoder (static KV cache + captured graphs) per wrapper, rebuilt when shapes or weights change (the
-    graphs hold pointers to the packed bf16 weight copies of the current parameter versions)."""
+    graphs hold pointers to the packed bf16 weight copies of the current parameter versions).
+
+    bias_fn(max_len) -> (table, override, u, cls, c) or None: the additive attention bias of the model
+    (decode.StackDecoder.set_bias), recomputed for every call and written into the engine's static buffers."""
     # the captured graphs hold raw pointers to the fp32 parameters and to their packed bf16 copies: key on storage
     # address AND version of every parameter (`p.data = ...`, load_state_dict(assign=True), .to(...) change the
     # address without bumping the version)
     ver = hash(tuple((p.data_ptr(), p._version) for p in owner.parameters()))
     max_len = -(-max_len // 256) * 256  # fewer distinct cache sizes -> fewer graph captures
     gens = (stack._packed.generation, owner.transformer._heads._pk.generation)
-    key = (batch, max_len, float(filter_thres), float(temperature), ver, gens, str(stack.norm.gamma.device))
+    bias = None if bias_fn is None else bias_fn(max_len)
+    # the captured bias-row launch holds the table's size and the constant c (the fine table's size depends on the
+    # number of frames)
+    bias_key = None if bias is None else (tuple(bias[0].shape), bias[1] is None, int(bias[4]))
+    key = (batch, max_len, float(filter_thres), float(temperature), ver, gens, str(stack.norm.gamma.device), bias_key)
     eng = getattr(owner, "_engine", None)
     if eng is None or eng[0] != key:
         dec = TokenDecoder(StackDecoder(stack, batch, max_len), embed_fn, logits_fn, filter_thres=filter_thres,
                            temperature=temperature, use_graph=USE_DECODE_GRAPHS)
         owner._engine = eng = (key, dec)
     eng[1].stack.set_key_mask(None)
+    if bias is not None:
+        eng[1].stack.set_bias(*bias)
     return eng[1]
 
 
@@ -501,8 +589,7 @@ class SemanticTransformerWrapper(nn.Module):
             ids = batch_unique_consecutive(ids, pad_value=self.pad_id)
         batch, start = ids.shape
         out = ids.clone()
-        if (use_kv_cache and start < max_length and engine_supported(self.transformer.transformer)
-                and bool((ids != self.pad_id).all())):
+        if use_kv_cache and start < max_length and bool((ids != self.pad_id).all()):
             return self._generate_graphed(out, max_length, filter_thres, temperature)
         last = (ids != self.pad_id).sum(dim=-1).long()
         kv_cache, logits = None, None
@@ -531,7 +618,8 @@ class SemanticTransformerWrapper(nn.Module):
         out = torch.cat((out, _sample_next(logits[:, -1], filter_thres, temperature)), dim=-1)
         dec = _cached_engine(self, tr.transformer, batch, max_length + 2, filter_thres, temperature,
                              embed_fn=lambda tok, _key: tr.semantic_embedding(tok),
-                             logits_fn=lambda o, _key: tr._heads.linear_decode(o, tr.to_logits.weight, tr.to_logits.bias, "sem"))
+                             logits_fn=lambda o, _key: tr._heads.linear_decode(o, tr.to_logits.weight, tr.to_logits.bias, "sem"),
+                             bias_fn=tr.decode_bias)
         dec.stack.load_cache(kv[0])
         dec.tok.copy_(out[:, -1])
         for _ in range(out.shape[1], max_length):
@@ -581,7 +669,7 @@ def _frame_sampler(step_fn, n_quantizers, time_steps, seq, filter_thres, tempera
 
 
 def _frame_sampler_graphed(owner, stack, step_fn, n_quantizers, time_steps, seq, filter_thres, temperature, *,
-                           embed_fn, head_fn, prefix_len, key_mask=None):
+                           embed_fn, head_fn, prefix_len, key_mask=None, bias_fn=None):
     """`_frame_sampler` with the KV cache on the CUDA-graph decode engine (decode.py): the first token goes through
     the normal forward (which also fills the cache), every further token is one graph replay.  One graph per
     quantizer index of the token being fed back (embedding offset, next head, EOS rule all depend on it only).
@@ -607,7 +695,7 @@ def _frame_sampler_graphed(owner, stack, step_fn, n_quantizers, time_steps, seq,
         return lg
 
     dec = _cached_engine(owner, stack, batch, prefix_len + total + 1, filter_thres, temperature, embed_fn=embed_fn,
-                         logits_fn=logits_fn)
+                         logits_fn=logits_fn, bias_fn=bias_fn)
     dec.stack.load_cache(kv[0])
     if exists(key_mask):
         dec.stack.set_key_mask(key_mask)
@@ -675,14 +763,14 @@ class CoarseTransformerWrapper(nn.Module):
 
         tr = self.transformer
         q_n = self.num_coarse_quantizers
-        if (use_kv_cache and not kwargs and engine_supported(tr.transformer) and coarse.shape[-1] % q_n == 0
-                and max_time_steps > 0):
+        if use_kv_cache and not kwargs and coarse.shape[-1] % q_n == 0 and max_time_steps > 0:
             cb = tr.codebook_size
+            n_sem = semantic_token_ids.reshape(batch, -1).shape[-1]
             seq = _frame_sampler_graphed(
                 self, tr.transformer, step, q_n, range(0, max_time_steps), coarse.clone(), filter_thres, temperature,
                 embed_fn=lambda tok, q: tr.coarse_embedding(tok + q * cb) + tr.coarse_quantize_embedding.weight[q],
                 head_fn=lambda o, q: tr._heads.linear_decode(o, tr.coarse_logit_weights[q], None, ("coarse", q)),
-                prefix_len=semantic_token_ids.reshape(batch, -1).shape[-1] + 2 + coarse.shape[-1])
+                prefix_len=n_sem + 2 + coarse.shape[-1], bias_fn=lambda ml: tr.decode_bias(n_sem, ml))
         else:
             seq = _frame_sampler(step, q_n, range(0, max_time_steps), coarse.clone(), filter_thres, temperature,
                                  use_kv_cache)
@@ -803,8 +891,7 @@ class FineTransformerWrapper(nn.Module):
 
         tr = self.transformer
         q_n = self.num_fine_quantizers
-        if (use_kv_cache and not kwargs and engine_supported(tr.transformer) and not exists(tr.pos_bias_mlp)
-                and fine.shape[-1] % q_n == 0 and steps > first):
+        if use_kv_cache and not kwargs and fine.shape[-1] % q_n == 0 and steps > first:
             cb = tr.codebook_size
             # padded / eos coarse positions are never attended to (FineTransformer.forward, :1175-1184)
             keep = F.pad((coarse != tr.pad_id) & (coarse != tr.eos_id), (1, 0), value=True)
@@ -812,7 +899,8 @@ class FineTransformerWrapper(nn.Module):
                 self, tr.transformer, step, q_n, range(first, steps), fine.clone(), filter_thres, temperature,
                 embed_fn=lambda tok, q: tr.fine_embedding(tok + q * cb) + tr.fine_quantize_embedding.weight[q],
                 head_fn=lambda o, q: tr._heads.linear_decode(o, tr.fine_logit_weights[q], None, ("fine", q)),
-                prefix_len=coarse.shape[-1] + 2 + fine.shape[-1], key_mask=None if bool(keep.all()) else keep)
+                prefix_len=coarse.shape[-1] + 2 + fine.shape[-1], key_mask=None if bool(keep.all()) else keep,
+                bias_fn=lambda ml: tr.decode_bias(coarse.shape[-1], steps * q_n, ml))
         else:
             seq = _frame_sampler(step, q_n, range(first, steps), fine.clone(), filter_thres, temperature,
                                  use_kv_cache)

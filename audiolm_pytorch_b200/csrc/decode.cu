@@ -4,8 +4,9 @@
 // reference re-concatenates the cache with torch.cat per layer per step, :363-365).
 //
 //   alm_kv_append        : k_cache[b, *len, :] = kv_new[b, 0:64], v_cache[b, *len, :] = kv_new[b, 64:128]
-//   alm_mqa_attn_decode  : o[b, h, :] = softmax_j<=*len( q[b,h,:] . k_cache[b,j,:] * scale ) v_cache[b,j,:]
-// Both read the cache length from `len` at run time, so the launch parameters never change between steps.
+//   alm_mqa_attn_decode  : o[b, h, :] = softmax_j<=*len( q[b,h,:] . k_cache[b,j,:] * scale (+ bias[h, j]) ) v_cache[b,j,:]
+//   alm_decode_bias_row  : bias[h, j] for the new token at position *len (relative-position / cross / fine 2-D bias)
+// All three read the cache length from `len` at run time, so the launch parameters never change between steps.
 // One warp per (batch, head): lanes stride over the keys with a private online softmax (fp32), then the 32
 // partial states are merged with shuffles.  K/V rows are shared by all heads (MQA) and stay in L1/L2.
 #include "alm_common.cuh"
@@ -27,12 +28,15 @@ __global__ void kv_append_kernel(const __nv_bfloat16* __restrict__ kv_new, long 
   else vc[(size_t)bb * cache_bstride + (size_t)pos * DEC_D + (c - DEC_D)] = v;
 }
 
+// HAS_BIAS: an additive fp32 score bias, one row per head (bias[head * bias_ld + j]) shared by every sequence of the
+// batch; the scores are in log2 units (q carries scale * log2 e), so the bias enters as bias * log2 e.
+template <bool HAS_BIAS>
 __global__ void __launch_bounds__(256)
 mqa_attn_decode_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __nv_bfloat16* __restrict__ kc,
                        const __nv_bfloat16* __restrict__ vc, long long cache_bstride, const int* __restrict__ len,
                        int max_len, const uint8_t* __restrict__ key_mask, long long mask_bstride,
-                       __nv_bfloat16* __restrict__ o, long long ldo, float* __restrict__ partial, int h,
-                       float scale_log2) {
+                       const float* __restrict__ bias, long long bias_ld, __nv_bfloat16* __restrict__ o, long long ldo,
+                       float* __restrict__ partial, int h, float scale_log2) {
   // grid (b, splits): each CTA covers one contiguous slice of the keys (flash-decoding); with splits > 1 the
   // per-slice softmax states go to `partial` [b, splits, h, 66] = {m, l, acc[64]} and a second kernel merges them
   const int b = blockIdx.x, split = blockIdx.y, splits = gridDim.y;
@@ -72,6 +76,7 @@ mqa_attn_decode_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const
         s = fmaf(qv[i * 8 + 4], bf16_lo(u.z), s); s = fmaf(qv[i * 8 + 5], bf16_hi(u.z), s);
         s = fmaf(qv[i * 8 + 6], bf16_lo(u.w), s); s = fmaf(qv[i * 8 + 7], bf16_hi(u.w), s);
       }
+      if constexpr (HAS_BIAS) s = fmaf(__ldg(bias + (size_t)head * bias_ld + j), 1.4426950408889634f, s);
       const float m_new = fmaxf(m, s);
       const float alpha = exp2f(m - m_new), p = exp2f(s - m_new);
       l = fmaf(l, alpha, p);
@@ -128,6 +133,29 @@ __global__ void mqa_attn_decode_combine_kernel(const float* __restrict__ partial
     }
     o[(size_t)b * ldo + i] = __float2bfloat16(l > 0.f ? a / l : 0.f);
   }
+}
+
+// bias[h, j] (j <= L = *len) of the token at cache position L.  Every bias of the models reduces to one rule over
+// per-position int32 coordinates u[t] and classes cls[t]:
+//   bias[h, j] = (cls[L] != cls[j] || cls[L] < 0) ? override[h] : table[u[L] - u[j] + c, h]
+// (table [rows, h] fp32, override [h] fp32 or null = 0).  A table row outside [0, rows) writes NaN rather than
+// reading out of bounds.  Entries j > L are not written (the attention never reads them).
+__global__ void decode_bias_row_kernel(const float* __restrict__ table, int rows, const float* __restrict__ override_h,
+                                       const int* __restrict__ u, const int* __restrict__ cls, int c,
+                                       const int* __restrict__ len, int max_len, float* __restrict__ out, long long ld,
+                                       int h) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x, head = blockIdx.y;
+  const int L = *len;
+  if (L < 0 || L >= max_len || j > L) return;
+  const int cl = cls[L];
+  float v;
+  if (cl < 0 || cls[j] != cl) {
+    v = override_h ? override_h[head] : 0.f;
+  } else {
+    const int r = u[L] - u[j] + c;
+    v = (r >= 0 && r < rows) ? table[(size_t)r * h + head] : __int_as_float(0x7fc00000);
+  }
+  out[(size_t)head * ld + j] = v;
 }
 
 
@@ -202,27 +230,41 @@ extern "C" int alm_kv_append(const void* kv_new, int64_t ld, void* k_cache, void
 
 extern "C" int alm_mqa_attn_decode(const void* q, int64_t ldq, const void* k_cache, const void* v_cache,
                                    int64_t cache_bstride, const int32_t* len, int max_len, const void* key_mask,
-                                   int64_t mask_bstride, void* o, int64_t ldo, float* workspace, int splits, int b,
-                                   int h, float scale, alm_stream_t stream_) {
+                                   int64_t mask_bstride, const float* bias, int64_t bias_ld, void* o, int64_t ldo,
+                                   float* workspace, int splits, int b, int h, float scale, alm_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ALM_REQUIRE(q && k_cache && v_cache && len && o && b > 0 && h > 0 && max_len > 0, ALM_ERR_ARG);
   ALM_REQUIRE(splits >= 1 && splits <= 64 && (splits == 1 || workspace != nullptr), ALM_ERR_ARG);
+  ALM_REQUIRE(bias == nullptr || bias_ld >= max_len, ALM_ERR_ARG);
   ALM_REQUIRE(ldq % 8 == 0 && ldo % 2 == 0 && cache_bstride % 8 == 0, ALM_ERR_ALIGN);
   ALM_REQUIRE((reinterpret_cast<uintptr_t>(q) & 15u) == 0 && (reinterpret_cast<uintptr_t>(k_cache) & 15u) == 0 &&
                   (reinterpret_cast<uintptr_t>(v_cache) & 15u) == 0, ALM_ERR_ALIGN);
   const int threads = 32 * min(h, 8);
   dim3 grid(b, splits);
-  mqa_attn_decode_kernel<<<grid, threads, 0, stream>>>((const __nv_bfloat16*)q, ldq, (const __nv_bfloat16*)k_cache,
-                                                       (const __nv_bfloat16*)v_cache, cache_bstride, len, max_len,
-                                                       (const uint8_t*)key_mask, mask_bstride, (__nv_bfloat16*)o, ldo,
-                                                       splits > 1 ? workspace : nullptr, h,
-                                                       scale * 1.4426950408889634f);
+  auto kernel = bias ? mqa_attn_decode_kernel<true> : mqa_attn_decode_kernel<false>;
+  kernel<<<grid, threads, 0, stream>>>((const __nv_bfloat16*)q, ldq, (const __nv_bfloat16*)k_cache,
+                                       (const __nv_bfloat16*)v_cache, cache_bstride, len, max_len,
+                                       (const uint8_t*)key_mask, mask_bstride, bias, bias_ld, (__nv_bfloat16*)o, ldo,
+                                       splits > 1 ? workspace : nullptr, h, scale * 1.4426950408889634f);
   ALM_CHECK_LAUNCH();
   if (splits > 1) {
     mqa_attn_decode_combine_kernel<<<b, 256, 0, stream>>>(workspace, (__nv_bfloat16*)o, ldo, h, splits);
     ALM_CHECK_LAUNCH();
   }
   ALM_LAUNCHED(splits > 1 ? 2 : 1);
+  return ALM_OK;
+}
+
+extern "C" int alm_decode_bias_row(const float* table, int rows, const float* override_h, const int32_t* u,
+                                   const int32_t* cls, int c, const int32_t* len, int max_len, float* out, int64_t ld,
+                                   int h, alm_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ALM_REQUIRE(table && u && cls && len && out && rows > 0 && max_len > 0 && h > 0 && h <= 65535 && ld >= max_len,
+              ALM_ERR_ARG);
+  dim3 grid(ceil_div(max_len, 256), h);
+  decode_bias_row_kernel<<<grid, 256, 0, stream>>>(table, rows, override_h, u, cls, c, len, max_len, out, ld, h);
+  ALM_CHECK_LAUNCH();
+  ALM_LAUNCHED(1);
   return ALM_OK;
 }
 

@@ -12,6 +12,12 @@ works on STATIC buffers: the K/V cache is a preallocated [depth, b, max_len, 64]
 a device int32 (`alm_kv_append`, `alm_mqa_attn_decode` read it at run time), the token goes in and out through a
 device buffer.  The step is therefore captured ONCE per sampling position class in a CUDA graph and replayed per
 token; the host only replays the graph and polls for EOS.
+
+Every stack `Transformer` accepts runs here: the plain residual (num_residual_streams=1) takes resid_ln steps
+instead of the hyper-connection ones, and a model with an additive attention bias (flash_attn=False: relative
+position bias, the coarse cross bias, the fine 2-D bias) hands the engine a per-position description of it
+(`StackDecoder.set_bias`); each step writes the new token's bias row once (`alm_decode_bias_row`) and every layer's
+decode attention adds it to its scores.
 """
 from __future__ import annotations
 
@@ -31,16 +37,10 @@ f32 = torch.float32
 FUSED_STACK_STEP = False
 
 
-def engine_supported(tr: Transformer) -> bool:
-    """the static-cache step is built for the 4-stream hyper-connection stack on the flash path"""
-    return tr.num_residual_streams == 4 and tr.rel_pos_bias is None
-
-
 class StackDecoder:
     """One-token incremental forward of a `Transformer` stack against a static KV cache."""
 
     def __init__(self, tr: Transformer, batch: int, max_len: int):
-        assert engine_supported(tr)
         dev = next(tr.parameters()).device
         self.tr, self.b, self.max_len = tr, batch, max_len
         self.kc = torch.zeros(tr.depth, batch, max_len, 64, device=dev, dtype=bf16)
@@ -50,6 +50,7 @@ class StackDecoder:
         self.mask = torch.ones(batch, max_len, device=dev, dtype=torch.uint8)
         self.host_len = 0  # host mirror of `len` (graph replays advance it too): a full cache is an error, not a drop
         self._fused = None  # (signature, pointer table, scratch, out) of the one-kernel step
+        self.bias = None    # static (table, override, u, cls, c, row) of the attention bias, see set_bias
 
     def _fused_state(self):
         """device pointer table + per-CTA regrouped operand copies of alm_decode_stack_step; rebuilt only when a
@@ -85,10 +86,11 @@ class StackDecoder:
         return self._fused
 
     def fused_ok(self):
+        """the one-kernel step covers the 4-stream stack without an attention bias"""
         tr = self.tr
         inner = tr.layers[0][2].branch.inner
         return (FUSED_STACK_STEP and self.b <= ops.DECODE_STEP_MAX_ROWS and tr.dim <= 2048 and tr.heads <= 64
-                and inner <= 4096 and tr.depth <= 64)
+                and inner <= 4096 and tr.depth <= 64 and tr.num_residual_streams == 4 and self.bias is None)
 
     def barrier_timeouts(self) -> int:
         """sticky error flag of the one-kernel step (a device-wide barrier gave up waiting); 0 when healthy"""
@@ -111,11 +113,39 @@ class StackDecoder:
         if mask is not None:
             self.mask[:, :mask.shape[1]] = mask.to(torch.uint8)
 
+    def set_bias(self, table, override, u, cls, c):
+        """The additive attention bias shared by every layer and sequence, as the rule of `alm_decode_bias_row`:
+        for the token at cache position L and keys j <= L,
+            bias[h, j] = (cls[L] != cls[j] or cls[L] < 0) ? override[h] : table[u[L] - u[j] + c, h]
+        table fp32 [P, H], override [H] or None, u / cls int32 [max_len] (the models' `decode_bias`).
+        The first call allocates STATIC buffers that captured graphs keep pointing at; later calls rewrite them in
+        place, so the table size, the presence of an override and c must not change (the engine cache keys on them)."""
+        H = self.tr.heads
+        assert table.dim() == 2 and table.shape[1] == H and u.shape == (self.max_len,) and cls.shape == (self.max_len,)
+        if self.bias is None:
+            dev = self.kc.device
+            self.bias = (torch.empty(table.shape, device=dev, dtype=f32),
+                         None if override is None else torch.empty(H, device=dev, dtype=f32),
+                         torch.empty(self.max_len, device=dev, dtype=torch.int32),
+                         torch.empty(self.max_len, device=dev, dtype=torch.int32), int(c),
+                         torch.zeros(H, self.max_len, device=dev, dtype=f32))
+        bt, bo, bu, bc, c0, _ = self.bias
+        assert bt.shape == table.shape and (bo is None) == (override is None) and c0 == int(c), \
+            "the bias table's size, override and c are fixed once set"
+        bt.copy_(table.detach())
+        if bo is not None:
+            bo.copy_(override.detach().reshape(H))
+        bu.copy_(u)
+        bc.copy_(cls)
+
     @torch.no_grad()
     def step(self, x):
         """x [b, d] (embedding of the new token) -> normed output [b, d] bf16; appends to the cache, len += 1."""
         tr = self.tr
         b, d, H = self.b, tr.dim, tr.heads
+        if tr.rel_pos_bias is not None and self.bias is None:
+            raise ops._lib.AlmError("this stack has a relative position bias: set it with StackDecoder.set_bias "
+                                    "(the models' decode_bias) before decoding")
         x2 = x.reshape(b, d).to(f32).contiguous()
         if self.fused_ok():
             _, table, scratch, out, _, G = self._fused_state()
@@ -125,8 +155,18 @@ class StackDecoder:
             return out   # (the kernel advanced self.len)
         # a few rows: every Linear is a weight-read-bound matrix-vector product (alm_gemv_bf16 over all SMs)
         mm = (lambda a, w: ops.gemv(a, w)) if b <= 8 else (lambda a, w: ops.gemm(a, w))
+        brow = None
+        if self.bias is not None:   # the new token's bias row, read by every layer
+            table, over, u, cls, c, brow = self.bias
+            ops.decode_bias_row(table, over, u, cls, c, self.len, brow)
+        # the residual stream as in Transformer._walk_forward: fp32 r (plain, resid_ln) or bf16 R [b, 4, d]
+        # (hyper-connections); `bin_` (the un-normalised branch input) feeds to_kv
+        plain = tr.num_residual_streams == 1
         hc0 = tr.layers[0][0]
-        R, bin_, xn, beta, _ = ops.hc_pre_fwd(hc0.kernel_params(), hc0.branch.norm.gamma, x_expand=x2, M=b, d=d)
+        if plain:
+            r, xn, bin_, _ = ops.resid_ln_fwd(x2, None, hc0.branch.norm.gamma, want_raw=True)
+        else:
+            R, bin_, xn, beta, _ = ops.hc_pre_fwd(hc0.kernel_params(), hc0.branch.norm.gamma, x_expand=x2, M=b, d=d)
         v_first = None
         for i, (attn_hc, _, ff_hc) in enumerate(tr.layers):
             W = tr._weights(i)
@@ -139,18 +179,27 @@ class StackDecoder:
             elif tr.add_value_residual:
                 v_first = kv[:, 64:].clone()
             ops.kv_append(kv, self.kc[i], self.vc[i], self.len)
-            o = ops.mqa_attn_decode(q, self.kc[i], self.vc[i], self.len, heads=H, key_mask=self.mask)
+            o = ops.mqa_attn_decode(q, self.kc[i], self.vc[i], self.len, heads=H, key_mask=self.mask, bias=brow)
             Y = mm(o, W["wo"])
-            R2, _, xn2, beta2, _ = ops.hc_pre_fwd(ff_hc.kernel_params(), getattr(f, "0").gamma, R_in=R, Y=Y,
-                                                  beta_prev=beta, M=b, d=d)
+            if plain:
+                r, xn2, _, _ = ops.resid_ln_fwd(r, Y, getattr(f, "0").gamma)
+            else:
+                R2, _, xn2, beta2, _ = ops.hc_pre_fwd(ff_hc.kernel_params(), getattr(f, "0").gamma, R_in=R, Y=Y,
+                                                      beta_prev=beta, M=b, d=d)
             h = mm(xn2, W["w1"])
             gn, _ = ops.geglu_ln_fwd(h, getattr(f, "3").gamma, inner=inner, inner_pad=ip)
             Y2 = mm(gn, W["w2"])
             if i + 1 < tr.depth:
                 nxt = tr.layers[i + 1][0]
-                R, bin_, xn, beta, _ = ops.hc_pre_fwd(nxt.kernel_params(), nxt.branch.norm.gamma, R_in=R2, Y=Y2,
-                                                      beta_prev=beta2, M=b, d=d)
-        out, _ = ops.hc_post_fwd(R2, Y2, beta2, tr.norm.gamma, M=b, d=d)
+                if plain:
+                    r, xn, bin_, _ = ops.resid_ln_fwd(r, Y2, nxt.branch.norm.gamma, want_raw=True)
+                else:
+                    R, bin_, xn, beta, _ = ops.hc_pre_fwd(nxt.kernel_params(), nxt.branch.norm.gamma, R_in=R2, Y=Y2,
+                                                          beta_prev=beta2, M=b, d=d)
+        if plain:
+            out = ops.resid_ln_fwd(r, Y2, tr.norm.gamma)[1]
+        else:
+            out, _ = ops.hc_post_fwd(R2, Y2, beta2, tr.norm.gamma, M=b, d=d)
         self.len.add_(1)
         return out
 

@@ -309,22 +309,40 @@ def kv_append(kv_new, k_cache, v_cache, cache_len):
     _lib.call("alm_kv_append", kv_new, kv_new.stride(0), k_cache, v_cache, k_cache.stride(0), cache_len, max_len, b)
 
 
-def mqa_attn_decode(q, k_cache, v_cache, cache_len, *, heads, key_mask=None, scale=None, splits=None):
+def mqa_attn_decode(q, k_cache, v_cache, cache_len, *, heads, key_mask=None, scale=None, splits=None, bias=None):
     """one new query per sequence against the static cache: q [b, heads*64] bf16 -> o [b, heads*64] bf16.
-    Attends keys 0..cache_len (inclusive: the new token has just been appended at position cache_len)."""
-    _check_cuda(q, k_cache, v_cache, cache_len, key_mask)
+    Attends keys 0..cache_len (inclusive: the new token has just been appended at position cache_len).
+    bias: fp32 [heads, >= max_len] added to the scores of every sequence (row j of head h: bias[h, j]) or None."""
+    _check_cuda(q, k_cache, v_cache, cache_len, key_mask, bias)
     b, max_len, _ = k_cache.shape
     assert q.shape == (b, heads * 64) and q.dtype == bf16 and q.stride(1) == 1
     o = torch.empty(b, heads * 64, device=q.device, dtype=bf16)
     if key_mask is not None:
         assert key_mask.dtype == torch.uint8 and key_mask.shape[0] == b and key_mask.shape[1] >= max_len
+    if bias is not None:
+        assert bias.dtype == f32 and bias.shape[0] == heads and bias.shape[1] >= max_len and bias.stride(1) == 1
     if splits is None:  # enough CTAs to spread a long cache over the SMs, fixed per cache size (static launch)
         splits = max(1, min(32, max_len // 128, num_sms(q.device) // max(1, b)))
     ws = torch.empty(b, splits, heads, 66, device=q.device, dtype=f32) if splits > 1 else None
     _lib.call("alm_mqa_attn_decode", q, q.stride(0), k_cache, v_cache, k_cache.stride(0), cache_len, max_len, key_mask,
-              0 if key_mask is None else key_mask.stride(0), o, o.stride(0), ws, splits, b, heads,
-              float(64 ** -0.5 if scale is None else scale))
+              0 if key_mask is None else key_mask.stride(0), bias, 0 if bias is None else bias.stride(0), o, o.stride(0),
+              ws, splits, b, heads, float(64 ** -0.5 if scale is None else scale))
     return o
+
+
+def decode_bias_row(table, override, u, cls, c, cache_len, out):
+    """out[h, j] (j <= L = cache_len) = (cls[L] != cls[j] or cls[L] < 0) ? override[h] : table[u[L] - u[j] + c, h].
+    table fp32 [rows, H], override fp32 [H] or None (= 0), u / cls int32 [max_len], out fp32 [H, >= max_len]."""
+    _check_cuda(table, override, u, cls, cache_len, out)
+    rows, H = table.shape
+    max_len = u.shape[0]
+    assert table.dtype == f32 and table.is_contiguous() and u.dtype == torch.int32 and cls.dtype == torch.int32
+    assert u.is_contiguous() and cls.is_contiguous() and cls.shape == u.shape and cache_len.dtype == torch.int32
+    assert out.dtype == f32 and out.shape[0] == H and out.shape[1] >= max_len and out.stride(1) == 1
+    if override is not None:
+        assert override.dtype == f32 and override.is_contiguous() and override.numel() == H
+    _lib.call("alm_decode_bias_row", table, rows, override, u, cls, int(c), cache_len, max_len, out, out.stride(0), H)
+    return out
 
 
 def head_ce_fwd(x, w, bias, labels, ignore_index):

@@ -139,6 +139,15 @@ int alm_bias_gather_bwd(const float* dbias, const int32_t* idx, float* dtable, f
  * row stride mask_bstride, 1 = attend) optional.  splits > 1 slices the keys over that many CTAs per sequence
  * (flash-decoding) and merges the partial softmax states in a second launch.  Replaces the per-step torch.cat of the cache and the n_q = 1
  * attention of Attention.forward (audiolm_pytorch.py:363-365, 390) inside generate (:1406-1511, 1608-1740, 1896-2039).
+ * bias (optional, fp32 [h, bias_ld >= max_len]): added to the scores of every sequence, softmax(q·kᵀ·scale + bias[h, j])
+ * as attend.py:117-144; null runs the bias-free kernel.
+ *   alm_decode_bias_row  that bias row for the token at position L = *len, from per-position int32 coordinates u[t] and
+ *                        classes cls[t] (both [max_len]):
+ *                        out[h, j] = (cls[L] != cls[j] || cls[L] < 0) ? override_h[h] : table[u[L] - u[j] + c, h]
+ *                        for j <= L (entries j > L are not written).  table fp32 [rows, h]; override_h fp32 [h] or null
+ *                        (= 0); a table row outside [0, rows) writes NaN.  One launch, constant parameters (graph-capturable).
+ *                        The relative-position bias (u = t, cls = 0), the coarse cross bias (cls = segment) and the fine
+ *                        2-D bias (u = frame * R + quantizer offset, cls = -1 for the start tokens) all take this form.
  */
 /* out[r, n] = sum_k x[r, k] W[n, k] (+ bias[n]) for rows <= 8 (a decode step's Linear layers: weight-read bound;
  * one warp per output column over all SMs).  W bf16 [N, ldw] with zero padding to a multiple of 8 columns. */
@@ -147,9 +156,12 @@ int alm_gemv_bf16(const void* x, int64_t ldx, const void* W, int64_t ldw, void* 
 int alm_kv_append(const void* kv_new, int64_t ld, void* k_cache, void* v_cache, int64_t cache_bstride,
                   const int32_t* len, int max_len, int b, alm_stream_t stream);
 int alm_mqa_attn_decode(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int64_t cache_bstride,
-                        const int32_t* len, int max_len, const void* key_mask, int64_t mask_bstride, void* o,
-                        int64_t ldo, float* workspace /* [b, splits, h, 66] fp32 when splits > 1 */, int splits, int b,
-                        int h, float scale, alm_stream_t stream);
+                        const int32_t* len, int max_len, const void* key_mask, int64_t mask_bstride, const float* bias,
+                        int64_t bias_ld, void* o, int64_t ldo,
+                        float* workspace /* [b, splits, h, 66] fp32 when splits > 1 */, int splits, int b, int h,
+                        float scale, alm_stream_t stream);
+int alm_decode_bias_row(const float* table, int rows, const float* override_h, const int32_t* u, const int32_t* cls,
+                        int c, const int32_t* len, int max_len, float* out, int64_t ld, int h, alm_stream_t stream);
 
 /* ---- fused logit head + cross entropy (the [M, V] fp32 logits never reach HBM) --------------------------------
  * Replaces `logits = head(x)` + `F.cross_entropy(logits, labels, ignore_index=...)` of the three wrappers' loss paths
