@@ -11,7 +11,7 @@
 // contiguous channels [8t, 8t+8) of every stream, so d/8 threads are active (d % 8 == 0, d <= 8192).
 #include "alm_common.cuh"
 #include "hyper_conn_v2.cuh"
-#include "hyper_conn_v3.cuh"
+#include "hyper_conn_ring.cuh"
 
 namespace alm {
 
@@ -74,8 +74,8 @@ __device__ __forceinline__ void load8f(const float* p, float (&f)[8]) {
 }
 
 // Saved per token for the backward: tanh of the dynamic alpha/beta pre-activations, 1/|R_s|, LN stats.
-//   aux [M, AUX] = { ta[S*(S+1)], tb[S], inv_nrm[S], mean, rstd }
-constexpr int HC_AUX = HC_S * HC_T + HC_S + HC_S + (HC_S * HC_T + HC_S) + 2;  // same stride as hc2::AUX (z slots unused here)
+//   aux [M, AUX] = { ta[S*(S+1)], tb[S], inv_nrm[S], ..., mean, rstd }
+constexpr int HC_AUX = hc2::AUX;  // same row as the d <= 1024 kernels (z slots unused here)
 
 // ---------------------------------------------------------------------------------------------
 // forward:  R = R_in + beta_prev (x) Y   (or R_s = x for every s when expanding)
@@ -212,7 +212,7 @@ hc_pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* _
 #pragma unroll
       for (int s = 0; s < HC_S; ++s)
         *reinterpret_cast<uint4*>(R_out + ((size_t)m * HC_S + s) * d + c0) = pack8(mix[s + 1]);
-      *reinterpret_cast<uint4*>(bin + (size_t)m * d + c0) = pack8(mix[0]);
+      if (bin != nullptr) *reinterpret_cast<uint4*>(bin + (size_t)m * d + c0) = pack8(mix[0]);
       float xo[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) xo[e] = (mix[0][e] - mean) * rstd * lng[e];
@@ -691,65 +691,35 @@ extern "C" int alm_hc_pre_bwd(const void* R_in, const void* Y, const float* beta
                               const void* dxn, const void* dbin_extra, const float* dbeta, void* dR_in, void* dY,
                               float* dbeta_prev, float* dx_expand, float dx_scale, float* g_gamma_hc,
                               float* g_dyn_alpha, float* g_dyn_beta, float* g_static_alpha, float* g_static_beta,
-                              float* g_alpha_scale, float* g_beta_scale, float* g_ln_gamma, void* w_out,
-                              void* wy_out, int M, int d, int streams, alm_stream_t stream_) {
+                              float* g_alpha_scale, float* g_beta_scale, float* g_ln_gamma, int M, int d,
+                              int streams, alm_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ALM_REQUIRE(streams == HC_S, ALM_ERR_UNSUPPORTED);
   ALM_REQUIRE(d % 8 == 0 && d >= 8 && d <= 8192 && M > 0, ALM_ERR_ARG);
-  ALM_REQUIRE((w_out == nullptr) == (wy_out == nullptr), ALM_ERR_ARG);
-  if (w_out != nullptr) {
-    // hc3: the per-channel parameter gradients are left to the caller (skinny GEMMs over w_out / wy_out)
-    ALM_REQUIRE(d <= 1024 && x_expand == nullptr && R_in != nullptr && Y != nullptr, ALM_ERR_UNSUPPORTED);
-    hc2::Params p3{gamma_hc, dyn_alpha, dyn_beta, static_alpha, static_beta, alpha_scale, beta_scale, ln_gamma};
-    hc2::Grads g3{g_gamma_hc, g_dyn_alpha, g_dyn_beta, g_static_alpha, g_static_beta, g_alpha_scale, g_beta_scale,
-                  g_ln_gamma};
-    const int nch = ceil_div(d, 256);
-    const size_t smem = hc3::bwd_smem(d);
-    static bool attr3 = false;
-    if (!attr3) {
-      ALM_CUDA_OK(cudaFuncSetAttribute(hc3::pre_bwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hc3::bwd_smem(256)));
-      ALM_CUDA_OK(cudaFuncSetAttribute(hc3::pre_bwd_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hc3::bwd_smem(512)));
-      ALM_CUDA_OK(cudaFuncSetAttribute(hc3::pre_bwd_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hc3::bwd_smem(768)));
-      ALM_CUDA_OK(cudaFuncSetAttribute(hc3::pre_bwd_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hc3::bwd_smem(1024)));
-      attr3 = true;
-    }
-    const int grid3 = min(ceil_div(M, hc3::TOK), 2 * num_sms());
-#define HC3_ARGS (const __nv_bfloat16*)R_in, (const __nv_bfloat16*)Y, beta_prev, p3, aux, (const __nv_bfloat16*)dR_out, \
-                 (const __nv_bfloat16*)dxn, (const __nv_bfloat16*)dbin_extra, dbeta, (__nv_bfloat16*)dR_in,             \
-                 (__nv_bfloat16*)dY, dbeta_prev, (__nv_bfloat16*)w_out, (__nv_bfloat16*)wy_out, g3, M, d
-    switch (nch) {
-      case 1: hc3::pre_bwd_kernel<1><<<grid3, hc3::THREADS, smem, stream>>>(HC3_ARGS); break;
-      case 2: hc3::pre_bwd_kernel<2><<<grid3, hc3::THREADS, smem, stream>>>(HC3_ARGS); break;
-      case 3: hc3::pre_bwd_kernel<3><<<grid3, hc3::THREADS, smem, stream>>>(HC3_ARGS); break;
-      default: hc3::pre_bwd_kernel<4><<<grid3, hc3::THREADS, smem, stream>>>(HC3_ARGS); break;
-    }
-#undef HC3_ARGS
-    ALM_CHECK_LAUNCH();
-    ALM_LAUNCHED(1);
-    return ALM_OK;
-  }
   if (d <= 1024) {
-    hc2::Params p2{gamma_hc, dyn_alpha, dyn_beta, static_alpha, static_beta, alpha_scale, beta_scale, ln_gamma};
-    hc2::Grads g2{g_gamma_hc, g_dyn_alpha, g_dyn_beta, g_static_alpha, g_static_beta, g_alpha_scale, g_beta_scale,
-                  g_ln_gamma};
-    const int tpt = 64;  // 2 warps per token (tpt 128: 4 warps per token, 2 CTAs/SM, 128-register cap, was slower)
-    const int tok = hc2::THREADS / tpt;
-    const int grid2 = min(ceil_div(M, tok), num_sms());
-    const size_t smem = hc2::bwd_smem(d, tpt);
+    // the ring stages rows with bulk copies: every staged row must start on 16 B (d % 8 == 0 keeps it so per row)
+    const void* staged[] = {R_in, Y, beta_prev, x_expand, aux, dR_out, dxn, dbin_extra, dbeta};
+    for (const void* p : staged) ALM_REQUIRE((reinterpret_cast<uintptr_t>(p) & 15) == 0, ALM_ERR_ARG);
+    ALM_REQUIRE(x_expand != nullptr ? dx_expand != nullptr
+                                    : (R_in && Y && beta_prev && dR_in && dY && dbeta_prev), ALM_ERR_ARG);
+    hc2::Params p{gamma_hc, dyn_alpha, dyn_beta, static_alpha, static_beta, alpha_scale, beta_scale, ln_gamma};
+    hc2::Grads g{g_gamma_hc, g_dyn_alpha, g_dyn_beta, g_static_alpha, g_static_beta, g_alpha_scale, g_beta_scale,
+                 g_ln_gamma};
     static bool attr_set = false;
     if (!attr_set) {
-      ALM_CUDA_OK(cudaFuncSetAttribute(hc2::pre_bwd_kernel<1, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)hc2::bwd_smem(512, 64)));
-      ALM_CUDA_OK(cudaFuncSetAttribute(hc2::pre_bwd_kernel<2, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       (int)hc2::bwd_smem(1024, 64)));
+      ALM_CUDA_OK(cudaFuncSetAttribute(hcr::pre_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)hcr::smem_bytes(1024)));
+      ALM_CUDA_OK(cudaFuncSetAttribute(hcr::pre_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)hcr::smem_bytes(1024)));
       attr_set = true;
     }
-#define HC2_BWD_ARGS (const __nv_bfloat16*)R_in, (const __nv_bfloat16*)Y, beta_prev, x_expand, p2, aux,              \
-                     (const __nv_bfloat16*)dR_out, (const __nv_bfloat16*)dxn, (const __nv_bfloat16*)dbin_extra, dbeta, \
-                     (__nv_bfloat16*)dR_in, (__nv_bfloat16*)dY, dbeta_prev, dx_expand, dx_scale, g2, M, d
-    if (d <= 512) hc2::pre_bwd_kernel<1, 64><<<grid2, hc2::THREADS, smem, stream>>>(HC2_BWD_ARGS);
-    else hc2::pre_bwd_kernel<2, 64><<<grid2, hc2::THREADS, smem, stream>>>(HC2_BWD_ARGS);
-#undef HC2_BWD_ARGS
+    const int grid = min(M, num_sms());
+#define HCR_ARGS (const __nv_bfloat16*)R_in, (const __nv_bfloat16*)Y, beta_prev, x_expand, p, aux,                  \
+                 (const __nv_bfloat16*)dR_out, (const __nv_bfloat16*)dxn, (const __nv_bfloat16*)dbin_extra, dbeta, \
+                 (__nv_bfloat16*)dR_in, (__nv_bfloat16*)dY, dbeta_prev, dx_expand, dx_scale, g, M, d
+    if (x_expand != nullptr) hcr::pre_bwd_kernel<true><<<grid, hcr::THREADS, hcr::smem_bytes(d), stream>>>(HCR_ARGS);
+    else hcr::pre_bwd_kernel<false><<<grid, hcr::THREADS, hcr::smem_bytes(d), stream>>>(HCR_ARGS);
+#undef HCR_ARGS
     ALM_CHECK_LAUNCH();
     ALM_LAUNCHED(1);
     return ALM_OK;
@@ -763,19 +733,6 @@ extern "C" int alm_hc_pre_bwd(const void* R_in, const void* Y, const float* beta
               (const __nv_bfloat16*)R_in, (const __nv_bfloat16*)Y, beta_prev, x_expand, prm, aux,
               (const __nv_bfloat16*)dR_out, (const __nv_bfloat16*)dxn, (const __nv_bfloat16*)dbin_extra, dbeta,
               (__nv_bfloat16*)dR_in, (__nv_bfloat16*)dY, dbeta_prev, dx_expand, dx_scale, gr, M, d);
-  ALM_CHECK_LAUNCH();
-  ALM_LAUNCHED(1);
-  return ALM_OK;
-}
-
-extern "C" int alm_hc_param_finish(const float* G, const float* gamma_hc, const float* dyn_alpha,
-                                   const float* dyn_beta, float* g_gamma_hc, float* g_dyn_alpha, float* g_dyn_beta,
-                                   int d, alm_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  ALM_REQUIRE(G && gamma_hc && dyn_alpha && dyn_beta && g_gamma_hc && g_dyn_alpha && g_dyn_beta && d > 0, ALM_ERR_ARG);
-  hc2::Params p{gamma_hc, dyn_alpha, dyn_beta, nullptr, nullptr, nullptr, nullptr, nullptr};
-  hc2::Grads g{g_gamma_hc, g_dyn_alpha, g_dyn_beta, nullptr, nullptr, nullptr, nullptr, nullptr};
-  hc3::hc_param_finish_kernel<<<ceil_div(d, 128), 128, 0, stream>>>(G, p, g, d);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);
   return ALM_OK;

@@ -1,11 +1,10 @@
-// Hyper-Connections kernels, second generation: 2 warps per token, 4 tokens per CTA, no CTA-wide barrier.
-// (The first generation in hyper_conn.cu uses one CTA per token with 5-6 __syncthreads per token and runs far off
-// the HBM roofline.)
+// Hyper-Connections forward, second generation (d <= 1024): 2 warps per token, 4 tokens per CTA, no CTA-wide
+// barrier.  (The first generation in hyper_conn.cu uses one CTA per token with 5-6 __syncthreads per token and runs
+// far off the HBM roofline.)  The backward is hyper_conn_ring.cuh.
 //
 //  - a token's 64 threads each own NCH chunks of 8 channels (16-B vector loads, fully coalesced);
 //  - reductions: warp shuffle + one 64-thread named barrier (bar.sync id, 64) through a tiny smem mailbox;
-//  - per-channel parameters live in shared memory (fp32); parameter gradients are accumulated in shared
-//    memory with red.shared and flushed once per CTA with global atomics.
+//  - per-channel parameters live in shared memory (fp32).
 #pragma once
 #include "alm_common.cuh"
 
@@ -15,7 +14,8 @@ namespace hc2 {
 constexpr int S = 4, T = 5;
 constexpr int THREADS = 256;      // a CTA holds THREADS / TPT token slots; TPT = threads per token (64 or 128)
 constexpr int MAILW = 32;        // floats per warp row of the reduction mailbox (largest reduction: 28 values)
-constexpr int AUX = S * T + S + S + (S * T + S) + 2;  // ta[20] tb[4] inv[4] z[24] (pre-tanh) mean rstd
+// ta[20] tb[4] inv[4] z[24] (pre-tanh) pad[2] mean rstd: 224-B rows, so that the backward stages a row with one bulk copy
+constexpr int AUX = S * T + S + S + (S * T + S) + 4;
 
 template <int TPT>
 __device__ __forceinline__ void bar_slot(int id) {
@@ -256,7 +256,7 @@ pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
           }
           *reinterpret_cast<uint4*>(R_out + ((size_t)m * S + (t - 1)) * d + ch[k]) = pack8(o);
         }
-        *reinterpret_cast<uint4*>(bin + (size_t)m * d + ch[k]) = pack8(bi[k]);
+        if (bin != nullptr) *reinterpret_cast<uint4*>(bin + (size_t)m * d + ch[k]) = pack8(bi[k]);
       }
     }
     slot_sum<2, TPT>(st, mail, which, w2, lane, bar_id);
@@ -281,326 +281,15 @@ pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
         a[S * T + S + s] = inv[s];
         beta_out[(size_t)m * S + s] = beta[s];
       }
+      a[AUX - 4] = 0.f;  // pad: the row is copied whole, so it is written (run-to-run identical aux)
+      a[AUX - 3] = 0.f;
       a[AUX - 2] = mean;
       a[AUX - 1] = rstd;
     }
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// smem for the backward adds PRIVATE per-slot gradient accumulators [TOK][8][d]: gG, gBf, gLn, gA[T]
-template <int NCH, int TPT>
-__global__ void __launch_bounds__(THREADS, TPT == 128 ? 2 : 1)
-pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __restrict__ Y,
-               const float* __restrict__ beta_prev, const float* __restrict__ x_expand, Params prm,
-               const float* __restrict__ aux, const __nv_bfloat16* __restrict__ dR_out,
-               const __nv_bfloat16* __restrict__ dxn, const __nv_bfloat16* __restrict__ dbin_extra,
-               const float* __restrict__ dbeta, __nv_bfloat16* __restrict__ dR_in, __nv_bfloat16* __restrict__ dY,
-               float* __restrict__ dbeta_prev, float* __restrict__ dx_expand, float dx_scale, Grads gr, int M,
-               int d) {
-  extern __shared__ float sm[];
-  constexpr int TOK = THREADS / TPT, WPT = TPT / 32;
-  float* sGradAll = sm + 8 * d;              // [TOK][8][d]: private per token slot -> plain RMW, no atomics
-  float* mailbox = sm + (8 + 8 * TOK) * d;   // [TOK][2][WPT][MAILW]
-  stage_params(sm, prm, d);
-  for (int i = threadIdx.x; i < 8 * TOK * d; i += blockDim.x) sGradAll[i] = 0.f;
-  __syncthreads();
-  const float* sG1 = sm;
-  const float* sBf = sm + d;
-  const float* sLn = sm + 2 * d;
-  const float* sA = sm + 3 * d;
-  const int slot = threadIdx.x / TPT, lt = threadIdx.x % TPT, w2 = lt >> 5, lane = lt & 31;
-  float* sGrad = sGradAll + (size_t)slot * 8 * d;
-  float* gG = sGrad;
-  float* gBf = sGrad + d;
-  float* gLn = sGrad + 2 * d;
-  float* gA = sGrad + 3 * d;
-  float* mail = mailbox + slot * (2 * WPT * MAILW);
-  int which = 0;
-  const int bar_id = 1 + slot;
-  const float sqrt_d = sqrtf((float)d);
-  const float a_scale = *prm.alpha_scale, b_scale = *prm.beta_scale;
-  float Astat[S][T];
-#pragma unroll
-  for (int s = 0; s < S; ++s)
-#pragma unroll
-    for (int t = 0; t < T; ++t) Astat[s][t] = prm.static_alpha[s * T + t];
-  float acc_small[S * T + S + 2];
-#pragma unroll
-  for (int i = 0; i < S * T + S + 2; ++i) acc_small[i] = 0.f;
-  int ch[NCH];
-  bool act[NCH];
-#pragma unroll
-  for (int k = 0; k < NCH; ++k) { ch[k] = (lt + TPT * k) * 8; act[k] = ch[k] < d; }
-
-  for (int m = blockIdx.x * TOK + slot; m < M; m += gridDim.x * TOK) {
-    {  // L2 prefetch of the next token's rows (the kernel is latency-bound at 8 warps / SM)
-      const int mn = m + gridDim.x * TOK;
-      if (mn < M && (lt & 7) == 0) {
-#pragma unroll
-        for (int k = 0; k < NCH; ++k)
-          if (act[k]) {
-            if (x_expand != nullptr) {
-              prefetch_l2(x_expand + (size_t)mn * d + ch[k]);
-              prefetch_l2(x_expand + (size_t)mn * d + ch[k] + 32);
-            } else {
-              prefetch_l2(Y + (size_t)mn * d + ch[k]);
-#pragma unroll
-              for (int s = 0; s < S; ++s) prefetch_l2(R_in + ((size_t)mn * S + s) * d + ch[k]);
-            }
-#pragma unroll
-            for (int s = 0; s < S; ++s) prefetch_l2(dR_out + ((size_t)mn * S + s) * d + ch[k]);
-            prefetch_l2(dxn + (size_t)mn * d + ch[k]);
-            if (dbin_extra != nullptr) prefetch_l2(dbin_extra + (size_t)mn * d + ch[k]);
-          }
-      }
-    }
-    const float* a = aux + (size_t)m * AUX;
-    float ta[S][T], tb[S], inv[S], alpha[S][T], bp[S], dbe[S];
-#pragma unroll
-    for (int s = 0; s < S; ++s) {
-#pragma unroll
-      for (int t = 0; t < T; ++t) {
-        ta[s][t] = a[s * T + t];
-        alpha[s][t] = fmaf(ta[s][t], a_scale, Astat[s][t]);
-      }
-      tb[s] = a[S * T + s];
-      inv[s] = a[S * T + S + s];
-      dbe[s] = dbeta[(size_t)m * S + s];
-      bp[s] = (x_expand == nullptr) ? beta_prev[(size_t)m * S + s] : 0.f;
-    }
-    const float mean = a[AUX - 2], rstd = a[AUX - 1];
-
-    float R[S][NCH][8], yv[NCH][8], dmix[T][NCH][8];
-    float lnred[2] = {0.f, 0.f};
-#pragma unroll
-    for (int k = 0; k < NCH; ++k) {
-#pragma unroll
-      for (int e = 0; e < 8; ++e) yv[k][e] = 0.f;
-      if (act[k]) {
-        if (x_expand != nullptr) {
-          const float4 xa = *reinterpret_cast<const float4*>(x_expand + (size_t)m * d + ch[k]);
-          const float4 xb = *reinterpret_cast<const float4*>(x_expand + (size_t)m * d + ch[k] + 4);
-          const float xv[8] = {xa.x, xa.y, xa.z, xa.w, xb.x, xb.y, xb.z, xb.w};
-#pragma unroll
-          for (int s = 0; s < S; ++s)
-#pragma unroll
-            for (int e = 0; e < 8; ++e) R[s][k][e] = xv[e];
-        } else {
-          unpack8(*reinterpret_cast<const uint4*>(Y + (size_t)m * d + ch[k]), yv[k]);
-#pragma unroll
-          for (int s = 0; s < S; ++s) {
-            float rv[8];
-            unpack8(*reinterpret_cast<const uint4*>(R_in + ((size_t)m * S + s) * d + ch[k]), rv);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) R[s][k][e] = fmaf(bp[s], yv[k][e], rv[e]);
-          }
-        }
-#pragma unroll
-        for (int s = 0; s < S; ++s)
-          unpack8(*reinterpret_cast<const uint4*>(dR_out + ((size_t)m * S + s) * d + ch[k]), dmix[s + 1][k]);
-        // LayerNorm backward, part 1 (dmix[0] temporarily holds gl = dxn * ln_gamma)
-        float dx8[8], lg[8], gl8[8];
-        unpack8(*reinterpret_cast<const uint4*>(dxn + (size_t)m * d + ch[k]), dx8);
-        lds4(sLn + ch[k], lg);
-        lds4(sLn + ch[k] + 4, lg + 4);
-        lds4(gLn + ch[k], gl8);
-        lds4(gLn + ch[k] + 4, gl8 + 4);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          float b = 0.f;
-#pragma unroll
-          for (int s = 0; s < S; ++s) b = fmaf(alpha[s][0], R[s][k][e], b);
-          const float xhat = (b - mean) * rstd;
-          const float gl = dx8[e] * lg[e];
-          gl8[e] = fmaf(dx8[e], xhat, gl8[e]);
-          lnred[0] += gl;
-          lnred[1] = fmaf(gl, xhat, lnred[1]);
-          dmix[0][k][e] = gl;
-        }
-        *reinterpret_cast<float4*>(gLn + ch[k]) = make_float4(gl8[0], gl8[1], gl8[2], gl8[3]);
-        *reinterpret_cast<float4*>(gLn + ch[k] + 4) = make_float4(gl8[4], gl8[5], gl8[6], gl8[7]);
-      } else {
-#pragma unroll
-        for (int s = 0; s < S; ++s)
-#pragma unroll
-          for (int e = 0; e < 8; ++e) { R[s][k][e] = 0.f; dmix[s + 1][k][e] = 0.f; }
-#pragma unroll
-        for (int e = 0; e < 8; ++e) dmix[0][k][e] = 0.f;
-      }
-    }
-    slot_sum<2, TPT>(lnred, mail, which, w2, lane, bar_id);
-    const float m1 = lnred[0] / d, m2 = lnred[1] / d;
-#pragma unroll
-    for (int k = 0; k < NCH; ++k)
-      if (act[k]) {
-        float ex[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) ex[e] = 0.f;
-        if (dbin_extra != nullptr) unpack8(*reinterpret_cast<const uint4*>(dbin_extra + (size_t)m * d + ch[k]), ex);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          float b = 0.f;
-#pragma unroll
-          for (int s = 0; s < S; ++s) b = fmaf(alpha[s][0], R[s][k][e], b);
-          const float xhat = (b - mean) * rstd;
-          dmix[0][k][e] = rstd * (dmix[0][k][e] - m1 - xhat * m2) + ex[e];
-        }
-      }
-    // d alpha
-    float dal[S * T];
-#pragma unroll
-    for (int s = 0; s < S; ++s)
-#pragma unroll
-      for (int t = 0; t < T; ++t) {
-        float acc = 0.f;
-#pragma unroll
-        for (int k = 0; k < NCH; ++k)
-#pragma unroll
-          for (int e = 0; e < 8; ++e) acc = fmaf(dmix[t][k][e], R[s][k][e], acc);
-        dal[s * T + t] = acc;
-      }
-    slot_sum<S * T, TPT>(dal, mail, which, w2, lane, bar_id);
-    float dwa[S][T], dwb[S];
-#pragma unroll
-    for (int s = 0; s < S; ++s) {
-#pragma unroll
-      for (int t = 0; t < T; ++t) {
-        const float g = dal[s * T + t];
-        dwa[s][t] = g * a_scale * (1.f - ta[s][t] * ta[s][t]);
-        acc_small[s * T + t] += g;
-        acc_small[S * T + S] = fmaf(g, ta[s][t], acc_small[S * T + S]);
-      }
-      dwb[s] = dbe[s] * b_scale * (1.f - tb[s] * tb[s]);
-      acc_small[S * T + s] += dbe[s];
-      acc_small[S * T + S + 1] = fmaf(dbe[s], tb[s], acc_small[S * T + S + 1]);
-    }
-    // dR (written in place over dmix[0..3]) + parameter-gradient contributions
-    float udot[S] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int k = 0; k < NCH; ++k) {
-      if (act[k]) {
-#pragma unroll
-        for (int h4 = 0; h4 < 2; ++h4) {
-          const int c = ch[k] + h4 * 4;
-          float g1[4], bf[4], av[T][4], pG[4], pBf[4], pA[T][4];
-          lds4(sG1 + c, g1);
-          lds4(sBf + c, bf);
-          lds4(gG + c, pG);
-          lds4(gBf + c, pBf);
-#pragma unroll
-          for (int t = 0; t < T; ++t) { lds4(sA + t * d + c, av[t]); lds4(gA + t * d + c, pA[t]); }
-#pragma unroll
-          for (int e4 = 0; e4 < 4; ++e4) {
-            const int e = h4 * 4 + e4;
-            float dm[T];
-#pragma unroll
-            for (int t = 0; t < T; ++t) dm[t] = dmix[t][k][e];
-#pragma unroll
-            for (int s = 0; s < S; ++s) {
-              float acc = 0.f;
-#pragma unroll
-              for (int t = 0; t < T; ++t) acc = fmaf(alpha[s][t], dm[t], acc);
-              float dn = dwb[s] * bf[e4];
-#pragma unroll
-              for (int t = 0; t < T; ++t) dn = fmaf(dwa[s][t], av[t][e4], dn);
-              const float rn = R[s][k][e] * inv[s];
-              const float nv = rn * g1[e4];
-              pG[e4] = fmaf(dn * rn, sqrt_d, pG[e4]);
-              pBf[e4] = fmaf(nv, dwb[s], pBf[e4]);
-#pragma unroll
-              for (int t = 0; t < T; ++t) pA[t][e4] = fmaf(nv, dwa[s][t], pA[t][e4]);
-              const float u = dn * g1[e4];
-              udot[s] = fmaf(u, R[s][k][e], udot[s]);
-              dmix[s][k][e] = fmaf(u, inv[s], acc);  // dR[s] (dm[] was read above)
-            }
-          }
-          *reinterpret_cast<float4*>(gG + c) = make_float4(pG[0], pG[1], pG[2], pG[3]);
-          *reinterpret_cast<float4*>(gBf + c) = make_float4(pBf[0], pBf[1], pBf[2], pBf[3]);
-#pragma unroll
-          for (int t = 0; t < T; ++t)
-            *reinterpret_cast<float4*>(gA + t * d + c) = make_float4(pA[t][0], pA[t][1], pA[t][2], pA[t][3]);
-        }
-      }
-    }
-    slot_sum<S, TPT>(udot, mail, which, w2, lane, bar_id);
-    float dbp[S] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int s = 0; s < S; ++s) {
-      const float kk = udot[s] * inv[s] * inv[s] * inv[s];
-#pragma unroll
-      for (int k = 0; k < NCH; ++k)
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          dmix[s][k][e] = fmaf(-R[s][k][e], kk, dmix[s][k][e]);
-          dbp[s] = fmaf(dmix[s][k][e], yv[k][e], dbp[s]);
-        }
-    }
-    if (x_expand != nullptr) {
-#pragma unroll
-      for (int k = 0; k < NCH; ++k)
-        if (act[k]) {
-          float o[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e)
-            o[e] = (dmix[0][k][e] + dmix[1][k][e] + dmix[2][k][e] + dmix[3][k][e]) * dx_scale;
-          float* dst = dx_expand + (size_t)m * d + ch[k];
-          *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1], o[2], o[3]);
-          *reinterpret_cast<float4*>(dst + 4) = make_float4(o[4], o[5], o[6], o[7]);
-        }
-    } else {
-      slot_sum<S, TPT>(dbp, mail, which, w2, lane, bar_id);
-#pragma unroll
-      for (int k = 0; k < NCH; ++k)
-        if (act[k]) {
-          float dy[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            float acc = 0.f;
-#pragma unroll
-            for (int s = 0; s < S; ++s) acc = fmaf(bp[s], dmix[s][k][e], acc);
-            dy[e] = acc;
-          }
-          *reinterpret_cast<uint4*>(dY + (size_t)m * d + ch[k]) = pack8(dy);
-#pragma unroll
-          for (int s = 0; s < S; ++s)
-            *reinterpret_cast<uint4*>(dR_in + ((size_t)m * S + s) * d + ch[k]) = pack8(dmix[s][k]);
-        }
-      if (lt == 0) {
-#pragma unroll
-        for (int s = 0; s < S; ++s) dbeta_prev[(size_t)m * S + s] = dbp[s];
-      }
-    }
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < d; i += blockDim.x) {
-    float acc[8];
-#pragma unroll
-    for (int a8 = 0; a8 < 8; ++a8) {
-      acc[a8] = 0.f;
-#pragma unroll
-      for (int sl = 0; sl < TOK; ++sl) acc[a8] += sGradAll[((size_t)sl * 8 + a8) * d + i];
-    }
-    atomicAdd(gr.gamma_hc + i, acc[0]);
-    atomicAdd(gr.dyn_beta + i, acc[1]);
-    atomicAdd(gr.ln_gamma + i, acc[2]);
-#pragma unroll
-    for (int t = 0; t < T; ++t) atomicAdd(gr.dyn_alpha + (size_t)i * T + t, acc[3 + t]);
-  }
-  if (lt == 0) {  // one thread per token slot holds that slot's scalar-parameter partial sums
-#pragma unroll
-    for (int i = 0; i < S * T; ++i) atomicAdd(gr.static_alpha + i, acc_small[i]);
-#pragma unroll
-    for (int s = 0; s < S; ++s) atomicAdd(gr.static_beta + s, acc_small[S * T + s]);
-    atomicAdd(gr.alpha_scale, acc_small[S * T + S]);
-    atomicAdd(gr.beta_scale, acc_small[S * T + S + 1]);
-  }
-}
-
 inline size_t fwd_smem(int d, int tpt) { return (size_t)(8 * d + (THREADS / tpt) * 2 * (tpt / 32) * MAILW) * sizeof(float); }
-inline size_t bwd_smem(int d, int tpt) {
-  return (size_t)((8 + 8 * (THREADS / tpt)) * d + (THREADS / tpt) * 2 * (tpt / 32) * MAILW) * sizeof(float);
-}
 
 }  // namespace hc2
 }  // namespace alm

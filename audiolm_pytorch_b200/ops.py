@@ -450,8 +450,7 @@ def bias_gather_bwd(dbias, idx, table_rows, *, want_override):
     return dtable, dover
 
 
-HC_BWD_SPLIT = True  # False: hc2 kernel with in-kernel parameter-gradient accumulators (kept for A/B tests)
-HC_AUX = 54  # floats of per-token state kept for the backward (see csrc/hyper_conn.cu)
+HC_AUX = 56  # floats of per-token state kept for the backward (see csrc/hyper_conn_v2.cuh)
 
 
 def _hc_param_ptrs(hc, ln_gamma):
@@ -459,18 +458,19 @@ def _hc_param_ptrs(hc, ln_gamma):
             hc["alpha_scale"], hc["beta_scale"], ln_gamma)
 
 
-def hc_pre_fwd(hc, ln_gamma, *, R_in=None, Y=None, beta_prev=None, x_expand=None, M, d, streams=4):
+def hc_pre_fwd(hc, ln_gamma, *, R_in=None, Y=None, beta_prev=None, x_expand=None, M, d, streams=4, want_bin=True):
     """depth(prev branch) + width(this branch) + pre-LayerNorm.  hc: dict of fp32 HC params.
 
-    Returns R_out [M,S,d] bf16, bin [M,d] bf16, xn [M,d] bf16, beta [M,S] f32, aux [M,30] f32.
+    Returns R_out [M,S,d] bf16, bin [M,d] bf16 (None unless want_bin), xn [M,d] bf16, beta [M,S] f32,
+    aux [M,HC_AUX] f32.
     """
     dev = ln_gamma.device
     R_out = torch.empty(M, streams, d, device=dev, dtype=bf16)
-    bin_ = torch.empty(M, d, device=dev, dtype=bf16)
+    bin_ = torch.empty(M, d, device=dev, dtype=bf16) if want_bin else None
     xn = torch.empty(M, d, device=dev, dtype=bf16)
     beta = torch.empty(M, streams, device=dev, dtype=f32)
     aux = torch.empty(M, HC_AUX, device=dev, dtype=f32)
-    with _timed("hc_pre_fwd", M * d * ((4 if x_expand is not None else 10) + 12), "byte"):
+    with _timed("hc_pre_fwd", M * d * ((4 if x_expand is not None else 10) + 10 + (2 if want_bin else 0)), "byte"):
         _lib.call("alm_hc_pre_fwd", R_in, Y, beta_prev, x_expand, *_hc_param_ptrs(hc, ln_gamma),
                   R_out, bin_, xn, beta, aux, M, d, streams)
     return R_out, bin_, xn, beta, aux
@@ -478,7 +478,8 @@ def hc_pre_fwd(hc, ln_gamma, *, R_in=None, Y=None, beta_prev=None, x_expand=None
 
 def hc_pre_bwd(hc, ln_gamma, grads, g_ln_gamma, aux, dR_out, dxn, dbeta, *, dbin_extra=None, R_in=None, Y=None,
                beta_prev=None, x_expand=None, dx_scale=1.0, M, d, streams=4):
-    """Backward of hc_pre_fwd.  `grads`: dict of fp32 accumulators shaped like `hc` (atomically added to).
+    """Backward of hc_pre_fwd.  `grads`: dict of fp32 accumulators shaped like `hc` (atomically added to, as is
+    g_ln_gamma).
 
     Returns (dR_in, dY, dbeta_prev) or dx_expand [M,d] f32 when the op expanded the streams.
     """
@@ -491,26 +492,12 @@ def hc_pre_bwd(hc, ln_gamma, grads, g_ln_gamma, aux, dR_out, dxn, dbeta, *, dbin
         dR_in = torch.empty(M, streams, d, device=dev, dtype=bf16)
         dY = torch.empty(M, d, device=dev, dtype=bf16)
         dbp = torch.empty(M, streams, device=dev, dtype=f32)
-    # hc3 path: per-channel parameter gradients via two skinny wgmma GEMMs instead of in-kernel accumulators
-    split = x_expand is None and d <= 1024 and HC_BWD_SPLIT
-    w = torch.empty(M * streams, 8, device=dev, dtype=bf16) if split else None
-    wy = torch.empty(M, 8, device=dev, dtype=bf16) if split else None
     nbytes = M * d * ((4 + 8 + 2 + 4 if x_expand is not None else 8 + 2 + 8 + 2 + 8 + 2) + (2 if dbin_extra is not None else 0))
     with _timed("hc_pre_bwd", nbytes, "byte"):
         _lib.call("alm_hc_pre_bwd", R_in, Y, beta_prev, x_expand, *_hc_param_ptrs(hc, ln_gamma), aux, dR_out, dxn,
                   dbin_extra, dbeta, dR_in, dY, dbp, dx, float(dx_scale),
                   grads["gamma"], grads["dyn_alpha"], grads["dyn_beta"], grads["static_alpha"], grads["static_beta"],
-                  grads["alpha_scale"], grads["beta_scale"], g_ln_gamma, w, wy, M, d, streams)
-    if split:
-        G = torch.zeros(d, 8, device=dev, dtype=f32)
-        rows = M * streams
-        sk = max(1, min(64, (rows // 64) // 8, 2 * num_sms(dev) // max(1, (d + 127) // 128)))
-        # (HBM-bound: they stream R_in / Y once; kept out of the tensor-bound GEMM class of the roofline)
-        gemm(R_in.view(rows, d), w, a_mn=True, b_mn=True, out=G, acc_mode=2, split_k=sk, cls="gemm_skinny_hc_param_grad")
-        sk = max(1, min(64, (M // 64) // 8, 2 * num_sms(dev) // max(1, (d + 127) // 128)))
-        gemm(Y, wy, a_mn=True, b_mn=True, out=G, acc_mode=2, split_k=sk, cls="gemm_skinny_hc_param_grad")
-        _lib.call("alm_hc_param_finish", G, hc["gamma"], hc["dyn_alpha"], hc["dyn_beta"], grads["gamma"],
-                  grads["dyn_alpha"], grads["dyn_beta"], d)
+                  grads["alpha_scale"], grads["beta_scale"], g_ln_gamma, M, d, streams)
     return dx if x_expand is not None else (dR_in, dY, dbp)
 
 

@@ -263,14 +263,14 @@ class _StackFn(torch.autograd.Function):
 # ----------------------------------------------------------------------------------------------
 class _HyperStreams:
     """num_residual_streams == 4: a bf16 [M, 4, d] stream; depth (of the previous branch), width and LayerNorm are one
-    hc_pre kernel, which always writes `bin`.  Saves per step its inputs (R, Y, beta) and the kernel's aux state; the
+    hc_pre kernel, which writes `bin` only when the branch asks for it.  Saves per step its inputs (R, Y, beta) and the kernel's aux state; the
     exit saves its LN stats."""
 
     def __init__(self, save):
         self.saved = [] if save else None
 
-    def _pre(self, inputs, hc, gamma):
-        self.R, bin_, xn, self.beta, aux = ops.hc_pre_fwd(hc, gamma, **inputs, M=self.M, d=self.d)
+    def _pre(self, inputs, hc, gamma, want_bin=True):
+        self.R, bin_, xn, self.beta, aux = ops.hc_pre_fwd(hc, gamma, **inputs, M=self.M, d=self.d, want_bin=want_bin)
         if self.saved is not None:
             self.saved.append((inputs, aux))
         return xn, bin_
@@ -280,7 +280,7 @@ class _HyperStreams:
         return self._pre(dict(x_expand=x2), hc, gamma)
 
     def step(self, Y, hc, gamma, want_bin):
-        return self._pre(dict(R_in=self.R, Y=Y, beta_prev=self.beta), hc, gamma)
+        return self._pre(dict(R_in=self.R, Y=Y, beta_prev=self.beta), hc, gamma, want_bin)
 
     def exit(self, Y, gamma):
         out, stats = ops.hc_post_fwd(self.R, Y, self.beta, gamma, M=self.M, d=self.d)

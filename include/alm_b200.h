@@ -214,7 +214,8 @@ int alm_decode_stack_step(const void* layer_table, int n_layers, const float* x,
  *            (or R_s = x_expand for all s: expand_streams, audiolm_pytorch.py:524)
  *   bin, R_out = width connection of this branch (dynamic+static alpha/beta, RMSNorm over channels)
  *   xn     = LayerNorm(bin) * ln_gamma       the branch's pre-norm (audiolm_pytorch.py:347, 254)
- * aux [M, 54] keeps the tanh activations, 1/|R_s|, the pre-activations z and the LN mean/rstd for the backward.
+ * aux [M, 56] keeps the tanh activations, 1/|R_s|, the pre-activations z and the LN mean/rstd for the backward.
+ * bin may be NULL when no consumer needs the un-normalised branch input.
  * Replaces hyper_connections.HyperConnections.forward as used at audiolm_pytorch.py:446-454,
  * 528-547 (third-party; restated in oracle/third_party.py).  Only streams == 4 is built.
  */
@@ -230,16 +231,13 @@ int alm_hc_pre_bwd(const void* R_in, const void* Y, const float* beta_prev, cons
                    const void* dbin_extra, const float* dbeta, void* dR_in, void* dY, float* dbeta_prev,
                    float* dx_expand, float dx_scale, float* g_gamma_hc, float* g_dyn_alpha, float* g_dyn_beta,
                    float* g_static_alpha, float* g_static_beta, float* g_alpha_scale, float* g_beta_scale,
-                   float* g_ln_gamma, void* w_out, void* wy_out, int M, int d, int streams, alm_stream_t stream);
+                   float* g_ln_gamma, int M, int d, int streams, alm_stream_t stream);
 /*
- * alm_hc_pre_bwd with w_out / wy_out (both or neither; d <= 1024, not the expand branch): the kernel leaves the
- * per-channel parameter gradients (gamma_hc, dyn_alpha, dyn_beta) to the caller and writes
- *   w_out [M*4, 8] bf16 = inv_s * dz[t,s,c] (c < 6, zero padded),  wy_out [M, 8] bf16 = sum_s beta_prev_s * w[t,s,:]
- * so that G [d, 8] = R_in^T w_out + Y^T wy_out (two skinny alm_gemm_bf16 calls, MN-major operands) and
- * alm_hc_param_finish adds  g_dyn_alpha += g1*G[:, :5], g_dyn_beta += g1*G[:,5], g_gamma_hc += sqrt(d)*sum_c P_c G_c.
+ * alm_hc_pre_bwd atomically adds every parameter gradient (the hyper-connection parameters and ln_gamma) into the
+ * g_* buffers.  dbin_extra (the gradient of `bin` from a consumer other than the LayerNorm) may be NULL.  For
+ * d <= 1024 every per-token input (R_in, Y, beta_prev, x_expand, aux, dR_out, dxn, dbin_extra, dbeta) must be
+ * 16-B aligned.
  */
-int alm_hc_param_finish(const float* G, const float* gamma_hc, const float* dyn_alpha, const float* dyn_beta,
-                        float* g_gamma_hc, float* g_dyn_alpha, float* g_dyn_beta, int d, alm_stream_t stream);
 /* last depth connection + reduce_streams (sum) + final LayerNorm (audiolm_pytorch.py:551-555) */
 int alm_hc_post_fwd(const void* R_in, const void* Y, const float* beta_prev, const float* ln_gamma, void* out,
                     float* stats, int M, int d, int streams, alm_stream_t stream);

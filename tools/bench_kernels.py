@@ -60,18 +60,23 @@ if "hc" in which:
     lng = rnd(d, dt=f32)
     R, Y, bp = rnd(M, 4, d), rnd(M, d), rnd(M, 4, dt=f32)
     timeit("hc_pre_fwd", lambda: ops.hc_pre_fwd(hc, lng, R_in=R, Y=Y, beta_prev=bp, M=M, d=d), nbytes=M * d * 22)
+    timeit("hc_pre_fwd (no bin)", lambda: ops.hc_pre_fwd(hc, lng, R_in=R, Y=Y, beta_prev=bp, M=M, d=d, want_bin=False),
+           nbytes=M * d * 20)
     R_out, bin_, xn, beta, aux = ops.hc_pre_fwd(hc, lng, R_in=R, Y=Y, beta_prev=bp, M=M, d=d)
+    x = rnd(M, d, dt=f32)
+    aux_x = ops.hc_pre_fwd(hc, lng, x_expand=x, M=M, d=d)[4]
     dR, dxn, dbe, dbin = rnd(M, 4, d), rnd(M, d), rnd(M, 4, dt=f32), rnd(M, d)
     grads = {k_: torch.zeros_like(v_) for k_, v_ in hc.items()}
     gl = torch.zeros_like(lng)
 
-    def hcb():
-        return ops.hc_pre_bwd(hc, lng, grads, gl, aux, dR, dxn, dbe, dbin_extra=dbin, R_in=R, Y=Y, beta_prev=bp, M=M, d=d)
+    def hcb(extra):
+        return ops.hc_pre_bwd(hc, lng, grads, gl, aux, dR, dxn, dbe, dbin_extra=extra, R_in=R, Y=Y, beta_prev=bp, M=M,
+                              d=d)
 
-    timeit("hc_pre_bwd (+2 skinny gemm+finish)", hcb, nbytes=M * d * 32)
-    ops.HC_BWD_SPLIT = False
-    timeit("hc_pre_bwd hc2 (in-kernel pgrads)", hcb, nbytes=M * d * 32)
-    ops.HC_BWD_SPLIT = True
+    timeit("hc_pre_bwd (dbin_extra)", lambda: hcb(dbin), nbytes=M * d * 32)
+    timeit("hc_pre_bwd (no dbin_extra)", lambda: hcb(None), nbytes=M * d * 30)
+    timeit("hc_pre_bwd (expand)", lambda: ops.hc_pre_bwd(hc, lng, grads, gl, aux_x, dR, dxn, dbe, dbin_extra=dbin,
+                                                         x_expand=x, dx_scale=0.5, M=M, d=d), nbytes=M * d * 20)
 
 if "attn" in which:
     q, k, v = rnd(16, 2048, 512), rnd(16, 2048, 64), rnd(16, 2048, 64)
