@@ -101,6 +101,8 @@ def load() -> C.CDLL:
     lib.alm_gemm_head_ce_tiles.argtypes = [I]
     lib.alm_decode_stack_grid.restype = I
     lib.alm_decode_stack_grid.argtypes = []
+    lib.alm_decode_stack_plan.restype = I
+    lib.alm_decode_stack_plan.argtypes = [I, I, I, I, I, P]
     lib.alm_decode_stack_trace_offset.restype = L
     lib.alm_decode_stack_trace_offset.argtypes = [I, I, I, I]
     for name, argtypes in SIGNATURES.items():

@@ -951,6 +951,22 @@ inline SmemPlan smem_plan(int L, int b, int d, int H, int ip, int grid) {
   return p;
 }
 
+constexpr size_t SMEM_LIMIT = 224 * 1024;   // dynamic shared memory the kernel is allowed
+
+// Every shape limit of the kernel, in one place: alm_decode_stack_plan reports it to the host (which falls back to the
+// multi-kernel step for a refused shape) and alm_decode_stack_step refuses exactly these shapes.  Fills *plan.
+inline bool shape_supported(int L, int b, int d, int H, int inner, int grid, SmemPlan* plan) {
+  if (b < 1 || b > MAXB || H < 1 || H > 64 || L < 1 || L > MAXL) return false;
+  if (d % 8 != 0 || d < 8 || d > 2 * MAXP * NT || inner < 1 || inner > 8 * MAXG * NT - 8) return false;
+  const int ip = (inner + 7) & ~7, HD = H * DH;
+  // a thread owns one 8-channel chunk of K; per-warp partial sums of a phase must fit the shared-memory table
+  const int Ns[4] = {HD + 2 * DH, d, 2 * ip, d}, Ks[4] = {d, HD, d, ip};
+  for (int i = 0; i < 4; ++i)
+    if (Ks[i] / 8 > NT || ceil_div(Ns[i], grid) * ceil_div(Ks[i] / 8, 32) > MAX_SLOTS) return false;
+  *plan = smem_plan(L, b, d, H, ip, grid);
+  return plan->total <= SMEM_LIMIT;
+}
+
 struct Scratch {
   size_t counter, err, q, kvn, part, Y, Y2, h, trace, total;
 };
@@ -996,6 +1012,14 @@ extern "C" int64_t alm_decode_stack_scratch_bytes(int b, int d, int heads, int i
   return (int64_t)dstep::scratch_layout(b, d, heads, ip, dstep::pick_splits(b)).total;
 }
 
+extern "C" int alm_decode_stack_plan(int b, int d, int heads, int inner, int n_layers, int32_t* staged) {
+  dstep::SmemPlan plan;
+  if (!dstep::shape_supported(n_layers, b, d, heads, inner, num_sms(), &plan)) return ALM_ERR_UNSUPPORTED;
+  if (staged != nullptr)
+    for (int i = 0; i < 4; ++i) staged[i] = plan.st_off[i] >= 0;
+  return ALM_OK;
+}
+
 extern "C" int alm_decode_stack_step(const void* layer_table, int n_layers, const float* x, void* out,
                                      const float* final_gamma, int32_t* len, int max_len, int64_t cache_bstride,
                                      const void* key_mask, int64_t mask_bstride, void* scratch, int64_t scratch_bytes,
@@ -1003,28 +1027,20 @@ extern "C" int alm_decode_stack_step(const void* layer_table, int n_layers, cons
                                      int grid_ctas, alm_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ALM_REQUIRE(layer_table && x && out && final_gamma && len && scratch && n_layers > 0, ALM_ERR_ARG);
-  ALM_REQUIRE(b >= 1 && b <= dstep::MAXB && heads >= 1 && heads <= 64 && max_len > 0 && n_layers <= dstep::MAXL, ALM_ERR_UNSUPPORTED);
-  ALM_REQUIRE(d % 8 == 0 && d >= 8 && d <= 2 * dstep::MAXP * dstep::NT && inner >= 1 && inner <= 8 * dstep::MAXG * dstep::NT - 8, ALM_ERR_UNSUPPORTED);
+  ALM_REQUIRE(max_len > 0, ALM_ERR_UNSUPPORTED);
   ALM_REQUIRE(cache_bstride % 8 == 0 && (reinterpret_cast<uintptr_t>(scratch) & 255u) == 0, ALM_ERR_ALIGN);
-  const int ip = (inner + 7) & ~7;
-  const int splits = dstep::pick_splits(b);
   const int grid = num_sms();
   ALM_REQUIRE(grid_ctas == grid, ALM_ERR_ARG);   // the operands were regrouped for this many CTAs
+  dstep::SmemPlan plan;
+  ALM_REQUIRE(dstep::shape_supported(n_layers, b, d, heads, inner, grid, &plan), ALM_ERR_UNSUPPORTED);
+  const int ip = (inner + 7) & ~7;
+  const int splits = dstep::pick_splits(b);
   const dstep::Scratch lay = dstep::scratch_layout(b, d, heads, ip, splits);
   ALM_REQUIRE(scratch_bytes >= (int64_t)lay.total, ALM_ERR_ARG);
-  {  // a thread owns one 8-channel chunk of K; per-warp partial sums of a phase must fit the shared-memory table
-    const int HD = heads * dstep::DH;
-    const int Ns[4] = {HD + 2 * dstep::DH, d, 2 * ip, d}, Ks[4] = {d, HD, d, ip};
-    for (int i = 0; i < 4; ++i) {
-      ALM_REQUIRE(Ks[i] / 8 <= dstep::NT, ALM_ERR_UNSUPPORTED);
-      ALM_REQUIRE(ceil_div(Ns[i], grid) * ceil_div(Ks[i] / 8, 32) <= dstep::MAX_SLOTS, ALM_ERR_UNSUPPORTED);
-    }
-  }
-  const dstep::SmemPlan plan = dstep::smem_plan(n_layers, b, d, heads, ip, grid);
-  ALM_REQUIRE(plan.total <= 224 * 1024, ALM_ERR_UNSUPPORTED);
   static bool attr = false;
   if (!attr) {
-    ALM_CUDA_OK(cudaFuncSetAttribute(dstep::decode_stack_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+    ALM_CUDA_OK(cudaFuncSetAttribute(dstep::decode_stack_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)dstep::SMEM_LIMIT));
     attr = true;
   }
   uint8_t* sc = reinterpret_cast<uint8_t*>(scratch);

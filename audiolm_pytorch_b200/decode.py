@@ -86,11 +86,12 @@ class StackDecoder:
         return self._fused
 
     def fused_ok(self):
-        """the one-kernel step covers the 4-stream stack without an attention bias"""
+        """the one-kernel step covers the 4-stream stack without an attention bias, at the sizes its kernel takes
+        (ops.decode_stack_plan); everything else runs the multi-kernel step"""
         tr = self.tr
-        inner = tr.layers[0][2].branch.inner
-        return (FUSED_STACK_STEP and self.b <= ops.DECODE_STEP_MAX_ROWS and tr.dim <= 2048 and tr.heads <= 64
-                and inner <= 4096 and tr.depth <= 64 and tr.num_residual_streams == 4 and self.bias is None)
+        return (FUSED_STACK_STEP and self.b <= ops.DECODE_STEP_MAX_ROWS and tr.num_residual_streams == 4
+                and self.bias is None
+                and ops.decode_stack_plan(self.b, tr.dim, tr.heads, tr.layers[0][2].branch.inner, tr.depth) is not None)
 
     def barrier_timeouts(self) -> int:
         """sticky error flag of the one-kernel step (a device-wide barrier gave up waiting); 0 when healthy"""

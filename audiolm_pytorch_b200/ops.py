@@ -5,6 +5,9 @@ stream.  No function has a CPU or stock-PyTorch implementation.
 """
 from __future__ import annotations
 
+import ctypes
+import functools
+
 import torch
 
 from . import _lib
@@ -394,6 +397,16 @@ def decode_stack_scratch(b, d, heads, inner, device):
 def decode_stack_grid():
     """CTAs of the one-kernel decode step (= SMs); the engine regroups its operands for this count."""
     return int(_lib.load().alm_decode_stack_grid())
+
+
+@functools.lru_cache(maxsize=None)
+def decode_stack_plan(b, d, heads, inner, n_layers):
+    """None if alm_decode_stack_step refuses this shape on the current device, else for phases A, C, D, E (q|kv, out,
+    W1, W2 projections) whether the weight rows are staged in shared memory (True) or read from L2 (False)."""
+    staged = (ctypes.c_int32 * 4)()
+    if _lib.load().alm_decode_stack_plan(b, d, heads, inner, n_layers, staged) != 0:
+        return None
+    return tuple(bool(s) for s in staged)
 
 
 def regroup_rows(w, grid):

@@ -200,6 +200,10 @@ int alm_ce_finish(const float* part, int tiles, const float* lab_logit, const in
  *   at position *len and *len is incremented by the kernel.  scratch: alm_decode_stack_scratch_bytes() bytes, 256-B
  *   aligned, owned by the caller; its first word pair is {barrier counter, sticky error flag (1 = a barrier timed out)}. */
 int alm_decode_stack_grid(void);
+/* Whether alm_decode_stack_step takes this shape on the current device: ALM_OK or ALM_ERR_UNSUPPORTED (the same test
+ * the step applies).  For an accepted shape, staged[0..3] (may be null) tells for phases A, C, D, E ([to_q ; to_kv],
+ * to_out, W1, W2) whether a CTA's weight rows are staged in shared memory (1) or read from L2 (0). */
+int alm_decode_stack_plan(int b, int d, int heads, int inner, int n_layers, int32_t* staged);
 int64_t alm_decode_stack_scratch_bytes(int b, int d, int heads, int inner);
 int64_t alm_decode_stack_trace_offset(int b, int d, int heads, int inner); /* debugging: phase stamps of -DALM_DSTEP_TRACE builds */
 int alm_decode_stack_step(const void* layer_table, int n_layers, const float* x, void* out, const float* final_gamma,

@@ -198,6 +198,30 @@ def test_regroup_rows_layout_of_the_decode_step_operands():
                 assert torch.equal(wp[c * pc + l], want), (N, grid, c, l)
 
 
+def test_one_kernel_decode_step_envelope_comes_from_its_plan():
+    """StackDecoder.fused_ok() takes the one-kernel step only for shapes alm_decode_stack_plan accepts.  At d = 1280
+    (and up to 1536) the W1 projection's per-warp partial sums (columns per CTA x warps per column) overflow the
+    kernel's table on an H100 (132 or 114 SMs), so a 4-stream model of that width decodes on the multi-kernel step."""
+    from audiolm_pytorch_b200 import decode, ops
+    from audiolm_pytorch_b200.transformer import Transformer
+
+    assert ops.decode_stack_plan(1, 1024, 8, 2730, 6) == (True, True, True, True)   # config C5: every phase staged
+    for d in (1280, 1536):
+        assert ops.decode_stack_plan(2, d, 8, int(d * 8 / 3), 1) is None, d
+    assert ops.decode_stack_plan(5, 64, 4, 170, 1) is None          # rows per step
+    assert ops.decode_stack_plan(1, 64, 65, 170, 1) is None         # heads
+    assert ops.decode_stack_plan(1, 64, 4, 170, 65) is None         # layers
+    assert ops.decode_stack_plan(1, 64, 4, 170, 64) is not None
+    default = decode.FUSED_STACK_STEP
+    decode.FUSED_STACK_STEP = True
+    try:
+        for d, want in ((1024, True), (1280, False), (1536, False)):
+            tr = Transformer(dim=d, depth=1, heads=8, flash_attn=True)
+            assert decode.StackDecoder(tr, 2, 16).fused_ok() is want, d
+    finally:
+        decode.FUSED_STACK_STEP = default
+
+
 def test_deferred_heads_flag_is_scoped_to_the_loss_forward():
     """the wrappers switch the transformers to LazyLogits only while they compute a loss; the flag is reset on exit and
     on exceptions, and heads.FUSED_HEAD_CE = False disables it (public forward signatures stay the reference's)."""
