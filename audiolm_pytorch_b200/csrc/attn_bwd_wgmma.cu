@@ -6,8 +6,10 @@
 //     dV += P^T dO   (P^T as register A operand)
 //     dK += dS^T Q,  dQ_partial = dS K   (dS^T stored as bf16 in smem, read K-major for dK and MN-major for dQ)
 // dV / dK accumulate in registers over all heads (MQA shares k/v: no atomics).  The partial dQ of each tile is
-// reduced into an fp32 workspace [b, n_q, h*64] with red.global.add; the host zeroes it beforehand (alm_attn_delta)
-// and converts it to bf16 dq afterwards.
+// staged in shared memory and reduce-added into an fp32 workspace [b, n_q, h*64] by TMA
+// (cp.reduce.async.bulk.tensor, two boxes per warpgroup and tile); the host zeroes it beforehand (alm_attn_delta) and
+// converts it to bf16 dq afterwards.  The elementwise phases (P^T, dS^T) are branch-free: masked, causal and tail
+// elements enter the exponential as -inf, so a key mask that differs between the rows of a warp costs no divergence.
 //
 // Q/K/V/dO tiles arrive by TMA (SWIZZLE_128B); the SAME smem tile serves as a K-major operand
 // (contraction over the 64-wide head dim) and as an MN-major operand (contraction over its 128 rows).
@@ -18,6 +20,8 @@
 // overlaps the dS arithmetic.  The two warpgroups meet once per iteration, on a named barrier, when both halves of
 // dS^T are in shared memory; dS^T is double-buffered so that barrier also orders its reuse.  Past that barrier both
 // have released the previous iteration's slot, so warp 0 refills it without waiting: STAGES - 1 loads stay ahead.
+// The same barrier frees a warpgroup's own key rows of the other dS^T slot (16 KB) until it writes its next dS^T
+// there, and that is where its dQ partial is staged: no extra shared memory.
 // With DROPOUT (keep mask Z from alm_common.cuh: dropout_keep, regenerated here, never stored):
 //     dV += (P^T o Z / (1-p)) dO,   dP^T <- dP^T o Z / (1-p),   dS^T = P^T (dP^T - delta)
 // delta = rowsum(dO o O) needs no change because O is the dropped output.  One thread's two key rows by its query
@@ -106,12 +110,27 @@ __device__ __forceinline__ uint64_t attn_bwd_keep_bits(const DropoutArgs& d, uin
 constexpr int AB_DS_TILE = AB_T * AB_T * 2;   // dS^T tile [128 keys][128 queries] bf16 = 32 KB
 constexpr int AB_SMEM = AB_TILE * (2 + 2 * AB_STAGES) + 2 * AB_DS_TILE + AB_STAGES * 2 * 512 + 256;
 constexpr uint32_t AB_DS_BAR = 1;             // named barrier of the two consumer warpgroups (0 is __syncthreads)
+constexpr uint32_t AB_WG_BAR = 2;             // + cw: named barrier of consumer warpgroup cw alone
+
+// Diagnostic build (-DALM_ATTN_BWD_TRACE, tools/attn_bwd_probe.py): warp 0 of each consumer warpgroup of CTA 0 writes
+// clock64() at the phase boundaries of its first AB_TRACE_ITERS iterations; alm_attn_bwd_trace_read copies them out.
+constexpr int AB_TRACE_ITERS = 128, AB_TRACE_STAMPS = 8;
+#ifdef ALM_ATTN_BWD_TRACE
+__device__ long long g_attn_bwd_trace[2][AB_TRACE_ITERS][AB_TRACE_STAMPS];
+#define AB_STAMP(i)                                                                                   \
+  do {                                                                                                \
+    if (blockIdx.x == 0 && (threadIdx.x & 127) == 0 && it < AB_TRACE_ITERS)                           \
+      g_attn_bwd_trace[threadIdx.x >> 7][it][i] = clock64();                                          \
+  } while (0)
+#else
+#define AB_STAMP(i)
+#endif
 
 template <bool HAS_BIAS, bool DROPOUT>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
-                    const AttnBwdParams p, const DropoutArgs drop) {
+                    const __grid_constant__ CUtensorMap tmdQ, const AttnBwdParams p, const DropoutArgs drop) {
   extern __shared__ __align__(1024) uint8_t smem[];
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint8_t* sK = smem;
@@ -139,6 +158,7 @@ mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmdO);
+    tma_prefetch_desc(&tmdQ);
     mbar_init(kv_full, 1);
     for (int i = 0; i < AB_STAGES; ++i) { mbar_init(&qdo_full[i], 1); mbar_init(&qdo_empty[i], 8); }
     fence_mbar_init();
@@ -189,7 +209,7 @@ mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   for (int e = 0; e < 32; ++e) { dv[e] = 0.f; dk[e] = 0.f; }
   const uint32_t k_all = smem_u32(sK);
   const uint32_t k_addr = k_all + cw * 8192, v_addr = smem_u32(sV) + cw * 8192;
-  const long long dq_ld = (long long)p.h * AB_D;
+  const bool wg_leader = (threadIdx.x & 127) == 0;   // issues this warpgroup's dQ reduce-adds
   if (n_iter > 0) mbar_wait(kv_full, 0);
   int stage = 0;
   uint32_t phase = 0;
@@ -197,7 +217,9 @@ mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     const int head = it / q_per_head;
     const int q0 = (qb_min + it % q_per_head) * AB_T;
     [[maybe_unused]] const long long bias_head = HAS_BIAS ? (long long)head * p.bias_hs : 0;
+    AB_STAMP(0);
     mbar_wait(&qdo_full[stage], phase);
+    AB_STAMP(1);
     const uint32_t q_addr = smem_u32(sQ + stage * AB_TILE), do_addr = smem_u32(sdO + stage * AB_TILE);
     const uint32_t ds_addr = smem_u32(sDS + (it & 1) * AB_DS_TILE);
     // S^T = K Q^T and dP^T = V dO^T as two commit groups: the exponentials run while dP^T is computed
@@ -213,22 +235,27 @@ mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       wgmma_ss<AB_T>(dpt, wgmma_desc_sw128(v_addr + k * 32, 1024, 16), wgmma_desc_sw128(do_addr + k * 32, 1024, 16),
                      k > 0 ? 1u : 0u);
     wgmma_commit();
+    AB_STAMP(2);
     [[maybe_unused]] uint64_t keep = 0;
     if constexpr (DROPOUT)
       keep = attn_bwd_keep_bits(drop, ((uint32_t)batch * p.h + head) * (uint32_t)p.n_q_pad + q0 + c_lane, kj[0]);
     const float* lse_s = sLse + stage * AB_T;
     const float* del_s = sDelta + stage * AB_T;
-    // whole tile below the causal diagonal and inside n_q: only the per-row key flag matters
+    // key row kj[h] sees query qi iff key_ok[h] and q_lo[h] <= qi < q_end; a whole tile below the causal diagonal
+    // and inside n_q needs no range test.  Every per-element decision below is a select, never a branch: a branch
+    // around the exponential diverges wherever the key mask differs between the rows of a warp.
     const bool tile_full = (q0 + AB_T <= p.n_q) && (!p.causal || k0 + AB_T - 1 <= q0 + off);
-    auto visible = [&](int h, int qi) {
-      return key_ok[h] && (tile_full || (qi < p.n_q && (!p.causal || kj[h] <= qi + off)));
-    };
+    const int q_end = tile_full ? INT_MAX : p.n_q;
+    int q_lo[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) q_lo[h] = tile_full || !p.causal ? INT_MIN : kj[h] - off;
+    auto visible = [&](int h, int qi) { return key_ok[h] & (qi >= q_lo[h]) & (qi < q_end); };
     auto bias_index = [&](int h, int qi) {
       return bias_head + (long long)min(qi, p.n_q - 1) * p.bias_rs + min(kj[h], p.n_k - 1);
     };
     wgmma_wait<1>();
     wgmma_fence_acc(st);
-    // P^T = exp(S^T * scale - lse), kept in fp32 for dS
+    // P^T = exp(S^T * scale - lse), kept in fp32 for dS; invisible elements get ex2(-inf) = 0
 #pragma unroll
     for (int g = 0; g < AB_T / 8; ++g)
 #pragma unroll
@@ -241,9 +268,11 @@ mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
           const int e = 4 * g + 2 * h + c;
           float shift = -lv;
           if constexpr (HAS_BIAS) shift = fmaf(__ldg(p.bias + bias_index(h, qi)), LOG2E, shift);
-          st[e] = visible(h, qi) ? ex2_approx(fmaf(st[e], p.scale_log2, shift)) : 0.f;
+          const float x = fmaf(st[e], p.scale_log2, shift);
+          st[e] = ex2_approx(visible(h, qi) ? x : -INFINITY);
         }
       }
+    AB_STAMP(3);
     // dV += P^T dO runs under the dS arithmetic
     uint32_t pa[8][4];
     if constexpr (DROPOUT) {
@@ -262,6 +291,11 @@ mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     wgmma_commit();
     wgmma_wait<1>();
     wgmma_fence_acc(dpt);
+    // this warpgroup's rows of the dS^T slot staged the previous tile's dQ partial: its reduce must have read them
+    if (it > 0) {
+      if (wg_leader) bulk_wait_group_read<0>();
+      named_bar_sync(AB_WG_BAR + cw, 128);
+    }
     // dS^T = scale * P^T (dP^T - delta), stored as bf16 into the 128-B-swizzled dS^T tile: two 16-KB halves of
     // [128 keys][64 queries]; one half is the K-major A operand of dK (contraction over queries) and, read MN-major,
     // the A operand of dQ (contraction over keys)
@@ -294,8 +328,10 @@ mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         st_shared_u32(a, pack_bf16x2(dpt[4 * g + 2 * h], dpt[4 * g + 2 * h + 1]));
       }
     }
+    AB_STAMP(4);
     fence_proxy_async_smem();
     named_bar_sync(AB_DS_BAR, 2 * 128);  // both halves of dS^T written before either warpgroup reads them for dQ
+    AB_STAMP(5);
     // both warpgroups are past iteration it - 1 and have released its slot, so this wait does not block: refill it
     if (warp == 0 && it >= 1 && it - 1 + AB_STAGES < n_iter) {
       const int prev = stage == 0 ? AB_STAGES - 1 : stage - 1;
@@ -319,19 +355,35 @@ mqa_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     wgmma_fence_acc(dv);
     wgmma_fence_acc(dk);
     wgmma_fence_acc(dq);
+    AB_STAMP(6);
     if (lane == 0) mbar_arrive(&qdo_empty[stage]);
-    // partial dQ -> fp32 workspace (fire-and-forget reductions in L2)
+    // partial dQ -> fp32 workspace: staged in this warpgroup's own key rows of the OTHER dS^T slot (16 KB: rows
+    // [64 cw, 64 cw + 64) of both query halves), which nobody reads until this warpgroup rewrites them with dS^T of
+    // the next tile (the other warpgroup finished its dQ of tile it - 1 before the barrier above).  Each 8-KB half
+    // is a [64 queries][32 fp32] 128-B-swizzled box; one thread reduce-adds both into dq_acc by TMA, which clips
+    // the n_q tail.
+    const uint32_t stg = smem_u32(sDS + ((it + 1) & 1) * AB_DS_TILE) + cw * 8192;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int qi = q0 + cw * 64 + wl * 16 + (lane >> 2) + 8 * h;
-      if (qi < p.n_q) {
-        float* row = p.dq_acc + ((size_t)batch * p.n_q + qi) * dq_ld + head * AB_D + c_lane;
+      const int row = wl * 16 + (lane >> 2) + 8 * h;
 #pragma unroll
-        for (int g = 0; g < AB_D / 8; ++g) red_add_f32x2(row + 8 * g, dq[4 * g + 2 * h], dq[4 * g + 2 * h + 1]);
+      for (int g = 0; g < AB_D / 8; ++g) {
+        const int byte = 32 * (g & 3) + 4 * c_lane;
+        st_shared_f32x2(stg + (g >> 2) * (AB_DS_TILE / 2) + row * 128 + ((((byte >> 4) ^ (row & 7)) << 4) | (byte & 15)),
+                        dq[4 * g + 2 * h], dq[4 * g + 2 * h + 1]);
       }
     }
+    fence_proxy_async_smem();
+    named_bar_sync(AB_WG_BAR + cw, 128);
+    if (wg_leader) {
+      tma_reduce_add_3d(&tmdQ, stg, head * AB_D, q0 + cw * 64, batch);
+      tma_reduce_add_3d(&tmdQ, stg + AB_DS_TILE / 2, head * AB_D + 32, q0 + cw * 64, batch);
+      bulk_commit_group();
+    }
+    AB_STAMP(7);
     if (++stage == AB_STAGES) { stage = 0; phase ^= 1u; }
   }
+  if (wg_leader) bulk_wait_group<0>();
   // epilogue: dV, dK from registers
   __nv_bfloat16* rv[2];
   __nv_bfloat16* rk[2];
@@ -406,6 +458,14 @@ extern "C" int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64
     rc = make_tensor_map(&tmV, v, 2, 3, dims, strides, box, true);
     if (rc != ALM_OK) return rc;
   }
+  CUtensorMap tmdQ;  // fp32 dq_acc [b, n_q, h*64] in [64 queries][32 columns] boxes (128-B rows, swizzled)
+  {
+    uint64_t dims[3] = {(uint64_t)h * AB_D, (uint64_t)n_q, (uint64_t)b};
+    uint64_t strides[3] = {4, (uint64_t)h * AB_D * 4, (uint64_t)n_q * h * AB_D * 4};
+    uint32_t box[3] = {32, 64, 1};
+    int rc = make_tensor_map(&tmdQ, dq_acc, 4, 3, dims, strides, box, true);
+    if (rc != ALM_OK) return rc;
+  }
   AttnBwdParams p;
   p.lse = lse; p.delta = delta;
   p.kmask = reinterpret_cast<const uint32_t*>(key_mask);
@@ -430,13 +490,13 @@ extern "C" int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64
   dim3 grid(((n_k + AB_T - 1) / AB_T) * b);
   const bool drop = dropout_p > 0.f;
   if (bias != nullptr && drop)
-    mqa_attn_bwd_kernel<true, true><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p, dargs);
+    mqa_attn_bwd_kernel<true, true><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, tmdQ, p, dargs);
   else if (bias != nullptr)
-    mqa_attn_bwd_kernel<true, false><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p, dargs);
+    mqa_attn_bwd_kernel<true, false><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, tmdQ, p, dargs);
   else if (drop)
-    mqa_attn_bwd_kernel<false, true><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p, dargs);
+    mqa_attn_bwd_kernel<false, true><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, tmdQ, p, dargs);
   else
-    mqa_attn_bwd_kernel<false, false><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p, dargs);
+    mqa_attn_bwd_kernel<false, false><<<grid, AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, tmdQ, p, dargs);
   ALM_CHECK_LAUNCH();
   const long long rows = (long long)b * n_q;
   const int cols4 = h * AB_D / 4;
@@ -446,3 +506,11 @@ extern "C" int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64
   ALM_LAUNCHED(2);
   return ALM_OK;
 }
+
+#ifdef ALM_ATTN_BWD_TRACE
+// [2 warpgroups][AB_TRACE_ITERS][AB_TRACE_STAMPS] clock64 stamps of the last launch's CTA 0 -> host (synchronous)
+extern "C" int alm_attn_bwd_trace_read(long long* dst) {
+  ALM_CUDA_OK(cudaMemcpyFromSymbol(dst, alm::g_attn_bwd_trace, sizeof(alm::g_attn_bwd_trace)));
+  return ALM_OK;
+}
+#endif

@@ -106,6 +106,14 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* s
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
+// tensor reduce-add shared -> global (fp32 tensor maps: global += smem, in L2; out-of-bounds elements are skipped);
+// completion is tracked in bulk groups like tma_store_3d
+__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, uint32_t smem_src, int32_t c0, int32_t c1,
+                                                  int32_t c2) {
+  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // at most N of this thread's committed bulk groups still read their shared-memory source
 template <int N>
@@ -119,9 +127,8 @@ __device__ __forceinline__ void bulk_wait_group() {
 __device__ __forceinline__ void st_shared_u32(uint32_t smem_addr, uint32_t v) {
   asm volatile("st.shared.u32 [%0], %1;" ::"r"(smem_addr), "r"(v) : "memory");
 }
-// global fp32 reduction of two consecutive floats (8-B aligned), performed in L2 without a return value
-__device__ __forceinline__ void red_add_f32x2(float* gaddr, float a, float b) {
-  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(gaddr), "f"(a), "f"(b) : "memory");
+__device__ __forceinline__ void st_shared_f32x2(uint32_t smem_addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(smem_addr), "f"(a), "f"(b) : "memory");
 }
 // barrier over `nthreads` threads (a multiple of 32) on hardware barrier `id` (0 is __syncthreads')
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {

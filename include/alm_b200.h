@@ -99,10 +99,11 @@ int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int
 
 /*
  * Backward of alm_mqa_attn_fwd (one wgmma kernel per (batch, 128-key block): dK/dV accumulate over all heads in
- * registers, partial dQ products are reduced into dq_acc; a second kernel converts dq_acc to bf16 dq).
+ * registers, partial dQ products are reduce-added into dq_acc by TMA; a second kernel converts dq_acc to bf16 dq).
  * lse/delta are [b, h, n_q_pad] with n_q_pad a multiple of 128; delta = rowsum(dO * O) from alm_attn_delta.
- * dq_acc is an fp32 [b, n_q, h*64] contiguous workspace that must be zero on entry (alm_attn_delta zeroes it).
- * dq is summed with fp32 atomics, so it is not bitwise reproducible from run to run; dk and dv are.
+ * dq_acc is an fp32 [b, n_q, h*64] contiguous, 16-B aligned workspace that must be zero on entry (alm_attn_delta
+ * zeroes it).
+ * dq is summed with fp32 reductions in L2, so it is not bitwise reproducible from run to run; dk and dv are.
  * dropout_p / seed / site: those of the forward call (the mask is regenerated, not stored); with dropout_p > 0,
  * n_q_pad must be n_q rounded up to 128.
  * Autograd of attend.py:69-146.

@@ -85,6 +85,10 @@ if "attn" in which:
     o, lse = ops.mqa_attn_fwd(q, k, v, heads=8)
     do = rnd(16, 2048, 512)
     timeit("attn bwd (delta + fused + dq convert)", lambda: ops.mqa_attn_bwd(q, k, v, o, do, lse, heads=8), flops=2.5 * fl)
+    # the trainer always passes a key mask: ~15 % of keys dropped
+    km = ops.pack_key_mask(torch.rand(16, 2048, device=dev) > 0.15)
+    o, lse = ops.mqa_attn_fwd(q, k, v, heads=8, key_mask=km)
+    timeit("attn bwd, key mask", lambda: ops.mqa_attn_bwd(q, k, v, o, do, lse, heads=8, key_mask=km), flops=2.5 * fl)
 
 if "gemm" in which:
     from audiolm_pytorch_b200.transformer import best_split_k
