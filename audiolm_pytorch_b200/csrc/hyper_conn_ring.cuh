@@ -3,14 +3,14 @@
 //
 // One persistent CTA per SM with NC warpgroups; warpgroup c takes every NC-th token of the CTA.  Each warpgroup owns a
 // ring of NSC shared-memory stages, one token each, filled with 1-D bulk copies (cp.async.bulk completing on a full
-// mbarrier): the token's aux / dbeta / beta_prev scalars, R_in and dR_out [4, d], Y, dxn and dbin_extra [d] (x [d]
+// mbarrier): the token's aux / dbeta / beta_prev scalars, R_in and dR_out [S, d], Y, dxn and dbin_extra [d] (x [d]
 // fp32 instead of R_in and Y when the op expanded the streams).  While it computes one token, the next NSC - 1 are in
 // flight; a stage is refilled by the warpgroup itself once its reduction barrier shows that every thread is done with
 // the stage.  (There is no producer warp: a ninth warp per SM would cap every thread at 168 registers, 3 warps x 168
 // x 32 per quarter-SM register file, and the consumers need ~220.)  Thread l owns channels [8l, 8l + 8) of every
 // row, so the per-channel parameter gradients (gamma, dyn_alpha, dyn_beta, ln_gamma) stay in its registers for the
 // whole launch and are flushed once.  Per token:
-//   pass 1   every per-token dot product (34 sums) from the stage, one warpgroup reduction;
+//   pass 1   every per-token dot product (2 + 4S + S^2 sums, 34 at S = 4) from the stage, one warpgroup reduction;
 //   scalars  warp 0, one lane per (stream s, map column c): the tanh and RMS-norm backward coefficients;
 //   pass 2   dR_in, dY (or dx) and the parameter-gradient accumulators, again from the stage.
 // The RMS-norm backward needs no second reduction: with the forward's pre-activations z (kept in aux),
@@ -25,32 +25,38 @@
 namespace alm {
 namespace hcr {
 
-using hc2::AUX;
-using hc2::S;
-using hc2::T;
 constexpr int NC = 2;                   // warpgroups
 constexpr int NSC = 3;                  // ring stages per warpgroup (one token each)
 constexpr int NST = NC * NSC;
 constexpr int THREADS = NC * 128;
-constexpr int NRED = 34;                // pass-1 per-token sums
+constexpr int NRED = 34;                // pass-1 per-token sums, zero-padded: 2 + 4S + S*S <= 34 for S <= 4
 constexpr int MAILW = 36;               // floats per warp row of the reduction mailbox
-constexpr int COEF = 16;                // per-stream coefficient row: alpha[5], C[6], kk, pad
-constexpr int Z_OFF = S * T + S + S;    // aux: ta[20] tb[4] inv[4] z[24] pad[2] mean rstd
-constexpr int SCAL_B = 256;             // stage head: aux[AUX] dbeta[4] beta_prev[4] (fp32)
-static_assert(AUX * 4 + 32 == SCAL_B, "aux rows must be 16-B multiples so that one bulk copy stages a row");
+constexpr int COEF = 16;                // per-stream coefficient row: alpha[T], C[S + 2], kk, pad
+// The ring is built for S <= 4 streams: pass 1 then fits one reduce_scatter32 and warp 0's scalar phase one lane per
+// (stream, column) pair.
+__host__ __device__ constexpr bool ring_ok(int S) { return S >= 2 && S <= 4; }
+// Stage head: aux[AUX] then dbeta[S] and beta_prev[S] (fp32), 16-B aligned.  A bulk copy needs 16-B sizes and
+// addresses, so the [M, S] rows are staged only when S % 4 == 0; otherwise the kernel reads them from global memory.
+__host__ __device__ constexpr bool head_bulk(int S) { return S % 4 == 0; }
+__host__ __device__ constexpr int scal_bytes(int S) { return hc2::aux_floats(S) * 4 + (head_bulk(S) ? 8 * S : 0); }
+static_assert(scal_bytes(4) == 256, "the 4-stream stage head is 256 B");
+static_assert(scal_bytes(2) % 16 == 0 && scal_bytes(3) % 16 == 0 && scal_bytes(4) % 16 == 0,
+              "aux rows and the stage head must be 16-B multiples so that one bulk copy stages a row");
 
-// stage: scalars | R_in [4][d] bf16 (or x [d] fp32) | dR_out [4][d] | Y [d] | dxn [d] | dbin_extra [d]
-__host__ __device__ inline int off_dr(int d) { return SCAL_B + 8 * d; }
-__host__ __device__ inline int off_y(int d) { return SCAL_B + 16 * d; }
-__host__ __device__ inline int off_dxn(int d) { return SCAL_B + 18 * d; }
-__host__ __device__ inline int off_dbin(int d) { return SCAL_B + 20 * d; }
-__host__ __device__ inline int stage_bytes(int d) { return (SCAL_B + 22 * d + 127) / 128 * 128; }
-// shared memory: params [7][d] fp32 | mailboxes [NC][4][MAILW] | dbeta_prev partials [NC][4][S] | coefficients
-// [NC][S][COEF] | full[NST] mbarriers | ring [NC][NSC] stages (128-B aligned)
-__host__ __device__ inline int ring_offset(int d) {
-  return (4 * (7 * d + NC * (4 * MAILW + 4 * S + S * COEF)) + 8 * NST + 127) / 128 * 128;
+// stage: scalars | R_in [S][d] bf16 (or x [d] fp32) | dR_out [S][d] | Y [d] | dxn [d] | dbin_extra [d]
+template <int S> __host__ __device__ inline int off_dr(int d) { return scal_bytes(S) + 2 * S * d; }
+template <int S> __host__ __device__ inline int off_y(int d) { return scal_bytes(S) + 4 * S * d; }
+template <int S> __host__ __device__ inline int off_dxn(int d) { return off_y<S>(d) + 2 * d; }
+template <int S> __host__ __device__ inline int off_dbin(int d) { return off_y<S>(d) + 4 * d; }
+template <int S> __host__ __device__ inline int stage_bytes(int d) {
+  return (scal_bytes(S) + (4 * S + 6) * d + 127) / 128 * 128;
 }
-inline size_t smem_bytes(int d) { return (size_t)ring_offset(d) + (size_t)NST * stage_bytes(d); }
+// shared memory: params [S+3][d] fp32 | mailboxes [NC][4][MAILW] | dbeta_prev partials [NC][4][S] | coefficients
+// [NC][S][COEF] | full[NST] mbarriers | ring [NC][NSC] stages (128-B aligned)
+template <int S> __host__ __device__ inline int ring_offset(int d) {
+  return (4 * ((S + 3) * d + NC * (4 * MAILW + 4 * S + S * COEF)) + 8 * NST + 127) / 128 * 128;
+}
+template <int S> inline size_t smem_bytes(int d) { return (size_t)ring_offset<S>(d) + (size_t)NST * stage_bytes<S>(d); }
 
 // the per-channel parameters are stored so that thread l's channels 8l..8l+3 and 8l+4..8l+7 are two float4 at
 // [4l] and [d/2 + 4l]: a warp's 16-B loads are then contiguous (no bank-conflict replays)
@@ -83,7 +89,7 @@ __device__ __forceinline__ void lds8(const float* p, int half, float* f) {  // 8
   hc2::lds4(p + half, f + 4);
 }
 
-template <bool EXPAND>
+template <int S, bool EXPAND>
 __global__ void __launch_bounds__(THREADS, 1)
 pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __restrict__ Y,
                const float* __restrict__ beta_prev, const float* __restrict__ x_expand, hc2::Params prm,
@@ -92,14 +98,18 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
                const float* __restrict__ dbeta, __nv_bfloat16* __restrict__ dR_in, __nv_bfloat16* __restrict__ dY,
                float* __restrict__ dbeta_prev, float* __restrict__ dx_expand, float dx_scale, hc2::Grads gr, int M,
                int d) {
+  static_assert(ring_ok(S), "the ring backward is built for 2 to 4 streams");
+  constexpr int T = S + 1, AUX = hc2::aux_floats(S), Z_OFF = hc2::z_offset(S), SCAL_B = scal_bytes(S);
+  constexpr int NP = S + 3;  // per-channel parameter rows: ln_gamma, g1 * dyn_alpha[:, t] (T), g1 * dyn_beta
+  constexpr int NG = S + 2;  // map columns: T alpha columns and beta
   extern __shared__ __align__(128) unsigned char smem[];
-  float* sPar = reinterpret_cast<float*>(smem);  // [7][d]: ln_gamma, g1 * dyn_alpha[:, t], g1 * dyn_beta
-  float* sMail = sPar + 7 * d;                   // [NC][4][MAILW]
+  float* sPar = reinterpret_cast<float*>(smem);  // [NP][d]: ln_gamma, g1 * dyn_alpha[:, t], g1 * dyn_beta
+  float* sMail = sPar + NP * d;                  // [NC][4][MAILW]
   float* sDbp = sMail + NC * 4 * MAILW;          // [NC][4][S]
   float* sCoef = sDbp + NC * 4 * S;              // [NC][S][COEF]
   uint64_t* full = reinterpret_cast<uint64_t*>(sCoef + NC * S * COEF);
-  unsigned char* ring = smem + ring_offset(d);
-  const int stage_b = stage_bytes(d), half = d >> 1;
+  unsigned char* ring = smem + ring_offset<S>(d);
+  const int stage_b = stage_bytes<S>(d), half = d >> 1;
   const float sqrt_d = sqrtf((float)d);
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
     const int p = par_index(c, d);
@@ -127,27 +137,30 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
     const int ls = k % NSC;
     uint64_t* bar = my_full + ls;
     unsigned char* st = my_ring + (size_t)ls * stage_b;
-    const uint32_t bytes = (EXPAND ? SCAL_B - 16 + 4 * d : SCAL_B + 10 * d) + 10 * d + (has_dbin ? 2 * d : 0);
+    constexpr int head = AUX * 4 + (head_bulk(S) ? (EXPAND ? 4 * S : 8 * S) : 0);
+    const uint32_t bytes = head + (EXPAND ? 4 * d : (2 * S + 2) * d) + (2 * S + 2) * d + (has_dbin ? 2 * d : 0);
     if (lane == 0) mbar_arrive_expect_tx(bar, bytes);
     __syncwarp();
     const size_t md = (size_t)m * d;
     switch (lane) {
       case 0: bulk_copy_g2s(st, aux + (size_t)m * AUX, AUX * 4, bar); break;
-      case 1: bulk_copy_g2s(st + AUX * 4, dbeta + (size_t)m * S, 16, bar); break;
+      case 1:
+        if (head_bulk(S)) bulk_copy_g2s(st + AUX * 4, dbeta + (size_t)m * S, 4 * S, bar);
+        break;
       case 2:
-        if (!EXPAND) bulk_copy_g2s(st + AUX * 4 + 16, beta_prev + (size_t)m * S, 16, bar);
+        if (head_bulk(S) && !EXPAND) bulk_copy_g2s(st + AUX * 4 + 4 * S, beta_prev + (size_t)m * S, 4 * S, bar);
         break;
       case 3:
         if (EXPAND) bulk_copy_g2s(st + SCAL_B, x_expand + md, 4 * d, bar);
-        else bulk_copy_g2s(st + SCAL_B, R_in + md * S, 8 * d, bar);
+        else bulk_copy_g2s(st + SCAL_B, R_in + md * S, 2 * S * d, bar);
         break;
-      case 4: bulk_copy_g2s(st + off_dr(d), dR_out + md * S, 8 * d, bar); break;
+      case 4: bulk_copy_g2s(st + off_dr<S>(d), dR_out + md * S, 2 * S * d, bar); break;
       case 5:
-        if (!EXPAND) bulk_copy_g2s(st + off_y(d), Y + md, 2 * d, bar);
+        if (!EXPAND) bulk_copy_g2s(st + off_y<S>(d), Y + md, 2 * d, bar);
         break;
-      case 6: bulk_copy_g2s(st + off_dxn(d), dxn + md, 2 * d, bar); break;
+      case 6: bulk_copy_g2s(st + off_dxn<S>(d), dxn + md, 2 * d, bar); break;
       case 7:
-        if (has_dbin) bulk_copy_g2s(st + off_dbin(d), dbin_extra + md, 2 * d, bar);
+        if (has_dbin) bulk_copy_g2s(st + off_dbin<S>(d), dbin_extra + md, 2 * d, bar);
         break;
       default: break;
     }
@@ -156,12 +169,12 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
     for (int k = 0; k < NSC; ++k) fill(k);
   }
   {
-    float G[6][8], gLn[8];  // this thread's channels: G[c][e] = sum over its tokens of sum_s R_s C[s][c]; d ln_gamma
+    float G[NG][8], gLn[8];  // this thread's channels: G[c][e] = sum over its tokens of sum_s R_s C[s][c]; d ln_gamma
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       gLn[e] = 0.f;
 #pragma unroll
-      for (int c6 = 0; c6 < 6; ++c6) G[c6][e] = 0.f;
+      for (int c6 = 0; c6 < NG; ++c6) G[c6][e] = 0.f;
     }
     const int bar_id = 1 + cw;
     float* mail = sMail + cw * 4 * MAILW;
@@ -174,7 +187,8 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
     for (int s = 0; s < S; ++s) sa0[s] = prm.static_alpha[s * T];
     // scalar-phase role of warp 0's lanes: stream ss, column q (q < T: alpha column, q == T: beta, q == T + 1: kk)
     const int ss = lane >> 3, q = lane & 7;
-    const float stat = q < T ? prm.static_alpha[ss * T + q] : 0.f;
+    const bool sv = ss < S;  // (S < 4: the lanes of the missing streams stay idle)
+    const float stat = sv && q < T ? prm.static_alpha[ss * T + q] : 0.f;
     float small0 = 0.f, small1 = 0.f;  // q < T: d static_alpha, d alpha_scale part; q == T: d static_beta, d beta_scale part
     const float* pLn = sPar + lt * 4;
     int ls = 0;
@@ -189,7 +203,7 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
 #pragma unroll
       for (int s = 0; s < S; ++s) {
         alpha0[s] = fmaf(a[s * T], a_scale, sa0[s]);
-        bp[s] = EXPAND ? 0.f : a[AUX + S + s];
+        bp[s] = EXPAND ? 0.f : head_bulk(S) ? a[AUX + S + s] : beta_prev[(size_t)m * S + s];
       }
       const int c8 = lt * 8;
       // r[s][e] = R_in + beta_prev (x) Y  (or x)
@@ -205,7 +219,7 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
             for (int s = 0; s < S; ++s) r[s][e] = xv[e];
           }
         } else {
-          hc2::unpack8(*reinterpret_cast<const uint4*>(st + off_y(d) + 2 * c8), y);
+          hc2::unpack8(*reinterpret_cast<const uint4*>(st + off_y<S>(d) + 2 * c8), y);
 #pragma unroll
           for (int s = 0; s < S; ++s) {
             float rv[8];
@@ -216,17 +230,18 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
         }
       };
       // ---------------- pass 1 ----------------
-      // red: 0 sum gl | 1 sum gl*xhat | 2+s sum gl*R_s | 6+s sum R_s | 10+s sum xhat*R_s | 14+s sum ex*R_s |
-      //      18+4s+(t-1) sum dR_out[t-1]*R_s      (gl = dxn * ln_gamma, xhat = normalised branch input, ex = dbin_extra)
+      // red: 0 sum gl | 1 sum gl*xhat | 2+s sum gl*R_s | 2+S+s sum R_s | 2+2S+s sum xhat*R_s | 2+3S+s sum ex*R_s |
+      //      2+4S+S*s+(t-1) sum dR_out[t-1]*R_s  (gl = dxn * ln_gamma, xhat = normalised branch input, ex = dbin_extra;
+      //      S = 4: 2+s, 6+s, 10+s, 14+s, 18+4s+(t-1))
       float red[NRED];
 #pragma unroll
       for (int i = 0; i < NRED; ++i) red[i] = 0.f;
       if (act) {
         float r[S][8], y[8], dx[8], ex[8], lg[8];
         load_r(r, y);
-        hc2::unpack8(*reinterpret_cast<const uint4*>(st + off_dxn(d) + 2 * c8), dx);
+        hc2::unpack8(*reinterpret_cast<const uint4*>(st + off_dxn<S>(d) + 2 * c8), dx);
         if (has_dbin) {
-          hc2::unpack8(*reinterpret_cast<const uint4*>(st + off_dbin(d) + 2 * c8), ex);
+          hc2::unpack8(*reinterpret_cast<const uint4*>(st + off_dbin<S>(d) + 2 * c8), ex);
         } else {
 #pragma unroll
           for (int e = 0; e < 8; ++e) ex[e] = 0.f;
@@ -245,19 +260,22 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
 #pragma unroll
           for (int s = 0; s < S; ++s) {
             red[2 + s] = fmaf(gl, r[s][e], red[2 + s]);
-            red[6 + s] += r[s][e];
-            red[10 + s] = fmaf(xh, r[s][e], red[10 + s]);
-            red[14 + s] = fmaf(ex[e], r[s][e], red[14 + s]);
+            red[2 + S + s] += r[s][e];
+            red[2 + 2 * S + s] = fmaf(xh, r[s][e], red[2 + 2 * S + s]);
+            red[2 + 3 * S + s] = fmaf(ex[e], r[s][e], red[2 + 3 * S + s]);
           }
         }
 #pragma unroll
         for (int t = 1; t < T; ++t) {
           float dm[8];
-          hc2::unpack8(*reinterpret_cast<const uint4*>(st + off_dr(d) + 2 * ((t - 1) * d + c8)), dm);
+          hc2::unpack8(*reinterpret_cast<const uint4*>(st + off_dr<S>(d) + 2 * ((t - 1) * d + c8)), dm);
 #pragma unroll
           for (int e = 0; e < 8; ++e)
 #pragma unroll
-            for (int s = 0; s < S; ++s) red[18 + 4 * s + (t - 1)] = fmaf(dm[e], r[s][e], red[18 + 4 * s + (t - 1)]);
+            for (int s = 0; s < S; ++s) {
+              const int i = 2 + 4 * S + S * s + (t - 1);
+              red[i] = fmaf(dm[e], r[s][e], red[i]);
+            }
         }
       }
       {
@@ -285,9 +303,10 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
           dbeta_prev[(size_t)pend * S + lane] = (dbpm[lane] + dbpm[S + lane]) + (dbpm[2 * S + lane] + dbpm[3 * S + lane]);
         const float inv = a[S * T + S + ss];
         float zpart = 0.f, cst = 0.f;
-        if (q < T) {
-          const float dal = q == 0 ? fmaf(rstd, total(2 + ss) - m1 * total(6 + ss) - m2 * total(10 + ss), total(14 + ss))
-                                   : total(18 + 4 * ss + q - 1);
+        if (sv && q < T) {
+          const float dal = q == 0 ? fmaf(rstd, total(2 + ss) - m1 * total(2 + S + ss) - m2 * total(2 + 2 * S + ss),
+                                          total(2 + 3 * S + ss))
+                                   : total(2 + 4 * S + S * ss + q - 1);
           const float ta = a[ss * T + q];
           const float dw = dal * a_scale * (1.f - ta * ta);
           zpart = dw * a[Z_OFF + ss * T + q];
@@ -295,8 +314,8 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
           coef[ss * COEF + q] = fmaf(ta, a_scale, stat);  // alpha[s][q]
           small0 += dal;
           small1 = fmaf(dal, ta, small1);
-        } else if (q == T) {
-          const float tb = a[S * T + ss], dbe = a[AUX + ss];
+        } else if (sv && q == T) {
+          const float tb = a[S * T + ss], dbe = head_bulk(S) ? a[AUX + ss] : dbeta[(size_t)m * S + ss];
           const float dwb = dbe * b_scale * (1.f - tb * tb);
           zpart = dwb * a[Z_OFF + S * T + ss];
           cst = inv * dwb;
@@ -306,38 +325,40 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
         float zsum = zpart;
 #pragma unroll
         for (int o = 1; o < 8; o <<= 1) zsum += __shfl_xor_sync(0xffffffffu, zsum, o);
-        if (q <= T) coef[ss * COEF + T + q] = cst;                 // C[s][q]
-        else if (q == T + 1) coef[ss * COEF + 2 * T + 1] = inv * inv * zsum;  // kk[s]: RMS-norm backward coefficient
+        if (sv && q <= T) coef[ss * COEF + T + q] = cst;                 // C[s][q]
+        else if (sv && q == T + 1) coef[ss * COEF + 2 * T + 1] = inv * inv * zsum;  // kk[s]: RMS-norm backward coefficient
       }
       named_bar_sync(bar_id, 128);
       // ---------------- pass 2 ----------------
-      float al[S][T], C[S][6], kk[S];
+      float al[S][T], C[S][NG], kk[S];
 #pragma unroll
       for (int s = 0; s < S; ++s) {
-        float cf[12];
+        float cf[12];  // T + NG + 1 <= 12
 #pragma unroll
         for (int i = 0; i < 3; ++i) hc2::lds4(coef + s * COEF + 4 * i, cf + 4 * i);
 #pragma unroll
         for (int t = 0; t < T; ++t) al[s][t] = cf[t];
 #pragma unroll
-        for (int c6 = 0; c6 < 6; ++c6) C[s][c6] = cf[T + c6];
+        for (int c6 = 0; c6 < NG; ++c6) C[s][c6] = cf[T + c6];
         kk[s] = cf[2 * T + 1];
       }
-      float dbp[S] = {0.f, 0.f, 0.f, 0.f};
+      float dbp[S];
+#pragma unroll
+      for (int s = 0; s < S; ++s) dbp[s] = 0.f;
       if (act) {
         float r[S][8], y[8], dr[S][8], dy[8];
         load_r(r, y);
         uint4 dmp[S], dxp, exp_ = make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll
-        for (int t = 0; t < S; ++t) dmp[t] = *reinterpret_cast<const uint4*>(st + off_dr(d) + 2 * (t * d + c8));
-        dxp = *reinterpret_cast<const uint4*>(st + off_dxn(d) + 2 * c8);
-        if (has_dbin) exp_ = *reinterpret_cast<const uint4*>(st + off_dbin(d) + 2 * c8);
+        for (int t = 0; t < S; ++t) dmp[t] = *reinterpret_cast<const uint4*>(st + off_dr<S>(d) + 2 * (t * d + c8));
+        dxp = *reinterpret_cast<const uint4*>(st + off_dxn<S>(d) + 2 * c8);
+        if (has_dbin) exp_ = *reinterpret_cast<const uint4*>(st + off_dbin<S>(d) + 2 * c8);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          float pg[6][4], lg[4];
+          float pg[NG][4], lg[4];
           hc2::lds4(pLn + h * half, lg);
 #pragma unroll
-          for (int c6 = 0; c6 < 6; ++c6) hc2::lds4(pLn + (1 + c6) * d + h * half, pg[c6]);
+          for (int c6 = 0; c6 < NG; ++c6) hc2::lds4(pLn + (1 + c6) * d + h * half, pg[c6]);
 #pragma unroll
           for (int e4 = 0; e4 < 4; ++e4) {
             const int e = 4 * h + e4;
@@ -361,12 +382,12 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
 #pragma unroll
               for (int t = 0; t < T; ++t) acc = fmaf(al[s][t], dm[t], acc);
 #pragma unroll
-              for (int c6 = 0; c6 < 6; ++c6) acc = fmaf(C[s][c6], pg[c6][e4], acc);
+              for (int c6 = 0; c6 < NG; ++c6) acc = fmaf(C[s][c6], pg[c6][e4], acc);
               dr[s][e] = acc;
               dbp[s] = fmaf(acc, y[e], dbp[s]);
               dy[e] = fmaf(bp[s], acc, dy[e]);
 #pragma unroll
-              for (int c6 = 0; c6 < 6; ++c6) G[c6][e] = fmaf(r[s][e], C[s][c6], G[c6][e]);
+              for (int c6 = 0; c6 < NG; ++c6) G[c6][e] = fmaf(r[s][e], C[s][c6], G[c6][e]);
             }
           }
         }
@@ -374,7 +395,17 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
         if (EXPAND) {
           float o[8];
 #pragma unroll
-          for (int e = 0; e < 8; ++e) o[e] = ((dr[0][e] + dr[1][e]) + (dr[2][e] + dr[3][e])) * dx_scale;
+          for (int e = 0; e < 8; ++e) {
+            float sum;
+            if constexpr (S == 4) {
+              sum = (dr[0][e] + dr[1][e]) + (dr[2][e] + dr[3][e]);
+            } else {
+              sum = dr[0][e];
+#pragma unroll
+              for (int s = 1; s < S; ++s) sum += dr[s][e];
+            }
+            o[e] = sum * dx_scale;
+          }
           float* dst = dx_expand + md + c8;
           *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1], o[2], o[3]);
           *reinterpret_cast<float4*>(dst + 4) = make_float4(o[4], o[5], o[6], o[7]);
@@ -403,25 +434,25 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
     if (w == 0) {
       if (pend >= 0 && lane < S)
         dbeta_prev[(size_t)pend * S + lane] = (dbpm[lane] + dbpm[S + lane]) + (dbpm[2 * S + lane] + dbpm[3 * S + lane]);
-      if (q < T) atomicAdd(gr.static_alpha + ss * T + q, small0);
-      else if (q == T) atomicAdd(gr.static_beta + ss, small0);
-      const float as = warp_sum(q < T ? small1 : 0.f), bs = warp_sum(q == T ? small1 : 0.f);
+      if (sv && q < T) atomicAdd(gr.static_alpha + ss * T + q, small0);
+      else if (sv && q == T) atomicAdd(gr.static_beta + ss, small0);
+      const float as = warp_sum(sv && q < T ? small1 : 0.f), bs = warp_sum(sv && q == T ? small1 : 0.f);
       if (lane == 0) {
         atomicAdd(gr.alpha_scale, as);
         atomicAdd(gr.beta_scale, bs);
       }
     }
-    // per-channel partials of each warpgroup -> the ring, idle once every stage has been consumed: [NC][7][d]
+    // per-channel partials of each warpgroup -> the ring, idle once every stage has been consumed: [NC][NP][d]
     __syncthreads();
     if (act) {
-      float* buf = reinterpret_cast<float*>(ring) + (size_t)cw * 7 * d + lt * 8;
+      float* buf = reinterpret_cast<float*>(ring) + (size_t)cw * NP * d + lt * 8;
 #pragma unroll
-      for (int c6 = 0; c6 < 6; ++c6) {
+      for (int c6 = 0; c6 < NG; ++c6) {
         *reinterpret_cast<float4*>(buf + c6 * d) = make_float4(G[c6][0], G[c6][1], G[c6][2], G[c6][3]);
         *reinterpret_cast<float4*>(buf + c6 * d + 4) = make_float4(G[c6][4], G[c6][5], G[c6][6], G[c6][7]);
       }
-      *reinterpret_cast<float4*>(buf + 6 * d) = make_float4(gLn[0], gLn[1], gLn[2], gLn[3]);
-      *reinterpret_cast<float4*>(buf + 6 * d + 4) = make_float4(gLn[4], gLn[5], gLn[6], gLn[7]);
+      *reinterpret_cast<float4*>(buf + NG * d) = make_float4(gLn[0], gLn[1], gLn[2], gLn[3]);
+      *reinterpret_cast<float4*>(buf + NG * d + 4) = make_float4(gLn[4], gLn[5], gLn[6], gLn[7]);
     }
   }
   __syncthreads();
@@ -429,12 +460,12 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
   //   d dyn_alpha[:, t] += g1 G_t,  d dyn_beta += g1 G_5,  d gamma += sqrt(d) sum_c P_c G_c,  g1 = (gamma + 1) sqrt(d)
   const float* buf = reinterpret_cast<const float*>(ring);
   for (int i = threadIdx.x; i < d; i += blockDim.x) {
-    float g[7];
+    float g[NP];
 #pragma unroll
-    for (int k = 0; k < 7; ++k) {
+    for (int k = 0; k < NP; ++k) {
       g[k] = 0.f;
 #pragma unroll
-      for (int c = 0; c < NC; ++c) g[k] += buf[(size_t)(c * 7 + k) * d + i];
+      for (int c = 0; c < NC; ++c) g[k] += buf[(size_t)(c * NP + k) * d + i];
     }
     const float g1 = (prm.gamma_hc[i] + 1.f) * sqrt_d;
     float acc = g[T] * prm.dyn_beta[i];
@@ -445,7 +476,7 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
       atomicAdd(gr.dyn_alpha + (size_t)i * T + t, g1 * g[t]);
     }
     atomicAdd(gr.gamma_hc + i, sqrt_d * acc);
-    atomicAdd(gr.ln_gamma + i, g[6]);
+    atomicAdd(gr.ln_gamma + i, g[NG]);
   }
 }
 

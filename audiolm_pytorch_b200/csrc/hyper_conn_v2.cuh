@@ -1,8 +1,9 @@
-// Hyper-Connections forward, second generation (d <= 1024): 2 warps per token, 4 tokens per CTA, no CTA-wide
-// barrier.  (The first generation in hyper_conn.cu uses one CTA per token with 5-6 __syncthreads per token and runs
-// far off the HBM roofline.)  The backward is hyper_conn_ring.cuh.
+// Hyper-Connections forward, second generation (d <= 1024): 2 warps per token and 4 tokens per CTA for S <= 4, 4
+// warps per token and 2 tokens per CTA for S = 5..8; no CTA-wide barrier.  (The first generation in hyper_conn.cuh
+// uses one CTA per token with 5-6 __syncthreads per token and runs far off the HBM roofline.)  The backward is
+// hyper_conn_ring.cuh (S <= 4) and hyper_conn_ring_wide.cuh (S >= 5).
 //
-//  - a token's 64 threads each own NCH chunks of 8 channels (16-B vector loads, fully coalesced);
+//  - a token's TPT threads each own NCH chunks of 8 channels (16-B vector loads, fully coalesced);
 //  - reductions: warp shuffle + one 64-thread named barrier (bar.sync id, 64) through a tiny smem mailbox;
 //  - per-channel parameters live in shared memory (fp32).
 #pragma once
@@ -11,11 +12,16 @@
 namespace alm {
 namespace hc2 {
 
-constexpr int S = 4, T = 5;
 constexpr int THREADS = 256;      // a CTA holds THREADS / TPT token slots; TPT = threads per token (64 or 128)
-constexpr int MAILW = 32;        // floats per warp row of the reduction mailbox (largest reduction: 28 values)
-// ta[20] tb[4] inv[4] z[24] (pre-tanh) pad[2] mean rstd: 224-B rows, so that the backward stages a row with one bulk copy
-constexpr int AUX = S * T + S + S + (S * T + S) + 4;
+// floats per warp row of the reduction mailbox: the largest reduction has S * (S + 3) values (32 at S = 4)
+__host__ __device__ constexpr int mailw(int S) { return S * (S + 3) <= 32 ? 32 : (S * (S + 3) + 3) / 4 * 4; }
+// Per-token aux row for S streams (T = S + 1 map columns):
+//   ta[S*T] tb[S] inv[S] z[S*T + S] (pre-tanh) pad mean rstd
+// rounded up to 4 floats so that the backward stages a row with one bulk copy (S = 4: 56 floats, 224-B rows)
+__host__ __device__ constexpr int aux_floats(int S) { return (2 * S * (S + 1) + 3 * S + 4 + 3) / 4 * 4; }
+__host__ __device__ constexpr int z_offset(int S) { return S * (S + 1) + 2 * S; }
+__host__ __device__ constexpr int z_end(int S) { return 2 * S * (S + 1) + 3 * S; }
+static_assert(aux_floats(4) == 56, "the 4-stream aux row is 56 floats");
 
 template <int TPT>
 __device__ __forceinline__ void bar_slot(int id) {
@@ -23,7 +29,7 @@ __device__ __forceinline__ void bar_slot(int id) {
 }
 
 // sum N values over the TPT threads of a token slot; all of them get the result.
-template <int N, int TPT>
+template <int N, int TPT, int MAILW>
 __device__ __forceinline__ void slot_sum(float (&v)[N], float* mail /*[2][TPT/32][MAILW]*/, int& which, int w2, int lane,
                                          int bar_id) {
   constexpr int WPT = TPT / 32;
@@ -80,7 +86,8 @@ struct Grads {
   float* alpha_scale; float* beta_scale; float* ln_gamma;
 };
 
-// smem: [0,d) g1 = (gamma+1)*sqrt(d); [d,2d) dyn_beta; [2d,3d) ln_gamma; [3d, 8d) dyn_alpha transposed [T][d]
+// smem: [0,d) g1 = (gamma+1)*sqrt(d); [d,2d) dyn_beta; [2d,3d) ln_gamma; [3d, (3+T)d) dyn_alpha transposed [T][d]
+template <int T>
 __device__ __forceinline__ void stage_params(float* sm, const Params& p, int d) {
   const float sqrt_d = sqrtf((float)d);
   for (int i = threadIdx.x; i < d; i += blockDim.x) {
@@ -93,16 +100,17 @@ __device__ __forceinline__ void stage_params(float* sm, const Params& p, int d) 
 }
 
 // ------------------------------------------------------------------------------------------------
-template <int NCH, int TPT>
-__global__ void __launch_bounds__(THREADS, 2)
+template <int S, int NCH, int TPT>
+__global__ void __launch_bounds__(THREADS, S <= 4 ? 2 : 1)
 pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __restrict__ Y,
                const float* __restrict__ beta_prev, const float* __restrict__ x_expand, Params prm,
                __nv_bfloat16* __restrict__ R_out, __nv_bfloat16* __restrict__ bin, __nv_bfloat16* __restrict__ xn,
                float* __restrict__ beta_out, float* __restrict__ aux, int M, int d) {
   extern __shared__ float sm[];
+  constexpr int T = S + 1, AUX = aux_floats(S), MAILW = mailw(S);
   constexpr int TOK = THREADS / TPT, WPT = TPT / 32;
-  float* mailbox = sm + 8 * d;  // [TOK][2][WPT][MAILW]
-  stage_params(sm, prm, d);
+  float* mailbox = sm + (3 + T) * d;  // [TOK][2][WPT][MAILW]
+  stage_params<T>(sm, prm, d);
   __syncthreads();
   const float* sG1 = sm;
   const float* sBf = sm + d;
@@ -204,7 +212,7 @@ pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
         }
       }
     }
-    slot_sum<S * T + S + S, TPT>(w, mail, which, w2, lane, bar_id);
+    slot_sum<S * T + S + S, TPT, MAILW>(w, mail, which, w2, lane, bar_id);
     float inv[S];
 #pragma unroll
     for (int s = 0; s < S; ++s) {
@@ -214,7 +222,7 @@ pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
       w[S * T + s] *= inv[s];
     }
     if (lt == 0) {  // pre-activations: the backward's RMS-norm term needs them (hyper_conn_v3.cuh)
-      float* az = aux + (size_t)m * AUX + S * T + S + S;
+      float* az = aux + (size_t)m * AUX + z_offset(S);
 #pragma unroll
       for (int i = 0; i < S * T + S; ++i) az[i] = w[i];
     }
@@ -259,7 +267,7 @@ pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
         if (bin != nullptr) *reinterpret_cast<uint4*>(bin + (size_t)m * d + ch[k]) = pack8(bi[k]);
       }
     }
-    slot_sum<2, TPT>(st, mail, which, w2, lane, bar_id);
+    slot_sum<2, TPT, MAILW>(st, mail, which, w2, lane, bar_id);
     const float mean = st[0] / d;
     const float rstd = rsqrtf(fmaxf(st[1] / d - mean * mean, 0.f) + 1e-5f);
 #pragma unroll
@@ -281,15 +289,17 @@ pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
         a[S * T + S + s] = inv[s];
         beta_out[(size_t)m * S + s] = beta[s];
       }
-      a[AUX - 4] = 0.f;  // pad: the row is copied whole, so it is written (run-to-run identical aux)
-      a[AUX - 3] = 0.f;
+#pragma unroll
+      for (int i = z_end(S); i < AUX - 2; ++i) a[i] = 0.f;  // pad: the row is copied whole, so it is written
       a[AUX - 2] = mean;
       a[AUX - 1] = rstd;
     }
   }
 }
 
-inline size_t fwd_smem(int d, int tpt) { return (size_t)(8 * d + (THREADS / tpt) * 2 * (tpt / 32) * MAILW) * sizeof(float); }
+inline size_t fwd_smem(int S, int d, int tpt) {
+  return (size_t)((4 + S) * d + (THREADS / tpt) * 2 * (tpt / 32) * mailw(S)) * sizeof(float);
+}
 
 }  // namespace hc2
 }  // namespace alm

@@ -160,14 +160,16 @@ class StackDecoder:
         if self.bias is not None:   # the new token's bias row, read by every layer
             table, over, u, cls, c, brow = self.bias
             ops.decode_bias_row(table, over, u, cls, c, self.len, brow)
-        # the residual stream as in Transformer._walk_forward: fp32 r (plain, resid_ln) or bf16 R [b, 4, d]
+        # the residual stream as in Transformer._walk_forward: fp32 r (plain, resid_ln) or bf16 R [b, S, d]
         # (hyper-connections); `bin_` (the un-normalised branch input) feeds to_kv
-        plain = tr.num_residual_streams == 1
+        S = tr.num_residual_streams
+        plain = S == 1
         hc0 = tr.layers[0][0]
         if plain:
             r, xn, bin_, _ = ops.resid_ln_fwd(x2, None, hc0.branch.norm.gamma, want_raw=True)
         else:
-            R, bin_, xn, beta, _ = ops.hc_pre_fwd(hc0.kernel_params(), hc0.branch.norm.gamma, x_expand=x2, M=b, d=d)
+            R, bin_, xn, beta, _ = ops.hc_pre_fwd(hc0.kernel_params(), hc0.branch.norm.gamma, x_expand=x2, M=b, d=d,
+                                                 streams=S)
         v_first = None
         for i, (attn_hc, _, ff_hc) in enumerate(tr.layers):
             W = tr._weights(i)
@@ -186,7 +188,7 @@ class StackDecoder:
                 r, xn2, _, _ = ops.resid_ln_fwd(r, Y, getattr(f, "0").gamma)
             else:
                 R2, _, xn2, beta2, _ = ops.hc_pre_fwd(ff_hc.kernel_params(), getattr(f, "0").gamma, R_in=R, Y=Y,
-                                                      beta_prev=beta, M=b, d=d)
+                                                      beta_prev=beta, M=b, d=d, streams=S)
             h = mm(xn2, W["w1"])
             gn, _ = ops.geglu_ln_fwd(h, getattr(f, "3").gamma, inner=inner, inner_pad=ip)
             Y2 = mm(gn, W["w2"])
@@ -196,11 +198,11 @@ class StackDecoder:
                     r, xn, bin_, _ = ops.resid_ln_fwd(r, Y2, nxt.branch.norm.gamma, want_raw=True)
                 else:
                     R, bin_, xn, beta, _ = ops.hc_pre_fwd(nxt.kernel_params(), nxt.branch.norm.gamma, R_in=R2, Y=Y2,
-                                                          beta_prev=beta2, M=b, d=d)
+                                                          beta_prev=beta2, M=b, d=d, streams=S)
         if plain:
             out = ops.resid_ln_fwd(r, Y2, tr.norm.gamma)[1]
         else:
-            out, _ = ops.hc_post_fwd(R2, Y2, beta2, tr.norm.gamma, M=b, d=d)
+            out, _ = ops.hc_post_fwd(R2, Y2, beta2, tr.norm.gamma, M=b, d=d, streams=S)
         self.len.add_(1)
         return out
 

@@ -463,7 +463,16 @@ def bias_gather_bwd(dbias, idx, table_rows, *, want_override):
     return dtable, dover
 
 
-HC_AUX = 56  # floats of per-token state kept for the backward (see csrc/hyper_conn_v2.cuh)
+HC_MIN_STREAMS, HC_MAX_STREAMS = 2, 8  # stream counts the hyper-connection kernels are built for
+
+
+def hc_aux_floats(streams):
+    """floats of per-token state kept for the backward (csrc/hyper_conn_v2.cuh: aux_floats): ta[S(S+1)] tb[S] inv[S]
+    z[S(S+1)+S] pad mean rstd, rounded up to a multiple of 4 so that one bulk copy stages a row"""
+    return (2 * streams * (streams + 1) + 3 * streams + 4 + 3) // 4 * 4
+
+
+HC_AUX = hc_aux_floats(4)
 
 
 def _hc_param_ptrs(hc, ln_gamma):
@@ -475,15 +484,17 @@ def hc_pre_fwd(hc, ln_gamma, *, R_in=None, Y=None, beta_prev=None, x_expand=None
     """depth(prev branch) + width(this branch) + pre-LayerNorm.  hc: dict of fp32 HC params.
 
     Returns R_out [M,S,d] bf16, bin [M,d] bf16 (None unless want_bin), xn [M,d] bf16, beta [M,S] f32,
-    aux [M,HC_AUX] f32.
+    aux [M, hc_aux_floats(S)] f32.
     """
     dev = ln_gamma.device
     R_out = torch.empty(M, streams, d, device=dev, dtype=bf16)
     bin_ = torch.empty(M, d, device=dev, dtype=bf16) if want_bin else None
     xn = torch.empty(M, d, device=dev, dtype=bf16)
     beta = torch.empty(M, streams, device=dev, dtype=f32)
-    aux = torch.empty(M, HC_AUX, device=dev, dtype=f32)
-    with _timed("hc_pre_fwd", M * d * ((4 if x_expand is not None else 10) + 10 + (2 if want_bin else 0)), "byte"):
+    aux = torch.empty(M, hc_aux_floats(streams), device=dev, dtype=f32)
+    rs = 2 * streams  # bytes per channel of the bf16 [S, d] residual
+    with _timed("hc_pre_fwd", M * d * ((4 if x_expand is not None else rs + 2) + rs + 2 + (2 if want_bin else 0)),
+                "byte"):
         _lib.call("alm_hc_pre_fwd", R_in, Y, beta_prev, x_expand, *_hc_param_ptrs(hc, ln_gamma),
                   R_out, bin_, xn, beta, aux, M, d, streams)
     return R_out, bin_, xn, beta, aux
@@ -505,7 +516,9 @@ def hc_pre_bwd(hc, ln_gamma, grads, g_ln_gamma, aux, dR_out, dxn, dbeta, *, dbin
         dR_in = torch.empty(M, streams, d, device=dev, dtype=bf16)
         dY = torch.empty(M, d, device=dev, dtype=bf16)
         dbp = torch.empty(M, streams, device=dev, dtype=f32)
-    nbytes = M * d * ((4 + 8 + 2 + 4 if x_expand is not None else 8 + 2 + 8 + 2 + 8 + 2) + (2 if dbin_extra is not None else 0))
+    rs = 2 * streams
+    nbytes = M * d * ((4 + rs + 2 + 4 if x_expand is not None else rs + 2 + rs + 2 + rs + 2)
+                      + (2 if dbin_extra is not None else 0))
     with _timed("hc_pre_bwd", nbytes, "byte"):
         _lib.call("alm_hc_pre_bwd", R_in, Y, beta_prev, x_expand, *_hc_param_ptrs(hc, ln_gamma), aux, dR_out, dxn,
                   dbin_extra, dbeta, dR_in, dY, dbp, dx, float(dx_scale),

@@ -262,15 +262,17 @@ class _StackFn(torch.autograd.Function):
 # parameters of the branch's wrapper and their gradient buffers (empty dicts for the plain residual).
 # ----------------------------------------------------------------------------------------------
 class _HyperStreams:
-    """num_residual_streams == 4: a bf16 [M, 4, d] stream; depth (of the previous branch), width and LayerNorm are one
-    hc_pre kernel, which writes `bin` only when the branch asks for it.  Saves per step its inputs (R, Y, beta) and the kernel's aux state; the
+    """num_residual_streams = S in 2..8: a bf16 [M, S, d] stream; depth (of the previous branch), width and LayerNorm
+    are one hc_pre kernel, which writes `bin` only when the branch asks for it.  Saves per step its inputs (R, Y, beta) and the kernel's aux state; the
     exit saves its LN stats."""
 
-    def __init__(self, save):
+    def __init__(self, save, streams):
         self.saved = [] if save else None
+        self.S = streams
 
     def _pre(self, inputs, hc, gamma, want_bin=True):
-        self.R, bin_, xn, self.beta, aux = ops.hc_pre_fwd(hc, gamma, **inputs, M=self.M, d=self.d, want_bin=want_bin)
+        self.R, bin_, xn, self.beta, aux = ops.hc_pre_fwd(hc, gamma, **inputs, M=self.M, d=self.d, streams=self.S,
+                                                          want_bin=want_bin)
         if self.saved is not None:
             self.saved.append((inputs, aux))
         return xn, bin_
@@ -283,20 +285,21 @@ class _HyperStreams:
         return self._pre(dict(R_in=self.R, Y=Y, beta_prev=self.beta), hc, gamma, want_bin)
 
     def exit(self, Y, gamma):
-        out, stats = ops.hc_post_fwd(self.R, Y, self.beta, gamma, M=self.M, d=self.d)
+        out, stats = ops.hc_post_fwd(self.R, Y, self.beta, gamma, M=self.M, d=self.d, streams=self.S)
         if self.saved is not None:
             self.saved.append(((self.R, Y, self.beta), stats))
         return out
 
     def exit_bwd(self, gamma, dout, g_gamma):
         (R, Y, beta), stats = self.saved.pop()
-        self.dR, dY, self.dbeta = ops.hc_post_bwd(R, Y, beta, gamma, stats, dout, g_gamma, M=self.M, d=self.d)
+        self.dR, dY, self.dbeta = ops.hc_post_bwd(R, Y, beta, gamma, stats, dout, g_gamma, M=self.M, d=self.d,
+                                                  streams=self.S)
         return dY
 
     def _pre_bwd(self, hc, gamma, g_hc, g_gamma, dxn, dbin, **kw):
         inputs, aux = self.saved.pop()
         return ops.hc_pre_bwd(hc, gamma, g_hc, g_gamma, aux, self.dR, dxn, self.dbeta, dbin_extra=dbin, **inputs, **kw,
-                              M=self.M, d=self.d)
+                              M=self.M, d=self.d, streams=self.S)
 
     def step_bwd(self, hc, gamma, g_hc, g_gamma, dxn, dbin=None):
         self.dR, dY, self.dbeta = self._pre_bwd(hc, gamma, g_hc, g_gamma, dxn, dbin)
@@ -378,8 +381,9 @@ class Transformer(nn.Module):
         rel_pos_bias = rel_pos_bias and not flash_attn
         if cross_attend or cond_as_self_attn_prefix:
             raise NotImplementedError("text / audio conditioning is outside the accelerated hot path")
-        if num_residual_streams not in (1, 4):
-            raise NotImplementedError("residual-stream kernels are built for num_residual_streams in (1, 4)")
+        if num_residual_streams != 1 and not ops.HC_MIN_STREAMS <= num_residual_streams <= ops.HC_MAX_STREAMS:
+            raise NotImplementedError(f"residual-stream kernels are built for num_residual_streams = 1 or "
+                                      f"{ops.HC_MIN_STREAMS}..{ops.HC_MAX_STREAMS}")
         _check_dropout(attn_dropout, "attn_dropout")
         _check_dropout(ff_dropout, "ff_dropout")
         if dim % 8 != 0:
@@ -552,7 +556,7 @@ class Transformer(nn.Module):
         S = dict(shape=(b, n, d), x_dtype=x.dtype, mask=ops.pack_key_mask(mask),  # bits, packed once for every layer
                  bias=bias, drop=drop)
         P = self._layer_params()
-        res = _PlainStream(save) if self.num_residual_streams == 1 else _HyperStreams(save)
+        res = _PlainStream(save) if self.num_residual_streams == 1 else _HyperStreams(save, self.num_residual_streams)
         xn, bin_ = res.enter(x2, P[0][0], P[0][1]["ln"])
         L, kvs, v_first = [], [], None
         for i, (_, _, hc_f, p_f) in enumerate(P):

@@ -214,15 +214,17 @@ int alm_decode_stack_step(const void* layer_table, int n_layers, const float* x,
 
 /* ---- Hyper-Connections residual streams fused with the pre-LayerNorm (HBM-bound) ---------------- */
 /*
- * Internal layout: residual streams R [M, S=4, d] bf16, M = batch*seq.  One call per branch does
+ * Internal layout: residual streams R [M, S, d] bf16, M = batch*seq.  One call per branch does
  *   R      = R_in + beta_prev (x) Y          depth connection of the previous branch
  *            (or R_s = x_expand for all s: expand_streams, audiolm_pytorch.py:524)
  *   bin, R_out = width connection of this branch (dynamic+static alpha/beta, RMSNorm over channels)
  *   xn     = LayerNorm(bin) * ln_gamma       the branch's pre-norm (audiolm_pytorch.py:347, 254)
- * aux [M, 56] keeps the tanh activations, 1/|R_s|, the pre-activations z and the LN mean/rstd for the backward.
+ * aux [M, A] keeps the tanh activations, 1/|R_s|, the pre-activations z and the LN mean/rstd for the backward;
+ * A = 2S(S+1) + 3S + 4 rounded up to a multiple of 4 (S = 4: 56).
  * bin may be NULL when no consumer needs the un-normalised branch input.
  * Replaces hyper_connections.HyperConnections.forward as used at audiolm_pytorch.py:446-454,
- * 528-547 (third-party; restated in oracle/third_party.py).  Only streams == 4 is built.
+ * 528-547 (third-party; restated in oracle/third_party.py).  streams = 2..8 are built; any other count, or a d whose
+ * first-generation kernel (d > 1024) needs more shared memory than the device allows, returns ALM_ERR_UNSUPPORTED.
  */
 int alm_hc_pre_fwd(const void* R_in, const void* Y, const float* beta_prev, const float* x_expand,
                    const float* gamma_hc, const float* dyn_alpha, const float* dyn_beta, const float* static_alpha,

@@ -25,7 +25,7 @@ from audiolm_pytorch_b200.soundstream import SoundStream  # noqa: E402
 ap = argparse.ArgumentParser()
 ap.add_argument("steps", nargs="?", type=int, default=64, help="tokens per generate() window")
 ap.add_argument("--no-flash", action="store_true", help="flash_attn=False (the reference's constructor default)")
-ap.add_argument("--streams", type=int, default=4, choices=(1, 4), help="num_residual_streams")
+ap.add_argument("--streams", type=int, default=4, choices=range(1, 9), help="num_residual_streams")
 ap.add_argument("--skip-codec", action="store_true", help="do not time the codec decode")
 args = ap.parse_args()
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Stand-alone timings of the HBM-bound row kernels, attention and every wgmma GEMM shape at C3 sizes (CUDA events,
 L2 flushed between iterations).
-usage: python tools/bench_kernels.py [geglu] [hc] [attn] [gemm] [dropout] ..."""
+usage: python tools/bench_kernels.py [geglu] [hc [--streams S]] [attn] [gemm] [dropout] ..."""
 import sys
 from pathlib import Path
 
@@ -14,7 +14,13 @@ dev = "cuda"
 bf16, f32 = torch.bfloat16, torch.float32
 torch.manual_seed(0)
 M, d, H = 16 * 2048, 1024, 8
-which = set(sys.argv[1:]) or {"geglu", "hc", "attn"}
+args = sys.argv[1:]
+S = 4  # hyper-connection residual streams (hc)
+if "--streams" in args:
+    i = args.index("--streams")
+    S = int(args[i + 1])
+    del args[i:i + 2]
+which = set(args) or {"geglu", "hc", "attn"}
 flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)
 
 
@@ -54,29 +60,33 @@ if "geglu" in which:
     timeit("geglu_ln_bwd", lambda: ops.geglu_ln_bwd(h, g, st, dgn, gg, inner=2730, inner_pad=ip), nbytes=M * ip * 10)
 
 if "hc" in which:
-    hc = dict(gamma=rnd(d, dt=f32, k=0.1), dyn_alpha=rnd(d, 5, dt=f32, k=0.05), dyn_beta=rnd(d, dt=f32, k=0.05),
-              static_alpha=rnd(4, 5, dt=f32), static_beta=rnd(4, dt=f32), alpha_scale=torch.tensor(0.3, device=dev),
+    T, rs = S + 1, 2 * S  # map columns; bytes per channel of the bf16 [S, d] residual
+    hc = dict(gamma=rnd(d, dt=f32, k=0.1), dyn_alpha=rnd(d, T, dt=f32, k=0.05), dyn_beta=rnd(d, dt=f32, k=0.05),
+              static_alpha=rnd(S, T, dt=f32), static_beta=rnd(S, dt=f32), alpha_scale=torch.tensor(0.3, device=dev),
               beta_scale=torch.tensor(0.3, device=dev))
     lng = rnd(d, dt=f32)
-    R, Y, bp = rnd(M, 4, d), rnd(M, d), rnd(M, 4, dt=f32)
-    timeit("hc_pre_fwd", lambda: ops.hc_pre_fwd(hc, lng, R_in=R, Y=Y, beta_prev=bp, M=M, d=d), nbytes=M * d * 22)
-    timeit("hc_pre_fwd (no bin)", lambda: ops.hc_pre_fwd(hc, lng, R_in=R, Y=Y, beta_prev=bp, M=M, d=d, want_bin=False),
-           nbytes=M * d * 20)
-    R_out, bin_, xn, beta, aux = ops.hc_pre_fwd(hc, lng, R_in=R, Y=Y, beta_prev=bp, M=M, d=d)
+    R, Y, bp = rnd(M, S, d), rnd(M, d), rnd(M, S, dt=f32)
+    print(f"hyper-connections: S={S} streams, M={M}, d={d}")
+    timeit("hc_pre_fwd", lambda: ops.hc_pre_fwd(hc, lng, R_in=R, Y=Y, beta_prev=bp, M=M, d=d, streams=S),
+           nbytes=M * d * (2 * rs + 6))
+    timeit("hc_pre_fwd (no bin)", lambda: ops.hc_pre_fwd(hc, lng, R_in=R, Y=Y, beta_prev=bp, M=M, d=d, streams=S,
+                                                         want_bin=False), nbytes=M * d * (2 * rs + 4))
+    R_out, bin_, xn, beta, aux = ops.hc_pre_fwd(hc, lng, R_in=R, Y=Y, beta_prev=bp, M=M, d=d, streams=S)
     x = rnd(M, d, dt=f32)
-    aux_x = ops.hc_pre_fwd(hc, lng, x_expand=x, M=M, d=d)[4]
-    dR, dxn, dbe, dbin = rnd(M, 4, d), rnd(M, d), rnd(M, 4, dt=f32), rnd(M, d)
+    aux_x = ops.hc_pre_fwd(hc, lng, x_expand=x, M=M, d=d, streams=S)[4]
+    dR, dxn, dbe, dbin = rnd(M, S, d), rnd(M, d), rnd(M, S, dt=f32), rnd(M, d)
     grads = {k_: torch.zeros_like(v_) for k_, v_ in hc.items()}
     gl = torch.zeros_like(lng)
 
     def hcb(extra):
         return ops.hc_pre_bwd(hc, lng, grads, gl, aux, dR, dxn, dbe, dbin_extra=extra, R_in=R, Y=Y, beta_prev=bp, M=M,
-                              d=d)
+                              d=d, streams=S)
 
-    timeit("hc_pre_bwd (dbin_extra)", lambda: hcb(dbin), nbytes=M * d * 32)
-    timeit("hc_pre_bwd (no dbin_extra)", lambda: hcb(None), nbytes=M * d * 30)
+    timeit("hc_pre_bwd (dbin_extra)", lambda: hcb(dbin), nbytes=M * d * (3 * rs + 8))
+    timeit("hc_pre_bwd (no dbin_extra)", lambda: hcb(None), nbytes=M * d * (3 * rs + 6))
     timeit("hc_pre_bwd (expand)", lambda: ops.hc_pre_bwd(hc, lng, grads, gl, aux_x, dR, dxn, dbe, dbin_extra=dbin,
-                                                         x_expand=x, dx_scale=0.5, M=M, d=d), nbytes=M * d * 20)
+                                                         x_expand=x, dx_scale=0.5, M=M, d=d, streams=S),
+           nbytes=M * d * (rs + 12))
 
 if "attn" in which:
     q, k, v = rnd(16, 2048, 512), rnd(16, 2048, 64), rnd(16, 2048, 64)
