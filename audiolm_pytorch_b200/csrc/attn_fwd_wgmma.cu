@@ -36,6 +36,7 @@ struct AttnFwdParams {
   int causal;
   float scale_log2;       // d^-1/2 * log2(e)
   int n_q_pad;            // n_q rounded up to 128: query rows of the dropout counter are (b*h + head) * n_q_pad + i
+  uint32_t drop_row0;     // dropout counter row of this launch's batch 0 (the host launches batch chunks, see below)
   DropoutArgs drop;
 };
 
@@ -157,7 +158,8 @@ mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   }
   const uint32_t* mrow = p.kmask ? p.kmask + (long long)batch * p.kb_stride : nullptr;
   const uint32_t q_addr = smem_u32(sQ) + cw * 8192;
-  [[maybe_unused]] const uint32_t drop_row = ((uint32_t)batch * p.h + head) * (uint32_t)p.n_q_pad + q0 + r_base;
+  [[maybe_unused]] const uint32_t drop_row =
+      p.drop_row0 + ((uint32_t)batch * p.h + head) * (uint32_t)p.n_q_pad + q0 + r_base;
 
   if (n_tiles > 0) mbar_wait(q_full, 0);
   int stage = 0;
@@ -277,15 +279,17 @@ mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
 }  // namespace alm
 
 namespace alm {
-// key mask bytes [b, n_k] (non-zero = attend) -> bits [b, 4 * ceil(n_k / 128)] (keys past n_k: 0)
-__global__ void pack_key_mask_kernel(const uint8_t* __restrict__ mask, uint32_t* __restrict__ bits, int n_k, int words) {
-  const int b = blockIdx.y;
-  const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (w >= words) return;
-  const int k = w * 32 + (threadIdx.x & 31);
-  const bool on = k < n_k && mask[(long long)b * n_k + k] != 0;
+// key mask bytes [b, n_k] (non-zero = attend) -> bits [b, 4 * ceil(n_k / 128)] (keys past n_k: 0); one warp per word
+// of the flattened [b * words] output on a 1-D grid, so the batch is not bound by the 65535 limit of grid.y
+__global__ void pack_key_mask_kernel(const uint8_t* __restrict__ mask, uint32_t* __restrict__ bits, int n_k, int words,
+                                     long long total) {
+  const long long i = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (i >= total) return;
+  const long long b = i / words;
+  const int k = (int)(i - b * words) * 32 + (threadIdx.x & 31);
+  const bool on = k < n_k && mask[b * n_k + k] != 0;
   const uint32_t v = __ballot_sync(0xffffffffu, on);
-  if ((threadIdx.x & 31) == 0) bits[(long long)b * words + w] = v;
+  if ((threadIdx.x & 31) == 0) bits[i] = v;
 }
 }  // namespace alm
 
@@ -294,9 +298,11 @@ extern "C" int alm_pack_key_mask(const void* key_mask, void* bits, int b, int n_
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ALM_REQUIRE(key_mask && bits && b > 0 && n_k > 0, ALM_ERR_ARG);
   const int words = (n_k + 127) / 128 * 4;
-  dim3 grid(ceil_div(words, 8), b);
-  pack_key_mask_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const uint8_t*>(key_mask),
-                                                 reinterpret_cast<uint32_t*>(bits), n_k, words);
+  const long long total = (long long)b * words;
+  const long long blocks = ceil_div(total, 8LL);
+  ALM_REQUIRE(blocks <= INT_MAX, ALM_ERR_UNSUPPORTED);
+  pack_key_mask_kernel<<<(unsigned)blocks, 256, 0, stream>>>(reinterpret_cast<const uint8_t*>(key_mask),
+                                                            reinterpret_cast<uint32_t*>(bits), n_k, words, total);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);
   return ALM_OK;
@@ -321,36 +327,14 @@ extern "C" int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64
     ALM_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15u) == 0, ALM_ERR_ALIGN);
   }
 
-  CUtensorMap tmQ, tmK, tmV;
-  {
-    uint64_t dims[3] = {(uint64_t)h * ATT_D, (uint64_t)n_q, (uint64_t)b};
-    uint64_t strides[3] = {2, (uint64_t)ldq * 2, (uint64_t)n_q * ldq * 2};
-    uint32_t box[3] = {ATT_D, ATT_BM, 1};
-    int rc = make_tensor_map(&tmQ, q, 2, 3, dims, strides, box, true);
-    if (rc != ALM_OK) return rc;
-  }
-  {
-    uint64_t dims[3] = {(uint64_t)ATT_D, (uint64_t)n_k, (uint64_t)b};
-    uint64_t strides[3] = {2, (uint64_t)ldk * 2, (uint64_t)k_bstride * 2};
-    uint32_t box[3] = {ATT_D, ATT_BN, 1};
-    int rc = make_tensor_map(&tmK, k, 2, 3, dims, strides, box, true);
-    if (rc != ALM_OK) return rc;
-    strides[1] = (uint64_t)ldv * 2;
-    strides[2] = (uint64_t)v_bstride * 2;
-    rc = make_tensor_map(&tmV, v, 2, 3, dims, strides, box, true);
-    if (rc != ALM_OK) return rc;
-  }
   AttnFwdParams p;
-  p.o = reinterpret_cast<__nv_bfloat16*>(o);
-  p.lse = lse;
-  p.kmask = reinterpret_cast<const uint32_t*>(key_mask);
   p.kb_stride = (n_k + 127) / 128 * 4;
   p.bias = bias;
   p.bias_hs = bias_hstride;
   p.bias_rs = bias_rstride;
   p.ldo = ldo;
   p.lse_stride = lse_stride;
-  p.b = b; p.h = h; p.n_q = n_q; p.n_k = n_k;
+  p.h = h; p.n_q = n_q; p.n_k = n_k;
   p.causal = causal;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.n_q_pad = (n_q + 127) / 128 * 128;
@@ -367,17 +351,52 @@ extern "C" int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64
                                      ATT_SMEM_BYTES));
     attr_set = true;
   }
-  dim3 grid((n_q + ATT_BM - 1) / ATT_BM, h, b);
   const bool drop = dropout_p > 0.f;
-  if (bias != nullptr && drop)
-    mqa_attn_fwd_kernel<true, true><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
-  else if (bias != nullptr)
-    mqa_attn_fwd_kernel<true, false><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
-  else if (drop)
-    mqa_attn_fwd_kernel<false, true><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
-  else
-    mqa_attn_fwd_kernel<false, false><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
-  ALM_CHECK_LAUNCH();
-  ALM_LAUNCHED(1);
+  // Batch is grid.z, which stops at 65535, so larger batches (the local attention passes batch x heads x windows)
+  // run as consecutive launches over chunks of batch rows: operands, outputs and the key mask are offset here, the
+  // dropout counter rows by p.drop_row0.  The (qblock, head, batch) order of each launch is unchanged.
+  constexpr int kMaxGridZ = 65535;
+  const int n_launch = ceil_div(b, kMaxGridZ);
+  for (int b0 = 0; b0 < b; b0 += kMaxGridZ) {
+    const int nb = min(b - b0, kMaxGridZ);
+    CUtensorMap tmQ, tmK, tmV;
+    {
+      uint64_t dims[3] = {(uint64_t)h * ATT_D, (uint64_t)n_q, (uint64_t)nb};
+      uint64_t strides[3] = {2, (uint64_t)ldq * 2, (uint64_t)n_q * ldq * 2};
+      uint32_t box[3] = {ATT_D, ATT_BM, 1};
+      int rc = make_tensor_map(&tmQ, reinterpret_cast<const __nv_bfloat16*>(q) + (long long)b0 * n_q * ldq, 2, 3, dims,
+                               strides, box, true);
+      if (rc != ALM_OK) return rc;
+    }
+    {
+      uint64_t dims[3] = {(uint64_t)ATT_D, (uint64_t)n_k, (uint64_t)nb};
+      uint64_t strides[3] = {2, (uint64_t)ldk * 2, (uint64_t)k_bstride * 2};
+      uint32_t box[3] = {ATT_D, ATT_BN, 1};
+      int rc = make_tensor_map(&tmK, reinterpret_cast<const __nv_bfloat16*>(k) + (long long)b0 * k_bstride, 2, 3, dims,
+                               strides, box, true);
+      if (rc != ALM_OK) return rc;
+      strides[1] = (uint64_t)ldv * 2;
+      strides[2] = (uint64_t)v_bstride * 2;
+      rc = make_tensor_map(&tmV, reinterpret_cast<const __nv_bfloat16*>(v) + (long long)b0 * v_bstride, 2, 3, dims,
+                           strides, box, true);
+      if (rc != ALM_OK) return rc;
+    }
+    p.o = reinterpret_cast<__nv_bfloat16*>(o) + (long long)b0 * n_q * ldo;
+    p.lse = lse != nullptr ? lse + (long long)b0 * h * lse_stride : nullptr;
+    p.kmask = key_mask != nullptr ? reinterpret_cast<const uint32_t*>(key_mask) + (long long)b0 * p.kb_stride : nullptr;
+    p.b = nb;
+    p.drop_row0 = (uint32_t)((long long)b0 * h * p.n_q_pad);
+    const dim3 grid((n_q + ATT_BM - 1) / ATT_BM, h, nb);
+    if (bias != nullptr && drop)
+      mqa_attn_fwd_kernel<true, true><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
+    else if (bias != nullptr)
+      mqa_attn_fwd_kernel<true, false><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
+    else if (drop)
+      mqa_attn_fwd_kernel<false, true><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
+    else
+      mqa_attn_fwd_kernel<false, false><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
+    ALM_CHECK_LAUNCH();
+  }
+  ALM_LAUNCHED(n_launch);
   return ALM_OK;
 }

@@ -217,6 +217,8 @@ def mqa_attn_fwd(q, k, v, *, heads, key_mask=None, causal=True, scale=None, retu
     dropout: optional (p, seed, site): dropout on the attention probabilities (attend.py:139-140); the mask element
     of (batch, head, query i, key j) is keep(seed, site, (batch*heads + head) * n_q_pad + i, j), n_q_pad = n_q
     rounded up to 128.  The returned lse is that of the un-dropped probabilities.
+    Accepted sizes: 1 <= n_q <= n_k and b * heads * n_q_pad < 2**32 (the 32-bit dropout counter), for any batch b:
+    the local attention calls this with b = batch * heads * windows, which passes 65535 on long clips.
     Returns o [b, n_q, heads*64] bf16 and lse [b, heads, n_q] fp32.
     """
     _check_cuda(q, k, v, bias)

@@ -71,6 +71,7 @@ int alm_embed_scatter(float* const* grad_tables, int n_tables, const int32_t* sr
  * Key-padding / forgetful-causal mask in the form the attention kernels read: uint8 [b, n_k] (non-zero = attend) ->
  * uint32 bits [b, 4 * ceil(n_k / 128)], bit i of word w = key 32 w + i.  One call per forward (all layers and the
  * backward share the result); a 128-key tile then costs every CTA one 16-byte load instead of 128 byte tests per row.
+ * Any b runs (one warp per output word on a 1-D grid).
  */
 int alm_pack_key_mask(const void* key_mask, void* bits, int b, int n_k, alm_stream_t stream);
 /*
@@ -90,6 +91,9 @@ int alm_pack_key_mask(const void* key_mask, void* bits, int b, int n_k, alm_stre
  * dropout_p in [0, 1): dropout on the attention probabilities (attend.py:139-140), applied to P before P V with the
  * mask keep(seed, site, (b*h + head) * n_q_pad + i, j), n_q_pad = n_q rounded up to 128 (see alm_dropout_bf16).
  * The LSE is that of the un-dropped probabilities.  dropout_p == 0 runs the dropout-free kernels.
+ * Accepted sizes: 1 <= n_q <= n_k and b * h * n_q_pad < 2^32 (the 32-bit dropout counter rows; checked with or
+ * without dropout).  Any such b runs: batches past 65535 (the grid.z limit) are launched in chunks of 65535 rows
+ * (the local attention calls this with b = batch * heads * windows).
  */
 int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int64_t k_bstride, const void* v,
                      int64_t ldv, int64_t v_bstride, const void* key_mask, void* o, int64_t ldo, float* lse,
