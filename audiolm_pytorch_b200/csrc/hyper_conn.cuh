@@ -10,11 +10,15 @@
 // token contiguous; M = batch * seq.  One CTA walks tokens with a grid stride; thread t owns the 8
 // contiguous channels [8t, 8t+8) of every stream, so d/8 threads are active (d % 8 == 0, d <= 8192).
 //
-// This header holds the first-generation kernels (one CTA per token, every d > 1024) and the launchers, templated on
-// S.  For d <= 1024 the launchers run hyper_conn_v2.cuh (forward) and hyper_conn_ring.cuh (backward, S <= 4) or
-// hyper_conn_ring_wide.cuh (backward, S = 5..8).  hyper_conn.cu dispatches the C ABI on the runtime stream count; the instantiations
-// are spread over hyper_conn_s*.cu so that they compile in parallel.
+// This header holds the launchers, templated on S, and the first-generation kernels (one CTA per token): hc_pre_fwd /
+// hc_pre_bwd for d > 1024, hc_post_fwd / hc_post_bwd for every d.  For d <= 1024 the pre launchers run
+// hc2::pre_fwd_kernel (hyper_conn_v2.cuh) and the ring backward: hcr::pre_bwd_kernel (hyper_conn_ring.cuh, S <= 4) or
+// hcr::pre_bwd_wide_kernel (hyper_conn_ring_wide.cuh, S = 5..8), both on the ring of hyper_conn_ring.cuh.
+// hyper_conn.cu dispatches the C ABI on the runtime stream count; the instantiations are spread over hyper_conn_s*.cu
+// so that they compile in parallel.
 #pragma once
+#include <type_traits>
+
 #include "alm_common.cuh"
 #include "hyper_conn_v2.cuh"
 #include "hyper_conn_ring.cuh"
@@ -24,22 +28,6 @@ namespace alm {
 
 constexpr int HC_MIN_S = 2, HC_MAX_S = 8;  // (S = 1 is the plain residual: resid_ln)
 constexpr int HC_MAX_WARPS = 32;
-
-struct HcParams {
-  const float* gamma_hc;  // [d]      RMSNorm gain (applied as gamma + 1)
-  const float* dyn_alpha; // [d, S+1]
-  const float* dyn_beta;  // [d]
-  const float* static_alpha;  // [S, S+1]
-  const float* static_beta;   // [S]
-  const float* alpha_scale;   // scalar
-  const float* beta_scale;    // scalar
-  const float* ln_gamma;  // [d] LayerNorm gain of the branch's pre-norm
-};
-
-struct HcGrads {  // fp32 accumulators (atomicAdd), same shapes as HcParams
-  float* gamma_hc; float* dyn_alpha; float* dyn_beta; float* static_alpha; float* static_beta;
-  float* alpha_scale; float* beta_scale; float* ln_gamma;
-};
 
 // sum N per-thread values over the whole CTA; every thread receives the totals.
 // `buf` is a [2][HALF][HC_MAX_WARPS] smem scratch, HALF >= every N the kernel reduces; alternating `which` removes the
@@ -66,22 +54,6 @@ __device__ __forceinline__ void block_sum(float (&v)[N], float* buf, int& which)
   which ^= 1;
 }
 
-__device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
-  f[0] = bf16_lo(u.x); f[1] = bf16_hi(u.x); f[2] = bf16_lo(u.y); f[3] = bf16_hi(u.y);
-  f[4] = bf16_lo(u.z); f[5] = bf16_hi(u.z); f[6] = bf16_lo(u.w); f[7] = bf16_hi(u.w);
-}
-__device__ __forceinline__ uint32_t pk2(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&v);
-}
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  return make_uint4(pk2(f[0], f[1]), pk2(f[2], f[3]), pk2(f[4], f[5]), pk2(f[6], f[7]));
-}
-__device__ __forceinline__ void load8f(const float* p, float (&f)[8]) {
-  const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
-  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-}
-
 // Saved per token for the backward: tanh of the dynamic alpha/beta pre-activations, 1/|R_s|, LN stats.
 //   aux [M, hc2::aux_floats(S)] = { ta[S*(S+1)], tb[S], inv_nrm[S], ..., mean, rstd }  (z slots unused here)
 
@@ -92,7 +64,7 @@ __device__ __forceinline__ void load8f(const float* p, float (&f)[8]) {
 template <int S, int MAXT>
 __global__ void __launch_bounds__(MAXT)
 hc_pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __restrict__ Y,
-                  const float* __restrict__ beta_prev, const float* __restrict__ x_expand, HcParams prm,
+                  const float* __restrict__ beta_prev, const float* __restrict__ x_expand, hc2::Params prm,
                   __nv_bfloat16* __restrict__ R_out, __nv_bfloat16* __restrict__ bin,
                   __nv_bfloat16* __restrict__ xn, float* __restrict__ beta_out, float* __restrict__ aux, int M,
                   int d) {
@@ -106,9 +78,12 @@ hc_pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* _
   const float sqrt_d = sqrtf((float)d);
   float g1[8], bfv[8], lng[8];
   if (act) {
-    load8f(prm.gamma_hc + c0, g1);
-    load8f(prm.dyn_beta + c0, bfv);
-    load8f(prm.ln_gamma + c0, lng);
+    hc2::lds4(prm.gamma_hc + c0, g1);
+    hc2::lds4(prm.gamma_hc + c0 + 4, g1 + 4);
+    hc2::lds4(prm.dyn_beta + c0, bfv);
+    hc2::lds4(prm.dyn_beta + c0 + 4, bfv + 4);
+    hc2::lds4(prm.ln_gamma + c0, lng);
+    hc2::lds4(prm.ln_gamma + c0 + 4, lng + 4);
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       g1[e] = (g1[e] + 1.f) * sqrt_d;
@@ -130,19 +105,20 @@ hc_pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* _
     if (act) {
       if (x_expand != nullptr) {
         float xv[8];
-        load8f(x_expand + (size_t)m * d + c0, xv);
+        hc2::lds4(x_expand + (size_t)m * d + c0, xv);
+        hc2::lds4(x_expand + (size_t)m * d + c0 + 4, xv + 4);
 #pragma unroll
         for (int s = 0; s < HC_S; ++s)
 #pragma unroll
           for (int e = 0; e < 8; ++e) R[s][e] = xv[e];
       } else {
         float yv[8];
-        unpack8(*reinterpret_cast<const uint4*>(Y + (size_t)m * d + c0), yv);
+        hc2::unpack8(*reinterpret_cast<const uint4*>(Y + (size_t)m * d + c0), yv);
 #pragma unroll
         for (int s = 0; s < HC_S; ++s) {
           const float bp = beta_prev[(size_t)m * HC_S + s];
           float rv[8];
-          unpack8(*reinterpret_cast<const uint4*>(R_in + ((size_t)m * HC_S + s) * d + c0), rv);
+          hc2::unpack8(*reinterpret_cast<const uint4*>(R_in + ((size_t)m * HC_S + s) * d + c0), rv);
 #pragma unroll
           for (int e = 0; e < 8; ++e) R[s][e] = rv[e] + bp * yv[e];
         }
@@ -220,12 +196,12 @@ hc_pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* _
     if (act) {
 #pragma unroll
       for (int s = 0; s < HC_S; ++s)
-        *reinterpret_cast<uint4*>(R_out + ((size_t)m * HC_S + s) * d + c0) = pack8(mix[s + 1]);
-      if (bin != nullptr) *reinterpret_cast<uint4*>(bin + (size_t)m * d + c0) = pack8(mix[0]);
+        *reinterpret_cast<uint4*>(R_out + ((size_t)m * HC_S + s) * d + c0) = hc2::pack8(mix[s + 1]);
+      if (bin != nullptr) *reinterpret_cast<uint4*>(bin + (size_t)m * d + c0) = hc2::pack8(mix[0]);
       float xo[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) xo[e] = (mix[0][e] - mean) * rstd * lng[e];
-      *reinterpret_cast<uint4*>(xn + (size_t)m * d + c0) = pack8(xo);
+      *reinterpret_cast<uint4*>(xn + (size_t)m * d + c0) = hc2::pack8(xo);
     }
     if (threadIdx.x == 0) {
       float* a = aux + (size_t)m * HC_AUX;
@@ -250,12 +226,12 @@ hc_pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* _
 template <int S, int MAXT>
 __global__ void __launch_bounds__(MAXT)
 hc_pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __restrict__ Y,
-                  const float* __restrict__ beta_prev, const float* __restrict__ x_expand, HcParams prm,
+                  const float* __restrict__ beta_prev, const float* __restrict__ x_expand, hc2::Params prm,
                   const float* __restrict__ aux, const __nv_bfloat16* __restrict__ dR_out,
                   const __nv_bfloat16* __restrict__ dxn, const __nv_bfloat16* __restrict__ dbin_extra,
                   const float* __restrict__ dbeta, __nv_bfloat16* __restrict__ dR_in,
                   __nv_bfloat16* __restrict__ dY, float* __restrict__ dbeta_prev, float* __restrict__ dx_expand,
-                  float dx_scale, HcGrads gr, int M, int d) {
+                  float dx_scale, hc2::Grads gr, int M, int d) {
   constexpr int HC_S = S, HC_T = S + 1, HC_AUX = hc2::aux_floats(S), HALF = HC_S * HC_T + HC_S;
   __shared__ float red[2 * HALF * HC_MAX_WARPS];  // the largest block_sum: S*T + S values
   extern __shared__ float dyn_smem[];
@@ -267,9 +243,12 @@ hc_pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* _
   const float sqrt_d = sqrtf((float)d);
   float g1[8], bfv[8], lng[8];
   if (act) {
-    load8f(prm.gamma_hc + c0, g1);
-    load8f(prm.dyn_beta + c0, bfv);
-    load8f(prm.ln_gamma + c0, lng);
+    hc2::lds4(prm.gamma_hc + c0, g1);
+    hc2::lds4(prm.gamma_hc + c0 + 4, g1 + 4);
+    hc2::lds4(prm.dyn_beta + c0, bfv);
+    hc2::lds4(prm.dyn_beta + c0 + 4, bfv + 4);
+    hc2::lds4(prm.ln_gamma + c0, lng);
+    hc2::lds4(prm.ln_gamma + c0 + 4, lng + 4);
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       g1[e] = (g1[e] + 1.f) * sqrt_d;
@@ -317,24 +296,25 @@ hc_pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* _
     if (act) {
       if (x_expand != nullptr) {
         float xv[8];
-        load8f(x_expand + (size_t)m * d + c0, xv);
+        hc2::lds4(x_expand + (size_t)m * d + c0, xv);
+        hc2::lds4(x_expand + (size_t)m * d + c0 + 4, xv + 4);
 #pragma unroll
         for (int s = 0; s < HC_S; ++s)
 #pragma unroll
           for (int e = 0; e < 8; ++e) R[s][e] = xv[e];
       } else {
-        unpack8(*reinterpret_cast<const uint4*>(Y + (size_t)m * d + c0), yv);
+        hc2::unpack8(*reinterpret_cast<const uint4*>(Y + (size_t)m * d + c0), yv);
 #pragma unroll
         for (int s = 0; s < HC_S; ++s) {
           float rv[8];
-          unpack8(*reinterpret_cast<const uint4*>(R_in + ((size_t)m * HC_S + s) * d + c0), rv);
+          hc2::unpack8(*reinterpret_cast<const uint4*>(R_in + ((size_t)m * HC_S + s) * d + c0), rv);
 #pragma unroll
           for (int e = 0; e < 8; ++e) R[s][e] = rv[e] + bp[s] * yv[e];
         }
       }
 #pragma unroll
       for (int s = 0; s < HC_S; ++s)
-        unpack8(*reinterpret_cast<const uint4*>(dR_out + ((size_t)m * HC_S + s) * d + c0), dmix[s + 1]);
+        hc2::unpack8(*reinterpret_cast<const uint4*>(dR_out + ((size_t)m * HC_S + s) * d + c0), dmix[s + 1]);
     } else {
 #pragma unroll
       for (int s = 0; s < HC_S; ++s)
@@ -346,7 +326,7 @@ hc_pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* _
     float lnred[2] = {0.f, 0.f};
     if (act) {
       float dx8[8];
-      unpack8(*reinterpret_cast<const uint4*>(dxn + (size_t)m * d + c0), dx8);
+      hc2::unpack8(*reinterpret_cast<const uint4*>(dxn + (size_t)m * d + c0), dx8);
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
         float b = 0.f;
@@ -365,7 +345,7 @@ hc_pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* _
       float ex[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) ex[e] = 0.f;
-      if (dbin_extra != nullptr) unpack8(*reinterpret_cast<const uint4*>(dbin_extra + (size_t)m * d + c0), ex);
+      if (dbin_extra != nullptr) hc2::unpack8(*reinterpret_cast<const uint4*>(dbin_extra + (size_t)m * d + c0), ex);
 #pragma unroll
       for (int e = 0; e < 8; ++e) dmix[0][e] = rstd * (gl[e] - m1 - xhat[e] * m2) + ex[e];
     } else {
@@ -465,10 +445,10 @@ hc_pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* _
           for (int s = 0; s < HC_S; ++s) acc += bp[s] * dR[s][e];
           dy[e] = acc;
         }
-        *reinterpret_cast<uint4*>(dY + (size_t)m * d + c0) = pack8(dy);
+        *reinterpret_cast<uint4*>(dY + (size_t)m * d + c0) = hc2::pack8(dy);
 #pragma unroll
         for (int s = 0; s < HC_S; ++s)
-          *reinterpret_cast<uint4*>(dR_in + ((size_t)m * HC_S + s) * d + c0) = pack8(dR[s]);
+          *reinterpret_cast<uint4*>(dR_in + ((size_t)m * HC_S + s) * d + c0) = hc2::pack8(dR[s]);
       }
       if (threadIdx.x == 0) {
 #pragma unroll
@@ -512,20 +492,23 @@ hc_post_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* 
   const int c0 = threadIdx.x * 8;
   const bool act = c0 < d;
   float lng[8];
-  if (act) load8f(ln_gamma + c0, lng);
+  if (act) {
+    hc2::lds4(ln_gamma + c0, lng);
+    hc2::lds4(ln_gamma + c0 + 4, lng + 4);
+  }
   for (int m = blockIdx.x; m < M; m += gridDim.x) {
     float xs[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) xs[e] = 0.f;
     if (act) {
       float yv[8];
-      unpack8(*reinterpret_cast<const uint4*>(Y + (size_t)m * d + c0), yv);
+      hc2::unpack8(*reinterpret_cast<const uint4*>(Y + (size_t)m * d + c0), yv);
       float bsum = 0.f;
 #pragma unroll
       for (int s = 0; s < HC_S; ++s) {
         bsum += beta_prev[(size_t)m * HC_S + s];
         float rv[8];
-        unpack8(*reinterpret_cast<const uint4*>(R_in + ((size_t)m * HC_S + s) * d + c0), rv);
+        hc2::unpack8(*reinterpret_cast<const uint4*>(R_in + ((size_t)m * HC_S + s) * d + c0), rv);
 #pragma unroll
         for (int e = 0; e < 8; ++e) xs[e] += rv[e];
       }
@@ -548,7 +531,7 @@ hc_post_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* 
       float o[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) o[e] = (xs[e] - mean) * rstd * lng[e];
-      *reinterpret_cast<uint4*>(out + (size_t)m * d + c0) = pack8(o);
+      *reinterpret_cast<uint4*>(out + (size_t)m * d + c0) = hc2::pack8(o);
     }
     if (threadIdx.x == 0) {
       stats[(size_t)m * 2] = mean;
@@ -572,7 +555,10 @@ hc_post_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* 
   float lng[8], gLn[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) gLn[e] = 0.f;
-  if (act) load8f(ln_gamma + c0, lng);
+  if (act) {
+    hc2::lds4(ln_gamma + c0, lng);
+    hc2::lds4(ln_gamma + c0 + 4, lng + 4);
+  }
   for (int m = blockIdx.x; m < M; m += gridDim.x) {
     const float mean = stats[(size_t)m * 2], rstd = stats[(size_t)m * 2 + 1];
     float xs[8], yv[8], gl[8], xhat[8];
@@ -581,17 +567,17 @@ hc_post_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* 
 #pragma unroll
     for (int e = 0; e < 8; ++e) { xs[e] = 0.f; yv[e] = 0.f; }
     if (act) {
-      unpack8(*reinterpret_cast<const uint4*>(Y + (size_t)m * d + c0), yv);
+      hc2::unpack8(*reinterpret_cast<const uint4*>(Y + (size_t)m * d + c0), yv);
 #pragma unroll
       for (int s = 0; s < HC_S; ++s) {
         bsum += beta_prev[(size_t)m * HC_S + s];
         float rv[8];
-        unpack8(*reinterpret_cast<const uint4*>(R_in + ((size_t)m * HC_S + s) * d + c0), rv);
+        hc2::unpack8(*reinterpret_cast<const uint4*>(R_in + ((size_t)m * HC_S + s) * d + c0), rv);
 #pragma unroll
         for (int e = 0; e < 8; ++e) xs[e] += rv[e];
       }
       float dv[8];
-      unpack8(*reinterpret_cast<const uint4*>(dout + (size_t)m * d + c0), dv);
+      hc2::unpack8(*reinterpret_cast<const uint4*>(dout + (size_t)m * d + c0), dv);
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
         xs[e] += bsum * yv[e];
@@ -617,13 +603,13 @@ hc_post_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* 
     }
     block_sum<1, HALF>(db, red, which);
     if (act) {
-      const uint4 pk = pack8(dxs);
+      const uint4 pk = hc2::pack8(dxs);
 #pragma unroll
       for (int s = 0; s < HC_S; ++s) *reinterpret_cast<uint4*>(dR_in + ((size_t)m * HC_S + s) * d + c0) = pk;
       float dy[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) dy[e] = bsum * dxs[e];
-      *reinterpret_cast<uint4*>(dY + (size_t)m * d + c0) = pack8(dy);
+      *reinterpret_cast<uint4*>(dY + (size_t)m * d + c0) = hc2::pack8(dy);
     }
     if (threadIdx.x == 0) {
 #pragma unroll
@@ -658,12 +644,16 @@ static inline size_t hc_smem_optin() {
       ALM_CUDA_OK(cudaFuncSetAttribute(K<S, T_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(smem)));  \
     K<S, T_><<<(grid), (threads), (smem), (stream)>>>(__VA_ARGS__);                                           \
   } while (0)
+#define HC_DISPATCH_FROM_256(K, grid, threads, smem, stream, ...)                             \
+  do {                                                                                        \
+    if ((threads) <= 256) HC_LAUNCH_ONE(K, 256, grid, threads, smem, stream, __VA_ARGS__);      \
+    else if ((threads) <= 512) HC_LAUNCH_ONE(K, 512, grid, threads, smem, stream, __VA_ARGS__); \
+    else HC_LAUNCH_ONE(K, 1024, grid, threads, smem, stream, __VA_ARGS__);                      \
+  } while (0)
 #define HC_DISPATCH(K, grid, threads, smem, stream, ...)                                      \
   do {                                                                                        \
     if ((threads) <= 128) HC_LAUNCH_ONE(K, 128, grid, threads, smem, stream, __VA_ARGS__);      \
-    else if ((threads) <= 256) HC_LAUNCH_ONE(K, 256, grid, threads, smem, stream, __VA_ARGS__); \
-    else if ((threads) <= 512) HC_LAUNCH_ONE(K, 512, grid, threads, smem, stream, __VA_ARGS__); \
-    else HC_LAUNCH_ONE(K, 1024, grid, threads, smem, stream, __VA_ARGS__);                      \
+    else HC_DISPATCH_FROM_256(K, grid, threads, smem, stream, __VA_ARGS__);                     \
   } while (0)
 static inline int hc_grid(int M, int threads) {
   const int per_sm = max(1, 1024 / threads);
@@ -674,61 +664,58 @@ static inline int hc_grid(int M, int threads) {
 // ---------------------------------------------------------------------------------------------
 // launchers for S streams (argument checks that do not depend on S are in the C ABI entries, hyper_conn.cu)
 // ---------------------------------------------------------------------------------------------
+// a kernel that takes more than 48 KB of dynamic shared memory: opt in once, for the largest size it is launched with
+template <auto K>
+cudaError_t hc_opt_in(size_t bytes) {
+  static const cudaError_t err = cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  return err;
+}
+
 template <int S>
 int hc_pre_fwd_s(const void* R_in, const void* Y, const float* beta_prev, const float* x_expand, const float* gamma_hc,
                  const float* dyn_alpha, const float* dyn_beta, const float* static_alpha, const float* static_beta,
                  const float* alpha_scale, const float* beta_scale, const float* ln_gamma, void* R_out, void* bin,
                  void* xn, float* beta_out, float* aux, int M, int d, cudaStream_t stream) {
-  if constexpr (hcr::ring_ok(S) || hcr::ring_wide_ok(S)) {
-    if (d <= 1024) {  // second-generation kernel: 2 or 4 warps per token, no CTA-wide barriers
-      hc2::Params p2{gamma_hc, dyn_alpha, dyn_beta, static_alpha, static_beta, alpha_scale, beta_scale, ln_gamma};
-      // S <= 4: 2 warps per token (4 warps per token was slower at d=1024).  S >= 5: 4 warps per token, so that a
-      // thread holds one 8-channel chunk of each stream (R[S][8]) and the kernel stays within its registers
-      constexpr int tpt = S <= 4 ? 64 : 128;
-      const int tok = hc2::THREADS / tpt;
-      const int grid = min(ceil_div(M, tok), num_sms() * 2);
-      const size_t smem = hc2::fwd_smem(S, d, tpt);
-#define HC2_FWD_ARGS (const __nv_bfloat16*)R_in, (const __nv_bfloat16*)Y, beta_prev, x_expand, p2, (__nv_bfloat16*)R_out, \
+  const hc2::Params prm{gamma_hc, dyn_alpha, dyn_beta, static_alpha, static_beta, alpha_scale, beta_scale, ln_gamma};
+  if (d <= 1024) {  // second-generation kernel: 2 or 4 warps per token, no CTA-wide barriers
+    // S <= 4: 2 warps per token (4 warps per token was slower at d=1024).  S >= 5: 4 warps per token, so that a
+    // thread holds one 8-channel chunk of each stream (R[S][8]) and the kernel stays within its registers
+    constexpr int tpt = S <= 4 ? 64 : 128;
+    const int tok = hc2::THREADS / tpt;
+    const int grid = min(ceil_div(M, tok), num_sms() * 2);
+    const size_t smem = hc2::fwd_smem(S, d, tpt);
+#define HC2_FWD_ARGS (const __nv_bfloat16*)R_in, (const __nv_bfloat16*)Y, beta_prev, x_expand, prm, (__nv_bfloat16*)R_out, \
                      (__nv_bfloat16*)bin, (__nv_bfloat16*)xn, beta_out, aux, M, d
-      if constexpr (S <= 4) {
-        if (d <= 512) hc2::pre_fwd_kernel<S, 1, 64><<<grid, hc2::THREADS, smem, stream>>>(HC2_FWD_ARGS);
-        else hc2::pre_fwd_kernel<S, 2, 64><<<grid, hc2::THREADS, smem, stream>>>(HC2_FWD_ARGS);
-      } else {
-        static const cudaError_t opt = cudaFuncSetAttribute(
-            hc2::pre_fwd_kernel<S, 1, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hc2::fwd_smem(S, 1024, 128));
-        ALM_CUDA_OK(opt);
-        hc2::pre_fwd_kernel<S, 1, 128><<<grid, hc2::THREADS, smem, stream>>>(HC2_FWD_ARGS);
-      }
-#undef HC2_FWD_ARGS
-      ALM_CHECK_LAUNCH();
-      ALM_LAUNCHED(1);
-      return ALM_OK;
+    if constexpr (S <= 4) {
+      if (d <= 512) hc2::pre_fwd_kernel<S, 1, 64><<<grid, hc2::THREADS, smem, stream>>>(HC2_FWD_ARGS);
+      else hc2::pre_fwd_kernel<S, 2, 64><<<grid, hc2::THREADS, smem, stream>>>(HC2_FWD_ARGS);
+    } else {
+      ALM_CUDA_OK((hc_opt_in<hc2::pre_fwd_kernel<S, 1, 128>>(hc2::fwd_smem(S, 1024, 128))));
+      hc2::pre_fwd_kernel<S, 1, 128><<<grid, hc2::THREADS, smem, stream>>>(HC2_FWD_ARGS);
     }
+#undef HC2_FWD_ARGS
+    ALM_CHECK_LAUNCH();
+    ALM_LAUNCHED(1);
+    return ALM_OK;
   }
-  HcParams prm{gamma_hc, dyn_alpha, dyn_beta, static_alpha, static_beta, alpha_scale, beta_scale, ln_gamma};
   const int threads = hc_threads(d);
-  HC_DISPATCH(hc_pre_fwd_kernel, hc_grid(M, threads), threads, (S + 1) * d * sizeof(float), stream,
-              (const __nv_bfloat16*)R_in, (const __nv_bfloat16*)Y, beta_prev, x_expand, prm, (__nv_bfloat16*)R_out,
-              (__nv_bfloat16*)bin, (__nv_bfloat16*)xn, beta_out, aux, M, d);
+  // d > 1024 here, so threads >= 160: the pre kernels need no MAXT = 128 instantiation
+  HC_DISPATCH_FROM_256(hc_pre_fwd_kernel, hc_grid(M, threads), threads, (S + 1) * d * sizeof(float), stream,
+                       (const __nv_bfloat16*)R_in, (const __nv_bfloat16*)Y, beta_prev, x_expand, prm,
+                       (__nv_bfloat16*)R_out, (__nv_bfloat16*)bin, (__nv_bfloat16*)xn, beta_out, aux, M, d);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);
   return ALM_OK;
 }
 
-// the ring needs more than 48 KB of dynamic shared memory: opt in once per instantiation, for the largest d it takes
+// the ring backward for S streams and its shared-memory layout: hyper_conn_ring.cuh for S <= 4,
+// hyper_conn_ring_wide.cuh for S = 5..8
 template <int S, bool EXPAND>
-cudaError_t hcr_opt_in() {
-  if constexpr (hcr::ring_ok(S)) {
-    static const cudaError_t err = cudaFuncSetAttribute(
-        hcr::pre_bwd_kernel<S, EXPAND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hcr::smem_bytes<S>(1024));
-    return err;
-  } else {
-    static const cudaError_t err =
-        cudaFuncSetAttribute(hcr::pre_bwd_wide_kernel<S, EXPAND>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)hcr::smem_bytes_w<S>(1024));
-    return err;
-  }
+constexpr auto hcr_kernel() {
+  if constexpr (hcr::ring_ok(S)) return hcr::pre_bwd_kernel<S, EXPAND>;
+  else return hcr::pre_bwd_wide_kernel<S, EXPAND>;
 }
+template <int S> using HcrLayout = std::conditional_t<hcr::ring_ok(S), hcr::NarrowLayout<S>, hcr::WideLayout<S>>;
 
 template <int S>
 int hc_pre_bwd_s(const void* R_in, const void* Y, const float* beta_prev, const float* x_expand, const float* gamma_hc,
@@ -738,47 +725,41 @@ int hc_pre_bwd_s(const void* R_in, const void* Y, const float* beta_prev, const 
                  float* dbeta_prev, float* dx_expand, float dx_scale, float* g_gamma_hc, float* g_dyn_alpha,
                  float* g_dyn_beta, float* g_static_alpha, float* g_static_beta, float* g_alpha_scale,
                  float* g_beta_scale, float* g_ln_gamma, int M, int d, cudaStream_t stream) {
-  if constexpr (hcr::ring_ok(S) || hcr::ring_wide_ok(S)) {
-    if (d <= 1024) {
-      // the ring stages rows with bulk copies: every staged row must start on 16 B (d % 8 == 0 keeps it so per row)
-      const void* staged[] = {R_in, Y, beta_prev, x_expand, aux, dR_out, dxn, dbin_extra, dbeta};
-      for (const void* p : staged) ALM_REQUIRE((reinterpret_cast<uintptr_t>(p) & 15) == 0, ALM_ERR_ARG);
-      ALM_REQUIRE(x_expand != nullptr ? dx_expand != nullptr
-                                      : (R_in && Y && beta_prev && dR_in && dY && dbeta_prev), ALM_ERR_ARG);
-      hc2::Params p{gamma_hc, dyn_alpha, dyn_beta, static_alpha, static_beta, alpha_scale, beta_scale, ln_gamma};
-      hc2::Grads g{g_gamma_hc, g_dyn_alpha, g_dyn_beta, g_static_alpha, g_static_beta, g_alpha_scale, g_beta_scale,
-                   g_ln_gamma};
-      const int grid = min(M, num_sms());
-      size_t smem;
-      if constexpr (hcr::ring_ok(S)) smem = hcr::smem_bytes<S>(d);
-      else smem = hcr::smem_bytes_w<S>(d);
-#define HCR_ARGS (const __nv_bfloat16*)R_in, (const __nv_bfloat16*)Y, beta_prev, x_expand, p, aux,                  \
+  const hc2::Params prm{gamma_hc, dyn_alpha, dyn_beta, static_alpha, static_beta, alpha_scale, beta_scale, ln_gamma};
+  const hc2::Grads gr{g_gamma_hc, g_dyn_alpha, g_dyn_beta, g_static_alpha, g_static_beta, g_alpha_scale, g_beta_scale,
+                      g_ln_gamma};
+  if (d <= 1024) {
+    // the ring stages rows with bulk copies: every staged row must start on 16 B (d % 8 == 0 keeps it so per row)
+    const void* staged[] = {R_in, Y, beta_prev, x_expand, aux, dR_out, dxn, dbin_extra, dbeta};
+    for (const void* p : staged) ALM_REQUIRE((reinterpret_cast<uintptr_t>(p) & 15) == 0, ALM_ERR_ARG);
+    ALM_REQUIRE(x_expand != nullptr ? dx_expand != nullptr
+                                    : (R_in && Y && beta_prev && dR_in && dY && dbeta_prev), ALM_ERR_ARG);
+    const int grid = min(M, num_sms());
+    const size_t smem = HcrLayout<S>::smem_bytes(d), smem_max = HcrLayout<S>::smem_bytes(1024);
+#define HCR_ARGS (const __nv_bfloat16*)R_in, (const __nv_bfloat16*)Y, beta_prev, x_expand, prm, aux,                  \
                  (const __nv_bfloat16*)dR_out, (const __nv_bfloat16*)dxn, (const __nv_bfloat16*)dbin_extra, dbeta, \
-                 (__nv_bfloat16*)dR_in, (__nv_bfloat16*)dY, dbeta_prev, dx_expand, dx_scale, g, M, d
-      if (x_expand != nullptr) {
-        ALM_CUDA_OK((hcr_opt_in<S, true>()));
-        if constexpr (hcr::ring_ok(S)) hcr::pre_bwd_kernel<S, true><<<grid, hcr::THREADS, smem, stream>>>(HCR_ARGS);
-        else hcr::pre_bwd_wide_kernel<S, true><<<grid, hcr::THREADS, smem, stream>>>(HCR_ARGS);
-      } else {
-        ALM_CUDA_OK((hcr_opt_in<S, false>()));
-        if constexpr (hcr::ring_ok(S)) hcr::pre_bwd_kernel<S, false><<<grid, hcr::THREADS, smem, stream>>>(HCR_ARGS);
-        else hcr::pre_bwd_wide_kernel<S, false><<<grid, hcr::THREADS, smem, stream>>>(HCR_ARGS);
-      }
-#undef HCR_ARGS
-      ALM_CHECK_LAUNCH();
-      ALM_LAUNCHED(1);
-      return ALM_OK;
+                 (__nv_bfloat16*)dR_in, (__nv_bfloat16*)dY, dbeta_prev, dx_expand, dx_scale, gr, M, d
+    if (x_expand != nullptr) {
+      constexpr auto K = hcr_kernel<S, true>();
+      ALM_CUDA_OK(hc_opt_in<K>(smem_max));
+      K<<<grid, hcr::THREADS, smem, stream>>>(HCR_ARGS);
+    } else {
+      constexpr auto K = hcr_kernel<S, false>();
+      ALM_CUDA_OK(hc_opt_in<K>(smem_max));
+      K<<<grid, hcr::THREADS, smem, stream>>>(HCR_ARGS);
     }
+#undef HCR_ARGS
+    ALM_CHECK_LAUNCH();
+    ALM_LAUNCHED(1);
+    return ALM_OK;
   }
-  HcParams prm{gamma_hc, dyn_alpha, dyn_beta, static_alpha, static_beta, alpha_scale, beta_scale, ln_gamma};
-  HcGrads gr{g_gamma_hc, g_dyn_alpha, g_dyn_beta, g_static_alpha, g_static_beta, g_alpha_scale, g_beta_scale,
-             g_ln_gamma};
   const int threads = hc_threads(d);
   const int grid = min(M, num_sms() * 2);
-  HC_DISPATCH(hc_pre_bwd_kernel, grid, threads, 2 * (S + 1) * d * sizeof(float), stream,
-              (const __nv_bfloat16*)R_in, (const __nv_bfloat16*)Y, beta_prev, x_expand, prm, aux,
-              (const __nv_bfloat16*)dR_out, (const __nv_bfloat16*)dxn, (const __nv_bfloat16*)dbin_extra, dbeta,
-              (__nv_bfloat16*)dR_in, (__nv_bfloat16*)dY, dbeta_prev, dx_expand, dx_scale, gr, M, d);
+  // d > 1024 here, so threads >= 160: the pre kernels need no MAXT = 128 instantiation
+  HC_DISPATCH_FROM_256(hc_pre_bwd_kernel, grid, threads, 2 * (S + 1) * d * sizeof(float), stream,
+                       (const __nv_bfloat16*)R_in, (const __nv_bfloat16*)Y, beta_prev, x_expand, prm, aux,
+                       (const __nv_bfloat16*)dR_out, (const __nv_bfloat16*)dxn, (const __nv_bfloat16*)dbin_extra, dbeta,
+                       (__nv_bfloat16*)dR_in, (__nv_bfloat16*)dY, dbeta_prev, dx_expand, dx_scale, gr, M, d);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);
   return ALM_OK;

@@ -27,7 +27,6 @@ namespace hcr {
 
 constexpr int NC = 2;                   // warpgroups
 constexpr int NSC = 3;                  // ring stages per warpgroup (one token each)
-constexpr int NST = NC * NSC;
 constexpr int THREADS = NC * 128;
 constexpr int NRED = 34;                // pass-1 per-token sums, zero-padded: 2 + 4S + S*S <= 34 for S <= 4
 constexpr int MAILW = 36;               // floats per warp row of the reduction mailbox
@@ -51,12 +50,19 @@ template <int S> __host__ __device__ inline int off_dbin(int d) { return off_y<S
 template <int S> __host__ __device__ inline int stage_bytes(int d) {
   return (scal_bytes(S) + (4 * S + 6) * d + 127) / 128 * 128;
 }
-// shared memory: params [S+3][d] fp32 | mailboxes [NC][4][MAILW] | dbeta_prev partials [NC][4][S] | coefficients
-// [NC][S][COEF] | full[NST] mbarriers | ring [NC][NSC] stages (128-B aligned)
-template <int S> __host__ __device__ inline int ring_offset(int d) {
-  return (4 * ((S + 3) * d + NC * (4 * MAILW + 4 * S + S * COEF)) + 8 * NST + 127) / 128 * 128;
-}
-template <int S> inline size_t smem_bytes(int d) { return (size_t)ring_offset<S>(d) + (size_t)NST * stage_bytes<S>(d); }
+// Shared memory of a ring backward with NSC_ stages per warpgroup, MW_ floats per mailbox row, CW_ per coefficient
+// row and ZW_ of z-partials per warpgroup (none for S <= 4):
+//   params [S+3][d] fp32 | mailboxes [NC][4][MW] | dbeta_prev partials [NC][4][S] | coefficients [NC][S][CW] |
+//   z-partials [NC][ZW] | full[NC * NSC] mbarriers | ring [NC][NSC] stages (128-B aligned)
+template <int S, int NSC_, int MW_, int CW_, int ZW_>
+struct RingLayout {
+  static constexpr int NSC = NSC_, NST = NC * NSC_, MW = MW_, CW = CW_, ZW = ZW_;
+  __host__ __device__ static int ring_offset(int d) {
+    return (4 * ((S + 3) * d + NC * (4 * MW + 4 * S + S * CW + ZW)) + 8 * NST + 127) / 128 * 128;
+  }
+  static size_t smem_bytes(int d) { return (size_t)ring_offset(d) + (size_t)NST * stage_bytes<S>(d); }
+};
+template <int S> using NarrowLayout = RingLayout<S, NSC, MAILW, COEF, 0>;
 
 // the per-channel parameters are stored so that thread l's channels 8l..8l+3 and 8l+4..8l+7 are two float4 at
 // [4l] and [d/2 + 4l]: a warp's 16-B loads are then contiguous (no bank-conflict replays)
@@ -84,6 +90,164 @@ __device__ __forceinline__ float reduce_scatter32(float (&v)[32], int lane) {
   return v[0];
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// The ring protocol and the parameter staging / flush, shared by pre_bwd_kernel and pre_bwd_wide_kernel
+// ---------------------------------------------------------------------------------------------------------------------
+// sPar [S+3][d] (par_index layout): ln_gamma, g1 * dyn_alpha[:, t], g1 * dyn_beta; then the NST full barriers armed
+template <int S, int NST>
+__device__ __forceinline__ void stage_params(float* sPar, uint64_t* full, const hc2::Params& prm, int d, float sqrt_d) {
+  constexpr int T = S + 1;
+  for (int c = threadIdx.x; c < d; c += blockDim.x) {
+    const int p = par_index(c, d);
+    const float g1 = (prm.gamma_hc[c] + 1.f) * sqrt_d;
+    sPar[p] = prm.ln_gamma[c];
+#pragma unroll
+    for (int t = 0; t < T; ++t) sPar[(1 + t) * d + p] = g1 * prm.dyn_alpha[(size_t)c * T + t];
+    sPar[(1 + T) * d + p] = g1 * prm.dyn_beta[c];
+  }
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < NST; ++i) mbar_init(&full[i], 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+}
+
+// stage token m into stage ls of a warpgroup's ring (warp 3: lane 0 arms the stage's barrier, lanes 0-7 copy)
+template <int S, bool EXPAND>
+__device__ __forceinline__ void fill_stage(unsigned char* my_ring, uint64_t* my_full, int ls, int stage_b, int m, int d,
+                                           int lane, bool has_dbin, const __nv_bfloat16* R_in, const __nv_bfloat16* Y,
+                                           const float* beta_prev, const float* x_expand, const float* aux,
+                                           const __nv_bfloat16* dR_out, const __nv_bfloat16* dxn,
+                                           const __nv_bfloat16* dbin_extra, const float* dbeta) {
+  constexpr int AUX = hc2::aux_floats(S), SCAL_B = scal_bytes(S);
+  uint64_t* bar = my_full + ls;
+  unsigned char* st = my_ring + (size_t)ls * stage_b;
+  constexpr int head = AUX * 4 + (head_bulk(S) ? (EXPAND ? 4 * S : 8 * S) : 0);
+  const uint32_t bytes = head + (EXPAND ? 4 * d : (2 * S + 2) * d) + (2 * S + 2) * d + (has_dbin ? 2 * d : 0);
+  if (lane == 0) mbar_arrive_expect_tx(bar, bytes);
+  __syncwarp();
+  const size_t md = (size_t)m * d;
+  switch (lane) {
+    case 0: bulk_copy_g2s(st, aux + (size_t)m * AUX, AUX * 4, bar); break;
+    case 1:
+      if (head_bulk(S)) bulk_copy_g2s(st + AUX * 4, dbeta + (size_t)m * S, 4 * S, bar);
+      break;
+    case 2:
+      if (head_bulk(S) && !EXPAND) bulk_copy_g2s(st + AUX * 4 + 4 * S, beta_prev + (size_t)m * S, 4 * S, bar);
+      break;
+    case 3:
+      if (EXPAND) bulk_copy_g2s(st + SCAL_B, x_expand + md, 4 * d, bar);
+      else bulk_copy_g2s(st + SCAL_B, R_in + md * S, 2 * S * d, bar);
+      break;
+    case 4: bulk_copy_g2s(st + off_dr<S>(d), dR_out + md * S, 2 * S * d, bar); break;
+    case 5:
+      if (!EXPAND) bulk_copy_g2s(st + off_y<S>(d), Y + md, 2 * d, bar);
+      break;
+    case 6: bulk_copy_g2s(st + off_dxn<S>(d), dxn + md, 2 * d, bar); break;
+    case 7:
+      if (has_dbin) bulk_copy_g2s(st + off_dbin<S>(d), dbin_extra + md, 2 * d, bar);
+      break;
+    default: break;
+  }
+}
+
+// the next stage and barrier phase of a warpgroup's ring
+template <int NSC_>
+__device__ __forceinline__ void advance(int& ls, uint32_t& phase) {
+  if (++ls == NSC_) {
+    ls = 0;
+    phase ^= 1;
+  }
+}
+
+// sum i of a warpgroup's four mailbox rows of MW floats
+template <int MW>
+__device__ __forceinline__ float mail_total(const float* mail, int i) {
+  return (mail[i] + mail[MW + i]) + (mail[2 * MW + i] + mail[3 * MW + i]);
+}
+
+// this thread's per-channel partials G [S+2][8] and gLn [8] -> the ring, idle once every stage has been consumed:
+// [NC][S+3][d]
+template <int S>
+__device__ __forceinline__ void store_partials(unsigned char* ring, const float (&G)[S + 2][8], const float (&gLn)[8],
+                                               int cw, int lt, int d) {
+  constexpr int NP = S + 3, NG = S + 2;
+  float* buf = reinterpret_cast<float*>(ring) + (size_t)cw * NP * d + lt * 8;
+#pragma unroll
+  for (int c = 0; c < NG; ++c) {
+    *reinterpret_cast<float4*>(buf + c * d) = make_float4(G[c][0], G[c][1], G[c][2], G[c][3]);
+    *reinterpret_cast<float4*>(buf + c * d + 4) = make_float4(G[c][4], G[c][5], G[c][6], G[c][7]);
+  }
+  *reinterpret_cast<float4*>(buf + NG * d) = make_float4(gLn[0], gLn[1], gLn[2], gLn[3]);
+  *reinterpret_cast<float4*>(buf + NG * d + 4) = make_float4(gLn[4], gLn[5], gLn[6], gLn[7]);
+}
+
+// CTA sum of the per-channel partials, folded into the parameter gradients:
+//   d dyn_alpha[:, t] += g1 G_t,  d dyn_beta += g1 G_T,  d gamma += sqrt(d) sum_c P_c G_c,  g1 = (gamma + 1) sqrt(d)
+template <int S>
+__device__ __forceinline__ void flush_param_grads(const unsigned char* ring, const hc2::Params& prm,
+                                                  const hc2::Grads& gr, int d, float sqrt_d) {
+  constexpr int T = S + 1, NP = S + 3, NG = S + 2;
+  const float* buf = reinterpret_cast<const float*>(ring);
+  for (int i = threadIdx.x; i < d; i += blockDim.x) {
+    float g[NP];
+#pragma unroll
+    for (int k = 0; k < NP; ++k) {
+      g[k] = 0.f;
+#pragma unroll
+      for (int c = 0; c < NC; ++c) g[k] += buf[(size_t)(c * NP + k) * d + i];
+    }
+    const float g1 = (prm.gamma_hc[i] + 1.f) * sqrt_d;
+    float acc = g[T] * prm.dyn_beta[i];
+    atomicAdd(gr.dyn_beta + i, g1 * g[T]);
+#pragma unroll
+    for (int t = 0; t < T; ++t) {
+      acc = fmaf(g[t], prm.dyn_alpha[(size_t)i * T + t], acc);
+      atomicAdd(gr.dyn_alpha + (size_t)i * T + t, g1 * g[t]);
+    }
+    atomicAdd(gr.gamma_hc + i, sqrt_d * acc);
+    atomicAdd(gr.ln_gamma + i, g[NG]);
+  }
+}
+
+// stage the k-th token of warpgroup cw (if the CTA has one) into its stage k % NSC
+template <int S, bool EXPAND, int NSC_>
+__device__ __forceinline__ void fill_token(int k, int cw, int M, unsigned char* my_ring, uint64_t* my_full, int stage_b,
+                                           int d, int lane, bool has_dbin, const __nv_bfloat16* R_in,
+                                           const __nv_bfloat16* Y, const float* beta_prev, const float* x_expand,
+                                           const float* aux, const __nv_bfloat16* dR_out, const __nv_bfloat16* dxn,
+                                           const __nv_bfloat16* dbin_extra, const float* dbeta) {
+  const int m = blockIdx.x + (cw + k * NC) * gridDim.x;
+  if (m >= M) return;
+  const int ls = k % NSC_;
+  fill_stage<S, EXPAND>(my_ring, my_full, ls, stage_b, m, d, lane, has_dbin, R_in, Y, beta_prev, x_expand, aux, dR_out,
+                        dxn, dbin_extra, dbeta);
+}
+// after the pass-1 barrier of the k-th token every thread is past token k - 1: warp 3 refills its stage with token
+// k - 1 + NSC
+template <int NSC_, class F>
+__device__ __forceinline__ void refill(int k, int w, F& fill) {
+  if (k > 0 && w == 3) {
+    fence_proxy_async_smem();
+    fill(k - 1 + NSC_);
+  }
+}
+// stage ls of a warpgroup's ring, once the bytes of its current fill (barrier phase `phase`) have landed
+__device__ __forceinline__ const unsigned char* wait_stage(uint64_t* my_full, unsigned char* my_ring, int ls,
+                                                           uint32_t phase, int stage_b) {
+  mbar_wait(&my_full[ls], phase);
+  return my_ring + (size_t)ls * stage_b;
+}
+// this thread's per-channel parameter-gradient partials, zeroed before the first token
+template <int NG>
+__device__ __forceinline__ void zero_partials(float (&G)[NG][8], float (&gLn)[8]) {
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    gLn[e] = 0.f;
+#pragma unroll
+    for (int c = 0; c < NG; ++c) G[c][e] = 0.f;
+  }
+}
 __device__ __forceinline__ void lds8(const float* p, int half, float* f) {  // 8 parameters of a thread's channels
   hc2::lds4(p, f);
   hc2::lds4(p + half, f + 4);
@@ -108,22 +272,10 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
   float* sDbp = sMail + NC * 4 * MAILW;          // [NC][4][S]
   float* sCoef = sDbp + NC * 4 * S;              // [NC][S][COEF]
   uint64_t* full = reinterpret_cast<uint64_t*>(sCoef + NC * S * COEF);
-  unsigned char* ring = smem + ring_offset<S>(d);
+  unsigned char* ring = smem + NarrowLayout<S>::ring_offset(d);
   const int stage_b = stage_bytes<S>(d), half = d >> 1;
   const float sqrt_d = sqrtf((float)d);
-  for (int c = threadIdx.x; c < d; c += blockDim.x) {
-    const int p = par_index(c, d);
-    const float g1 = (prm.gamma_hc[c] + 1.f) * sqrt_d;
-    sPar[p] = prm.ln_gamma[c];
-#pragma unroll
-    for (int t = 0; t < T; ++t) sPar[(1 + t) * d + p] = g1 * prm.dyn_alpha[(size_t)c * T + t];
-    sPar[(1 + T) * d + p] = g1 * prm.dyn_beta[c];
-  }
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < NST; ++i) mbar_init(&full[i], 1);
-    fence_mbar_init();
-  }
-  __syncthreads();
+  stage_params<S, NarrowLayout<S>::NST>(sPar, full, prm, d, sqrt_d);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, lt = threadIdx.x & 127;
   const int cw = warp >> 2, w = lt >> 5;
   const bool act = lt * 8 < d;  // this thread owns channels
@@ -132,50 +284,15 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
   unsigned char* my_ring = ring + (size_t)cw * NSC * stage_b;
   // stage the k-th token of this warpgroup into its stage k % NSC (warp 3: lane 0 arms the barrier, lanes 0-7 copy)
   auto fill = [&](int k) {
-    const int m = blockIdx.x + (cw + k * NC) * gridDim.x;
-    if (m >= M) return;
-    const int ls = k % NSC;
-    uint64_t* bar = my_full + ls;
-    unsigned char* st = my_ring + (size_t)ls * stage_b;
-    constexpr int head = AUX * 4 + (head_bulk(S) ? (EXPAND ? 4 * S : 8 * S) : 0);
-    const uint32_t bytes = head + (EXPAND ? 4 * d : (2 * S + 2) * d) + (2 * S + 2) * d + (has_dbin ? 2 * d : 0);
-    if (lane == 0) mbar_arrive_expect_tx(bar, bytes);
-    __syncwarp();
-    const size_t md = (size_t)m * d;
-    switch (lane) {
-      case 0: bulk_copy_g2s(st, aux + (size_t)m * AUX, AUX * 4, bar); break;
-      case 1:
-        if (head_bulk(S)) bulk_copy_g2s(st + AUX * 4, dbeta + (size_t)m * S, 4 * S, bar);
-        break;
-      case 2:
-        if (head_bulk(S) && !EXPAND) bulk_copy_g2s(st + AUX * 4 + 4 * S, beta_prev + (size_t)m * S, 4 * S, bar);
-        break;
-      case 3:
-        if (EXPAND) bulk_copy_g2s(st + SCAL_B, x_expand + md, 4 * d, bar);
-        else bulk_copy_g2s(st + SCAL_B, R_in + md * S, 2 * S * d, bar);
-        break;
-      case 4: bulk_copy_g2s(st + off_dr<S>(d), dR_out + md * S, 2 * S * d, bar); break;
-      case 5:
-        if (!EXPAND) bulk_copy_g2s(st + off_y<S>(d), Y + md, 2 * d, bar);
-        break;
-      case 6: bulk_copy_g2s(st + off_dxn<S>(d), dxn + md, 2 * d, bar); break;
-      case 7:
-        if (has_dbin) bulk_copy_g2s(st + off_dbin<S>(d), dbin_extra + md, 2 * d, bar);
-        break;
-      default: break;
-    }
+    fill_token<S, EXPAND, NSC>(k, cw, M, my_ring, my_full, stage_b, d, lane, has_dbin, R_in, Y, beta_prev, x_expand,
+                             aux, dR_out, dxn, dbin_extra, dbeta);
   };
   if (w == 3) {
     for (int k = 0; k < NSC; ++k) fill(k);
   }
   {
     float G[NG][8], gLn[8];  // this thread's channels: G[c][e] = sum over its tokens of sum_s R_s C[s][c]; d ln_gamma
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      gLn[e] = 0.f;
-#pragma unroll
-      for (int c6 = 0; c6 < NG; ++c6) G[c6][e] = 0.f;
-    }
+    zero_partials(G, gLn);
     const int bar_id = 1 + cw;
     float* mail = sMail + cw * 4 * MAILW;
     float* dbpm = sDbp + cw * 4 * S;
@@ -195,8 +312,7 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
     uint32_t phase = 0;
     int pend = -1;  // token whose dbeta_prev partials wait in dbpm
     for (int k = 0, m = blockIdx.x + cw * gridDim.x; m < M; ++k, m += NC * gridDim.x) {
-      mbar_wait(&my_full[ls], phase);
-      const unsigned char* st = my_ring + (size_t)ls * stage_b;
+      const unsigned char* st = wait_stage(my_full, my_ring, ls, phase, stage_b);
       const float* a = reinterpret_cast<const float*>(st);
       const float mean = a[AUX - 2], rstd = a[AUX - 1], nmr = -mean * rstd;
       float alpha0[S], bp[S];
@@ -291,11 +407,8 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
         }
       }
       named_bar_sync(bar_id, 128);
-      if (k > 0 && w == 3) {  // every thread is past token k - 1: its stage takes token k - 1 + NSC
-        fence_proxy_async_smem();
-        fill(k - 1 + NSC);
-      }
-      auto total = [&](int i) { return (mail[i] + mail[MAILW + i]) + (mail[2 * MAILW + i] + mail[3 * MAILW + i]); };
+      refill<NSC>(k, w, fill);
+      auto total = [&](int i) { return mail_total<MAILW>(mail, i); };
       const float m1 = total(0) * inv_d, m2 = total(1) * inv_d;
       // ---------------- per-token scalars (warp 0) ----------------
       if (w == 0) {
@@ -425,10 +538,7 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
         }
         pend = m;
       }
-      if (++ls == NSC) {
-        ls = 0;
-        phase ^= 1;
-      }
+      advance<NSC>(ls, phase);
     }
     named_bar_sync(bar_id, 128);
     if (w == 0) {
@@ -444,40 +554,10 @@ pre_bwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
     }
     // per-channel partials of each warpgroup -> the ring, idle once every stage has been consumed: [NC][NP][d]
     __syncthreads();
-    if (act) {
-      float* buf = reinterpret_cast<float*>(ring) + (size_t)cw * NP * d + lt * 8;
-#pragma unroll
-      for (int c6 = 0; c6 < NG; ++c6) {
-        *reinterpret_cast<float4*>(buf + c6 * d) = make_float4(G[c6][0], G[c6][1], G[c6][2], G[c6][3]);
-        *reinterpret_cast<float4*>(buf + c6 * d + 4) = make_float4(G[c6][4], G[c6][5], G[c6][6], G[c6][7]);
-      }
-      *reinterpret_cast<float4*>(buf + NG * d) = make_float4(gLn[0], gLn[1], gLn[2], gLn[3]);
-      *reinterpret_cast<float4*>(buf + NG * d + 4) = make_float4(gLn[4], gLn[5], gLn[6], gLn[7]);
-    }
+    if (act) store_partials<S>(ring, G, gLn, cw, lt, d);
   }
   __syncthreads();
-  // CTA sum of the per-channel partials, folded into the parameter gradients:
-  //   d dyn_alpha[:, t] += g1 G_t,  d dyn_beta += g1 G_5,  d gamma += sqrt(d) sum_c P_c G_c,  g1 = (gamma + 1) sqrt(d)
-  const float* buf = reinterpret_cast<const float*>(ring);
-  for (int i = threadIdx.x; i < d; i += blockDim.x) {
-    float g[NP];
-#pragma unroll
-    for (int k = 0; k < NP; ++k) {
-      g[k] = 0.f;
-#pragma unroll
-      for (int c = 0; c < NC; ++c) g[k] += buf[(size_t)(c * NP + k) * d + i];
-    }
-    const float g1 = (prm.gamma_hc[i] + 1.f) * sqrt_d;
-    float acc = g[T] * prm.dyn_beta[i];
-    atomicAdd(gr.dyn_beta + i, g1 * g[T]);
-#pragma unroll
-    for (int t = 0; t < T; ++t) {
-      acc = fmaf(g[t], prm.dyn_alpha[(size_t)i * T + t], acc);
-      atomicAdd(gr.dyn_alpha + (size_t)i * T + t, g1 * g[t]);
-    }
-    atomicAdd(gr.gamma_hc + i, sqrt_d * acc);
-    atomicAdd(gr.ln_gamma + i, g[NG]);
-  }
+  flush_param_grads<S>(ring, prm, gr, d, sqrt_d);
 }
 
 }  // namespace hcr

@@ -16,7 +16,6 @@ namespace alm {
 namespace hcr {
 
 constexpr int NSC_W = 2;
-constexpr int NST_W = NC * NSC_W;
 __host__ __device__ constexpr bool ring_wide_ok(int S) { return S >= 5 && S <= 8; }
 __host__ __device__ constexpr int nv_w(int S) { return 4 * S + S * S; }             // sums after the two LN sums
 __host__ __device__ constexpr int rounds_w(int S) { return (nv_w(S) + 31) / 32; }
@@ -25,15 +24,8 @@ __host__ __device__ constexpr int coef_w(int S) { return (2 * S + 4 + 3) / 4 * 4
 static_assert(scal_bytes(8) % 16 == 0 && hc2::aux_floats(5) % 4 == 0 && hc2::aux_floats(7) % 4 == 0,
               "aux rows and the stage head must be 16-B multiples so that one bulk copy stages a row");
 
-// shared memory: params [S+3][d] | mailboxes [NC][4][MAILW] | dbeta_prev partials [NC][4][S] | coefficients
-// [NC][S][COEF] | z-partials [NC][S][S+2] | full[NST_W] mbarriers | ring [NC][NSC_W] stages (128-B aligned)
-template <int S> __host__ __device__ inline int ring_offset_w(int d) {
-  return (4 * ((S + 3) * d + NC * (4 * mailw_w(S) + 4 * S + S * coef_w(S) + S * (S + 2))) + 8 * NST_W + 127) / 128 *
-         128;
-}
-template <int S> inline size_t smem_bytes_w(int d) {
-  return (size_t)ring_offset_w<S>(d) + (size_t)NST_W * stage_bytes<S>(d);
-}
+// z-partials: [S][S + 2] per warpgroup
+template <int S> using WideLayout = RingLayout<S, NSC_W, mailw_w(S), coef_w(S), S * (S + 2)>;
 
 __device__ __forceinline__ void unpack4(const uint2& u, float* f) {
   f[0] = bf16_lo(u.x); f[1] = bf16_hi(u.x); f[2] = bf16_lo(u.y); f[3] = bf16_hi(u.y);
@@ -59,22 +51,10 @@ pre_bwd_wide_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16*
   float* sCoef = sDbp + NC * 4 * S;              // [NC][S][CW]
   float* sZ = sCoef + NC * S * CW;               // [NC][S][NG]
   uint64_t* full = reinterpret_cast<uint64_t*>(sZ + NC * S * NG);
-  unsigned char* ring = smem + ring_offset_w<S>(d);
+  unsigned char* ring = smem + WideLayout<S>::ring_offset(d);
   const int stage_b = stage_bytes<S>(d), half = d >> 1;
   const float sqrt_d = sqrtf((float)d);
-  for (int c = threadIdx.x; c < d; c += blockDim.x) {
-    const int p = par_index(c, d);
-    const float g1 = (prm.gamma_hc[c] + 1.f) * sqrt_d;
-    sPar[p] = prm.ln_gamma[c];
-#pragma unroll
-    for (int t = 0; t < T; ++t) sPar[(1 + t) * d + p] = g1 * prm.dyn_alpha[(size_t)c * T + t];
-    sPar[(1 + T) * d + p] = g1 * prm.dyn_beta[c];
-  }
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < NST_W; ++i) mbar_init(&full[i], 1);
-    fence_mbar_init();
-  }
-  __syncthreads();
+  stage_params<S, WideLayout<S>::NST>(sPar, full, prm, d, sqrt_d);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, lt = threadIdx.x & 127;
   const int cw = warp >> 2, w = lt >> 5;
   const bool act = lt * 8 < d;
@@ -82,50 +62,15 @@ pre_bwd_wide_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16*
   uint64_t* my_full = full + cw * NSC_W;
   unsigned char* my_ring = ring + (size_t)cw * NSC_W * stage_b;
   auto fill = [&](int k) {
-    const int m = blockIdx.x + (cw + k * NC) * gridDim.x;
-    if (m >= M) return;
-    const int ls = k % NSC_W;
-    uint64_t* bar = my_full + ls;
-    unsigned char* st = my_ring + (size_t)ls * stage_b;
-    constexpr int head = AUX * 4 + (head_bulk(S) ? (EXPAND ? 4 * S : 8 * S) : 0);
-    const uint32_t bytes = head + (EXPAND ? 4 * d : (2 * S + 2) * d) + (2 * S + 2) * d + (has_dbin ? 2 * d : 0);
-    if (lane == 0) mbar_arrive_expect_tx(bar, bytes);
-    __syncwarp();
-    const size_t md = (size_t)m * d;
-    switch (lane) {
-      case 0: bulk_copy_g2s(st, aux + (size_t)m * AUX, AUX * 4, bar); break;
-      case 1:
-        if (head_bulk(S)) bulk_copy_g2s(st + AUX * 4, dbeta + (size_t)m * S, 4 * S, bar);
-        break;
-      case 2:
-        if (head_bulk(S) && !EXPAND) bulk_copy_g2s(st + AUX * 4 + 4 * S, beta_prev + (size_t)m * S, 4 * S, bar);
-        break;
-      case 3:
-        if (EXPAND) bulk_copy_g2s(st + SCAL_B, x_expand + md, 4 * d, bar);
-        else bulk_copy_g2s(st + SCAL_B, R_in + md * S, 2 * S * d, bar);
-        break;
-      case 4: bulk_copy_g2s(st + off_dr<S>(d), dR_out + md * S, 2 * S * d, bar); break;
-      case 5:
-        if (!EXPAND) bulk_copy_g2s(st + off_y<S>(d), Y + md, 2 * d, bar);
-        break;
-      case 6: bulk_copy_g2s(st + off_dxn<S>(d), dxn + md, 2 * d, bar); break;
-      case 7:
-        if (has_dbin) bulk_copy_g2s(st + off_dbin<S>(d), dbin_extra + md, 2 * d, bar);
-        break;
-      default: break;
-    }
+    fill_token<S, EXPAND, NSC_W>(k, cw, M, my_ring, my_full, stage_b, d, lane, has_dbin, R_in, Y, beta_prev, x_expand,
+                             aux, dR_out, dxn, dbin_extra, dbeta);
   };
   if (w == 3) {
     for (int k = 0; k < NSC_W; ++k) fill(k);
   }
   {
     float G[NG][8], gLn[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      gLn[e] = 0.f;
-#pragma unroll
-      for (int c = 0; c < NG; ++c) G[c][e] = 0.f;
-    }
+    zero_partials(G, gLn);
     const int bar_id = 1 + cw;
     float* mail = sMail + cw * 4 * MW;
     float* dbpm = sDbp + cw * 4 * S;
@@ -142,8 +87,7 @@ pre_bwd_wide_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16*
     uint32_t phase = 0;
     int pend = -1;
     for (int k = 0, m = blockIdx.x + cw * gridDim.x; m < M; ++k, m += NC * gridDim.x) {
-      mbar_wait(&my_full[ls], phase);
-      const unsigned char* st = my_ring + (size_t)ls * stage_b;
+      const unsigned char* st = wait_stage(my_full, my_ring, ls, phase, stage_b);
       const float* a = reinterpret_cast<const float*>(st);
       const float mean = a[AUX - 2], rstd = a[AUX - 1], nmr = -mean * rstd;
       float alpha0[S];
@@ -244,11 +188,8 @@ pre_bwd_wide_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16*
         }
       }
       named_bar_sync(bar_id, 128);
-      if (k > 0 && w == 3) {  // every thread is past token k - 1: its stage takes token k - 1 + NSC_W
-        fence_proxy_async_smem();
-        fill(k - 1 + NSC_W);
-      }
-      auto total = [&](int i) { return (mail[i] + mail[MW + i]) + (mail[2 * MW + i] + mail[3 * MW + i]); };
+      refill<NSC_W>(k, w, fill);
+      auto total = [&](int i) { return mail_total<MW>(mail, i); };
       const float m1 = total(0) * inv_d, m2 = total(1) * inv_d;
       // ---------------- per-token scalars (warp 0) ----------------
       if (w == 0) {
@@ -394,10 +335,7 @@ pre_bwd_wide_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16*
         }
       }
       if (!EXPAND) pend = m;
-      if (++ls == NSC_W) {
-        ls = 0;
-        phase ^= 1;
-      }
+      advance<NSC_W>(ls, phase);
     }
     named_bar_sync(bar_id, 128);
     if (w == 0) {
@@ -426,38 +364,10 @@ pre_bwd_wide_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16*
     }
     // per-channel partials of each warpgroup -> the ring, idle once every stage has been consumed: [NC][NP][d]
     __syncthreads();
-    if (act) {
-      float* buf = reinterpret_cast<float*>(ring) + (size_t)cw * NP * d + lt * 8;
-#pragma unroll
-      for (int c = 0; c < NG; ++c) {
-        *reinterpret_cast<float4*>(buf + c * d) = make_float4(G[c][0], G[c][1], G[c][2], G[c][3]);
-        *reinterpret_cast<float4*>(buf + c * d + 4) = make_float4(G[c][4], G[c][5], G[c][6], G[c][7]);
-      }
-      *reinterpret_cast<float4*>(buf + NG * d) = make_float4(gLn[0], gLn[1], gLn[2], gLn[3]);
-      *reinterpret_cast<float4*>(buf + NG * d + 4) = make_float4(gLn[4], gLn[5], gLn[6], gLn[7]);
-    }
+    if (act) store_partials<S>(ring, G, gLn, cw, lt, d);
   }
   __syncthreads();
-  const float* buf = reinterpret_cast<const float*>(ring);
-  for (int i = threadIdx.x; i < d; i += blockDim.x) {
-    float g[NP];
-#pragma unroll
-    for (int k = 0; k < NP; ++k) {
-      g[k] = 0.f;
-#pragma unroll
-      for (int c = 0; c < NC; ++c) g[k] += buf[(size_t)(c * NP + k) * d + i];
-    }
-    const float g1 = (prm.gamma_hc[i] + 1.f) * sqrt_d;
-    float acc = g[T] * prm.dyn_beta[i];
-    atomicAdd(gr.dyn_beta + i, g1 * g[T]);
-#pragma unroll
-    for (int t = 0; t < T; ++t) {
-      acc = fmaf(g[t], prm.dyn_alpha[(size_t)i * T + t], acc);
-      atomicAdd(gr.dyn_alpha + (size_t)i * T + t, g1 * g[t]);
-    }
-    atomicAdd(gr.gamma_hc + i, sqrt_d * acc);
-    atomicAdd(gr.ln_gamma + i, g[NG]);
-  }
+  flush_param_grads<S>(ring, prm, gr, d, sqrt_d);
 }
 
 }  // namespace hcr

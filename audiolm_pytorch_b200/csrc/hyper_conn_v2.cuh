@@ -78,10 +78,16 @@ __device__ __forceinline__ float tanh_fast(float x) {
 }
 
 struct Params {
-  const float* gamma_hc; const float* dyn_alpha; const float* dyn_beta; const float* static_alpha;
-  const float* static_beta; const float* alpha_scale; const float* beta_scale; const float* ln_gamma;
+  const float* gamma_hc;      // [d]      RMSNorm gain (applied as gamma + 1)
+  const float* dyn_alpha;     // [d, S+1]
+  const float* dyn_beta;      // [d]
+  const float* static_alpha;  // [S, S+1]
+  const float* static_beta;   // [S]
+  const float* alpha_scale;   // scalar
+  const float* beta_scale;    // scalar
+  const float* ln_gamma;      // [d] LayerNorm gain of the branch's pre-norm
 };
-struct Grads {
+struct Grads {  // fp32 accumulators (atomicAdd), same shapes as Params
   float* gamma_hc; float* dyn_alpha; float* dyn_beta; float* static_alpha; float* static_beta;
   float* alpha_scale; float* beta_scale; float* ln_gamma;
 };
@@ -221,7 +227,7 @@ pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
       for (int t = 0; t < T; ++t) w[s * T + t] *= inv[s];
       w[S * T + s] *= inv[s];
     }
-    if (lt == 0) {  // pre-activations: the backward's RMS-norm term needs them (hyper_conn_v3.cuh)
+    if (lt == 0) {  // pre-activations: the ring backward's RMS-norm term needs them (hyper_conn_ring.cuh)
       float* az = aux + (size_t)m * AUX + z_offset(S);
 #pragma unroll
       for (int i = 0; i < S * T + S; ++i) az[i] = w[i];
