@@ -33,6 +33,13 @@ SIGNATURES: dict[str, list] = {
     "alm_embed_scatter": [P, I, P, P, I, I, P],
     "alm_attn_delta": [P, L, P, L, P, L, P, I, I, I, P],
     "alm_kv_append": [P, L, P, P, L, P, I, I, P],
+    # the same calls with the head width (dim_head in {32, 64, 128}) as the last argument before the stream
+    "alm_mqa_attn_fwd_dh": [P, L, P, L, L, P, L, L, P, P, L, P, L, P, L, L, I, I, I, I, I, F, *DROP, I, P],
+    "alm_mqa_attn_bwd_dh": [P, L, P, L, L, P, L, L, P, L, P, P, P, I, P, L, P, P, L, P, L, P, P, L, L, I, I, I, I, I, F,
+                            *DROP, I, P],
+    "alm_attn_delta_dh": [P, L, P, L, P, L, P, I, I, I, I, P],
+    "alm_kv_append_dh": [P, L, P, P, L, P, I, I, I, P],
+    "alm_mqa_attn_decode_dh": [P, L, P, P, L, P, I, P, L, P, L, P, L, P, I, I, I, F, I, P],
     "alm_gemv_bf16": [P, L, P, L, P, I, L, P, I, I, I, P],
     "alm_gemm_head_ce": [P, L, P, L, P, P, L, I, P, P, P, P, P, P, L, I, I, I, P],
     "alm_ce_finish": [P, I, P, P, L, P, P, I, P],
@@ -103,6 +110,8 @@ def load() -> C.CDLL:
     lib.alm_decode_stack_grid.argtypes = []
     lib.alm_decode_stack_plan.restype = I
     lib.alm_decode_stack_plan.argtypes = [I, I, I, I, I, P]
+    lib.alm_decode_stack_plan_dh.restype = I
+    lib.alm_decode_stack_plan_dh.argtypes = [I, I, I, I, I, I, P]
     lib.alm_decode_stack_trace_offset.restype = L
     lib.alm_decode_stack_trace_offset.argtypes = [I, I, I, I]
     for name, argtypes in SIGNATURES.items():

@@ -45,10 +45,10 @@ inline int num_sms() {
   return n;
 }
 
-// Build a (up to) 3-D bf16/fp32 tiled tensor map with 128-B swizzle. dims/strides innermost first;
-// strides in BYTES for dims 1.. (dim 0 is contiguous). Returns ALM_OK or an error code.
+// Build a (up to) 3-D bf16/fp32 tiled tensor map. dims/strides innermost first; strides in BYTES for dims 1..
+// (dim 0 is contiguous); swizzle_bytes is 128, 64 or 0 (none). Returns ALM_OK or an error code.
 int make_tensor_map(CUtensorMap* out, const void* base, int elem_bytes, int rank, const uint64_t* dims,
-                    const uint64_t* strides_bytes, const uint32_t* box, bool swizzle128);
+                    const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes);
 
 template <typename T>
 __host__ __device__ constexpr T ceil_div(T a, T b) {

@@ -1,8 +1,10 @@
 // Multi-query causal attention forward for sm_90a (replaces attend.py:69-146 as called from
 // audiolm_pytorch.py:390): softmax(q k^T * d^-1/2, masked by key-padding mask and right-aligned causal
-// mask) v, with ONE shared k/v head of width 64 for all query heads.
+// mask) v, with ONE shared k/v head of width D = 32, 64 or 128 (a template parameter) for all query heads.
 //
-// One CTA = (batch b, head h, 128 queries).  Q/K/V tiles arrive by TMA into 128-B-swizzled smem; each of the two
+// One CTA = (batch b, head h, 128 queries).  Q/K/V tiles arrive by TMA into swizzled smem (SwizzledTile<D>: one
+// 128-B-swizzled [128 x 64] tile at D = 64, two of them side by side at D = 128, one 64-B-swizzled [128 x 32] tile at
+// D = 32); each of the two
 // consumer warpgroups owns 64 query rows: S = Q K^T is a wgmma with both operands in smem, the online (flash)
 // softmax runs on the S accumulator fragment in registers, and P V is a wgmma whose A operand (P, bf16) is taken
 // straight from those registers, accumulating O in registers.
@@ -11,6 +13,9 @@
 // tiles that lie fully below the causal diagonal take a predicate-free path.
 // With DROPOUT, P is multiplied by the keep mask (alm_common.cuh: dropout_keep) times 1/(1-p) when it is packed into
 // the A operand of P V; the row max, the row sum and the stored LSE use the un-dropped P.
+// D = 128 holds 64 O accumulators beside the 64 scores of a tile, more than the 168 registers a 384-thread CTA gives
+// every thread: there the producer warpgroup hands registers to the consumers (setmaxnreg 40 / 232), and the K/V ring
+// has 3 stages instead of 4 (Q + 3 x (K + V) = 224 KB).
 #include "alm_common.cuh"
 #include "ptx_sm90.cuh"
 
@@ -18,14 +23,17 @@ namespace alm {
 
 constexpr int ATT_BM = 128;     // queries per CTA
 constexpr int ATT_BN = 128;     // keys per tile
-constexpr int ATT_D = 64;       // head width (dim_head)
-constexpr int ATT_KV_STAGES = 4;
 constexpr int ATT_THREADS = 384;
-constexpr int ATT_TILE_BYTES = 128 * 64 * 2;  // 16 KB: one [128 x 64] bf16 SW128 tile
-constexpr int ATT_SMEM_BYTES = ATT_TILE_BYTES * (1 + 2 * ATT_KV_STAGES) + 256;
+template <int D>                // D = head width (dim_head)
+struct AttFwdCfg {
+  static constexpr int KV_STAGES = D == 128 ? 3 : 4;
+  static constexpr int HALF_BYTES = 128 * SwizzledTile<D>::ROW_BYTES;  // one swizzled [128 x min(D, 64)] half
+  static constexpr int TILE_BYTES = 128 * D * 2;                       // 16 KB at D = 64
+  static constexpr int SMEM_BYTES = TILE_BYTES * (1 + 2 * KV_STAGES) + 256;
+};
 
 struct AttnFwdParams {
-  __nv_bfloat16* o;       // [b, n_q, h*64] row stride ldo
+  __nv_bfloat16* o;       // [b, n_q, h*D] row stride ldo
   float* lse;             // [b, h, lse_stride] log2-domain LSE of the scaled scores (for backward); may be null
   const uint32_t* kmask;  // packed key mask (alm_pack_key_mask): bit i of word w of row b = key 32 w + i may be attended; may be null
   int kb_stride;          // words per batch row: 4 * ceil(n_k / 128)
@@ -72,10 +80,14 @@ __device__ __forceinline__ uint64_t attn_fwd_keep_bits(const DropoutArgs& d, uin
   return bits;
 }
 
-template <bool HAS_BIAS, bool DROPOUT>
+template <int ATT_D, bool HAS_BIAS, bool DROPOUT>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const AttnFwdParams p) {
+  using Tile = SwizzledTile<ATT_D>;
+  using Cfg = AttFwdCfg<ATT_D>;
+  constexpr int ATT_KV_STAGES = Cfg::KV_STAGES, ATT_TILE_BYTES = Cfg::TILE_BYTES, HALF = Cfg::HALF_BYTES;
+  constexpr bool REG_HANDOFF = ATT_D == 128;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw;
   if ((smem_u32(smem) & 1023u) != 0) __trap();  // SW128 tiles need 1024-B alignment
@@ -114,11 +126,14 @@ mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
   __syncthreads();
 
   if (wg == 0) {
+    if constexpr (REG_HANDOFF) setmaxnreg_dec<40>();
     if (warp == 0 && n_tiles > 0) {
       // ---------------- TMA producer (whole warp runs the loop, one elected lane issues) -------
       if (elect_one_sync()) {
         mbar_arrive_expect_tx(q_full, ATT_TILE_BYTES);
-        tma_load_3d(sQ, &tmQ, q_full, head * ATT_D, q0, batch);
+#pragma unroll
+        for (int hf = 0; hf < Tile::HALVES; ++hf)
+          tma_load_3d(sQ + hf * HALF, &tmQ, q_full, head * ATT_D + hf * Tile::HW, q0, batch);
       }
       __syncwarp();
       int stage = 0;
@@ -127,8 +142,11 @@ mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
         mbar_wait(&kv_empty[stage], phase ^ 1u);
         if (elect_one_sync()) {
           mbar_arrive_expect_tx(&kv_full[stage], 2 * ATT_TILE_BYTES);
-          tma_load_3d(sK + stage * ATT_TILE_BYTES, &tmK, &kv_full[stage], 0, j * ATT_BN, batch);
-          tma_load_3d(sV + stage * ATT_TILE_BYTES, &tmV, &kv_full[stage], 0, j * ATT_BN, batch);
+#pragma unroll
+          for (int hf = 0; hf < Tile::HALVES; ++hf) {
+            tma_load_3d(sK + stage * ATT_TILE_BYTES + hf * HALF, &tmK, &kv_full[stage], hf * Tile::HW, j * ATT_BN, batch);
+            tma_load_3d(sV + stage * ATT_TILE_BYTES + hf * HALF, &tmV, &kv_full[stage], hf * Tile::HW, j * ATT_BN, batch);
+          }
         }
         __syncwarp();
         if (++stage == ATT_KV_STAGES) { stage = 0; phase ^= 1u; }
@@ -139,6 +157,7 @@ mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
 
   // ---------------- consumers: warpgroup cw owns query rows [64 cw, 64 cw + 64) ----------------
   // fragment: this thread holds rows r_base + 8 h (h = 0, 1) and, of every 8-column group j, columns 8 j + c_lane + {0, 1}
+  if constexpr (REG_HANDOFF) setmaxnreg_inc<232>();
   const int cw = wg - 1;
   const int r_base = cw * 64 + (warp & 3) * 16 + (lane >> 2);
   const int c_lane = 2 * (lane & 3);
@@ -157,7 +176,7 @@ mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     if constexpr (HAS_BIAS) brow[h] = p.bias + (long long)head * p.bias_hs + (long long)min(qi, p.n_q - 1) * p.bias_rs;
   }
   const uint32_t* mrow = p.kmask ? p.kmask + (long long)batch * p.kb_stride : nullptr;
-  const uint32_t q_addr = smem_u32(sQ) + cw * 8192;
+  const uint32_t q_addr = smem_u32(sQ) + cw * 64 * Tile::ROW_BYTES;
   [[maybe_unused]] const uint32_t drop_row =
       p.drop_row0 + ((uint32_t)batch * p.h + head) * (uint32_t)p.n_q_pad + q0 + r_base;
 
@@ -172,8 +191,7 @@ mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < ATT_D / 16; ++k)
-      wgmma_ss<ATT_BN>(s, wgmma_desc_sw128(q_addr + k * 32, 1024, 16), wgmma_desc_sw128(k_addr + k * 32, 1024, 16),
-                       k > 0 ? 1u : 0u);
+      wgmma_ss<ATT_BN>(s, Tile::kmajor(q_addr, k, HALF), Tile::kmajor(k_addr, k, HALF), k > 0 ? 1u : 0u);
     wgmma_commit();
     [[maybe_unused]] uint64_t keep = 0;  // drawn while S = Q K^T runs
     if constexpr (DROPOUT) keep = attn_fwd_keep_bits(p.drop, drop_row, j * ATT_BN, c_lane);
@@ -243,12 +261,12 @@ mqa_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_consta
       pa[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
       pa[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
     }
-    // O += P V (V is the MN-major B operand: [keys][64 dims])
+    // O += P V (V is the MN-major B operand: [keys][D dims])
     wgmma_fence_acc(o_acc);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < ATT_BN / 16; ++kk)
-      wgmma_rs<ATT_D, 1>(o_acc, pa[kk], wgmma_desc_sw128(v_addr + kk * 2048, 1024, 8192), 1u);
+      wgmma_rs<ATT_D, 1>(o_acc, pa[kk], Tile::mnmajor(v_addr, kk, HALF), 1u);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_acc(o_acc);
@@ -308,13 +326,82 @@ extern "C" int alm_pack_key_mask(const void* key_mask, void* bits, int b, int n_
   return ALM_OK;
 }
 
-extern "C" int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int64_t k_bstride,
-                                const void* v, int64_t ldv, int64_t v_bstride, const void* key_mask, void* o,
-                                int64_t ldo, float* lse, int64_t lse_stride, const float* bias, int64_t bias_hstride,
-                                int64_t bias_rstride, int b, int h, int n_q, int n_k, int causal, float scale,
-                                float dropout_p, uint64_t seed, uint32_t site, alm_stream_t stream_) {
+namespace alm {
+// the four instantiations of one head width: attribute set-up once, then the launch over batch chunks
+template <int D>
+static int attn_fwd_launch(const void* q, int64_t ldq, const void* k, int64_t ldk, int64_t k_bstride, const void* v,
+                           int64_t ldv, int64_t v_bstride, const void* key_mask, void* o, int64_t ldo, float* lse,
+                           const float* bias, int b, bool drop, AttnFwdParams p, cudaStream_t stream) {
+  using Tile = SwizzledTile<D>;
+  constexpr int SMEM = AttFwdCfg<D>::SMEM_BYTES;
+  const int h = p.h, n_q = p.n_q, n_k = p.n_k;
+  static bool attr_set = false;
+  if (!attr_set) {
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<D, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<D, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<D, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<D, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    attr_set = true;
+  }
+  // Batch is grid.z, which stops at 65535, so larger batches (the local attention passes batch x heads x windows)
+  // run as consecutive launches over chunks of batch rows: operands, outputs and the key mask are offset here, the
+  // dropout counter rows by p.drop_row0.  The (qblock, head, batch) order of each launch is unchanged.
+  constexpr int kMaxGridZ = 65535;
+  const int n_launch = ceil_div(b, kMaxGridZ);
+  for (int b0 = 0; b0 < b; b0 += kMaxGridZ) {
+    const int nb = min(b - b0, kMaxGridZ);
+    CUtensorMap tmQ, tmK, tmV;
+    {
+      uint64_t dims[3] = {(uint64_t)h * D, (uint64_t)n_q, (uint64_t)nb};
+      uint64_t strides[3] = {2, (uint64_t)ldq * 2, (uint64_t)n_q * ldq * 2};
+      uint32_t box[3] = {Tile::HW, ATT_BM, 1};
+      int rc = make_tensor_map(&tmQ, reinterpret_cast<const __nv_bfloat16*>(q) + (long long)b0 * n_q * ldq, 2, 3, dims,
+                               strides, box, Tile::SWIZZLE);
+      if (rc != ALM_OK) return rc;
+    }
+    {
+      uint64_t dims[3] = {(uint64_t)D, (uint64_t)n_k, (uint64_t)nb};
+      uint64_t strides[3] = {2, (uint64_t)ldk * 2, (uint64_t)k_bstride * 2};
+      uint32_t box[3] = {Tile::HW, ATT_BN, 1};
+      int rc = make_tensor_map(&tmK, reinterpret_cast<const __nv_bfloat16*>(k) + (long long)b0 * k_bstride, 2, 3, dims,
+                               strides, box, Tile::SWIZZLE);
+      if (rc != ALM_OK) return rc;
+      strides[1] = (uint64_t)ldv * 2;
+      strides[2] = (uint64_t)v_bstride * 2;
+      rc = make_tensor_map(&tmV, reinterpret_cast<const __nv_bfloat16*>(v) + (long long)b0 * v_bstride, 2, 3, dims,
+                           strides, box, Tile::SWIZZLE);
+      if (rc != ALM_OK) return rc;
+    }
+    p.o = reinterpret_cast<__nv_bfloat16*>(o) + (long long)b0 * n_q * ldo;
+    p.lse = lse != nullptr ? lse + (long long)b0 * h * p.lse_stride : nullptr;
+    p.kmask = key_mask != nullptr ? reinterpret_cast<const uint32_t*>(key_mask) + (long long)b0 * p.kb_stride : nullptr;
+    p.b = nb;
+    p.drop_row0 = (uint32_t)((long long)b0 * h * p.n_q_pad);
+    const dim3 grid((n_q + ATT_BM - 1) / ATT_BM, h, nb);
+    if (bias != nullptr && drop)
+      mqa_attn_fwd_kernel<D, true, true><<<grid, ATT_THREADS, SMEM, stream>>>(tmQ, tmK, tmV, p);
+    else if (bias != nullptr)
+      mqa_attn_fwd_kernel<D, true, false><<<grid, ATT_THREADS, SMEM, stream>>>(tmQ, tmK, tmV, p);
+    else if (drop)
+      mqa_attn_fwd_kernel<D, false, true><<<grid, ATT_THREADS, SMEM, stream>>>(tmQ, tmK, tmV, p);
+    else
+      mqa_attn_fwd_kernel<D, false, false><<<grid, ATT_THREADS, SMEM, stream>>>(tmQ, tmK, tmV, p);
+    ALM_CHECK_LAUNCH();
+  }
+  ALM_LAUNCHED(n_launch);
+  return ALM_OK;
+}
+}  // namespace alm
+
+extern "C" int alm_mqa_attn_fwd_dh(const void* q, int64_t ldq, const void* k, int64_t ldk, int64_t k_bstride,
+                                   const void* v, int64_t ldv, int64_t v_bstride, const void* key_mask, void* o,
+                                   int64_t ldo, float* lse, int64_t lse_stride, const float* bias,
+                                   int64_t bias_hstride, int64_t bias_rstride, int b, int h, int n_q, int n_k,
+                                   int causal, float scale, float dropout_p, uint64_t seed, uint32_t site,
+                                   int dim_head, alm_stream_t stream_) {
   using namespace alm;
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ALM_REQUIRE(dim_head == 32 || dim_head == 64 || dim_head == 128, ALM_ERR_UNSUPPORTED);
   ALM_REQUIRE(q && k && v && o, ALM_ERR_ARG);
   ALM_REQUIRE(b > 0 && h > 0 && n_q > 0 && n_k > 0 && n_k >= n_q, ALM_ERR_ARG);
   ALM_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, ALM_ERR_ARG);
@@ -339,64 +426,21 @@ extern "C" int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64
   p.scale_log2 = scale * 1.4426950408889634f;
   p.n_q_pad = (n_q + 127) / 128 * 128;
   p.drop = make_dropout_args(dropout_p, seed, site);
-  static bool attr_set = false;
-  if (!attr_set) {
-    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     ATT_SMEM_BYTES));
-    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     ATT_SMEM_BYTES));
-    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     ATT_SMEM_BYTES));
-    ALM_CUDA_OK(cudaFuncSetAttribute(mqa_attn_fwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     ATT_SMEM_BYTES));
-    attr_set = true;
-  }
   const bool drop = dropout_p > 0.f;
-  // Batch is grid.z, which stops at 65535, so larger batches (the local attention passes batch x heads x windows)
-  // run as consecutive launches over chunks of batch rows: operands, outputs and the key mask are offset here, the
-  // dropout counter rows by p.drop_row0.  The (qblock, head, batch) order of each launch is unchanged.
-  constexpr int kMaxGridZ = 65535;
-  const int n_launch = ceil_div(b, kMaxGridZ);
-  for (int b0 = 0; b0 < b; b0 += kMaxGridZ) {
-    const int nb = min(b - b0, kMaxGridZ);
-    CUtensorMap tmQ, tmK, tmV;
-    {
-      uint64_t dims[3] = {(uint64_t)h * ATT_D, (uint64_t)n_q, (uint64_t)nb};
-      uint64_t strides[3] = {2, (uint64_t)ldq * 2, (uint64_t)n_q * ldq * 2};
-      uint32_t box[3] = {ATT_D, ATT_BM, 1};
-      int rc = make_tensor_map(&tmQ, reinterpret_cast<const __nv_bfloat16*>(q) + (long long)b0 * n_q * ldq, 2, 3, dims,
-                               strides, box, true);
-      if (rc != ALM_OK) return rc;
-    }
-    {
-      uint64_t dims[3] = {(uint64_t)ATT_D, (uint64_t)n_k, (uint64_t)nb};
-      uint64_t strides[3] = {2, (uint64_t)ldk * 2, (uint64_t)k_bstride * 2};
-      uint32_t box[3] = {ATT_D, ATT_BN, 1};
-      int rc = make_tensor_map(&tmK, reinterpret_cast<const __nv_bfloat16*>(k) + (long long)b0 * k_bstride, 2, 3, dims,
-                               strides, box, true);
-      if (rc != ALM_OK) return rc;
-      strides[1] = (uint64_t)ldv * 2;
-      strides[2] = (uint64_t)v_bstride * 2;
-      rc = make_tensor_map(&tmV, reinterpret_cast<const __nv_bfloat16*>(v) + (long long)b0 * v_bstride, 2, 3, dims,
-                           strides, box, true);
-      if (rc != ALM_OK) return rc;
-    }
-    p.o = reinterpret_cast<__nv_bfloat16*>(o) + (long long)b0 * n_q * ldo;
-    p.lse = lse != nullptr ? lse + (long long)b0 * h * lse_stride : nullptr;
-    p.kmask = key_mask != nullptr ? reinterpret_cast<const uint32_t*>(key_mask) + (long long)b0 * p.kb_stride : nullptr;
-    p.b = nb;
-    p.drop_row0 = (uint32_t)((long long)b0 * h * p.n_q_pad);
-    const dim3 grid((n_q + ATT_BM - 1) / ATT_BM, h, nb);
-    if (bias != nullptr && drop)
-      mqa_attn_fwd_kernel<true, true><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
-    else if (bias != nullptr)
-      mqa_attn_fwd_kernel<true, false><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
-    else if (drop)
-      mqa_attn_fwd_kernel<false, true><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
-    else
-      mqa_attn_fwd_kernel<false, false><<<grid, ATT_THREADS, ATT_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, p);
-    ALM_CHECK_LAUNCH();
-  }
-  ALM_LAUNCHED(n_launch);
-  return ALM_OK;
+#define ALM_ATT_FWD(DD) \
+  attn_fwd_launch<DD>(q, ldq, k, ldk, k_bstride, v, ldv, v_bstride, key_mask, o, ldo, lse, bias, b, drop, p, stream)
+  if (dim_head == 32) return ALM_ATT_FWD(32);
+  if (dim_head == 64) return ALM_ATT_FWD(64);
+  return ALM_ATT_FWD(128);
+#undef ALM_ATT_FWD
+}
+
+extern "C" int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int64_t k_bstride,
+                                const void* v, int64_t ldv, int64_t v_bstride, const void* key_mask, void* o,
+                                int64_t ldo, float* lse, int64_t lse_stride, const float* bias, int64_t bias_hstride,
+                                int64_t bias_rstride, int b, int h, int n_q, int n_k, int causal, float scale,
+                                float dropout_p, uint64_t seed, uint32_t site, alm_stream_t stream_) {
+  return alm_mqa_attn_fwd_dh(q, ldq, k, ldk, k_bstride, v, ldv, v_bstride, key_mask, o, ldo, lse, lse_stride, bias,
+                             bias_hstride, bias_rstride, b, h, n_q, n_k, causal, scale, dropout_p, seed, site, 64,
+                             stream_);
 }

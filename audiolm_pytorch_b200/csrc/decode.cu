@@ -3,21 +3,21 @@
 // (config C5: AudioLM.generate with use_kv_cache, audiolm_pytorch.py:1406-1511, 1608-1740, 1896-2039; the
 // reference re-concatenates the cache with torch.cat per layer per step, :363-365).
 //
-//   alm_kv_append        : k_cache[b, *len, :] = kv_new[b, 0:64], v_cache[b, *len, :] = kv_new[b, 64:128]
+//   alm_kv_append        : k_cache[b, *len, :] = kv_new[b, 0:D], v_cache[b, *len, :] = kv_new[b, D:2D]  (D = dim_head)
 //   alm_mqa_attn_decode  : o[b, h, :] = softmax_j<=*len( q[b,h,:] . k_cache[b,j,:] * scale (+ bias[h, j]) ) v_cache[b,j,:]
 //   alm_decode_bias_row  : bias[h, j] for the new token at position *len (relative-position / cross / fine 2-D bias)
 // All three read the cache length from `len` at run time, so the launch parameters never change between steps.
 // One warp per (batch, head): lanes stride over the keys with a private online softmax (fp32), then the 32
 // partial states are merged with shuffles.  K/V rows are shared by all heads (MQA) and stay in L1/L2.
+// The head width D (32, 64 or 128) is a template parameter of the attention kernels; at D = 128 the scaled query sits in
+// shared memory (every lane reads the same element: a broadcast) so that the 128 accumulators stay in registers.
 #include "alm_common.cuh"
 
 namespace alm {
 
-constexpr int DEC_D = 64;
-
 __global__ void kv_append_kernel(const __nv_bfloat16* __restrict__ kv_new, long long ld, __nv_bfloat16* __restrict__ kc,
                                  __nv_bfloat16* __restrict__ vc, long long cache_bstride, const int* __restrict__ len,
-                                 int max_len, int b) {
+                                 int max_len, int b, int DEC_D) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= b * 2 * DEC_D) return;
   const int pos = *len;
@@ -30,7 +30,7 @@ __global__ void kv_append_kernel(const __nv_bfloat16* __restrict__ kv_new, long 
 
 // HAS_BIAS: an additive fp32 score bias, one row per head (bias[head * bias_ld + j]) shared by every sequence of the
 // batch; the scores are in log2 units (q carries scale * log2 e), so the bias enters as bias * log2 e.
-template <bool HAS_BIAS>
+template <int DEC_D, bool HAS_BIAS>
 __global__ void __launch_bounds__(256)
 mqa_attn_decode_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const __nv_bfloat16* __restrict__ kc,
                        const __nv_bfloat16* __restrict__ vc, long long cache_bstride, const int* __restrict__ len,
@@ -38,7 +38,7 @@ mqa_attn_decode_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const
                        const float* __restrict__ bias, long long bias_ld, __nv_bfloat16* __restrict__ o, long long ldo,
                        float* __restrict__ partial, int h, float scale_log2) {
   // grid (b, splits): each CTA covers one contiguous slice of the keys (flash-decoding); with splits > 1 the
-  // per-slice softmax states go to `partial` [b, splits, h, 66] = {m, l, acc[64]} and a second kernel merges them
+  // per-slice softmax states go to `partial` [b, splits, h, D + 2] = {m, l, acc[D]} and a second kernel merges them
   const int b = blockIdx.x, split = blockIdx.y, splits = gridDim.y;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   const int n_all = min(*len + 1, max_len);  // the new token was appended at position *len
@@ -48,8 +48,12 @@ mqa_attn_decode_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const
   const __nv_bfloat16* kb = kc + (size_t)b * cache_bstride;
   const __nv_bfloat16* vb = vc + (size_t)b * cache_bstride;
   const uint8_t* mrow = key_mask ? key_mask + (size_t)b * mask_bstride : nullptr;
+  constexpr bool Q_SMEM = DEC_D > 64;
+  constexpr int QR = Q_SMEM ? 1 : DEC_D;
+  __shared__ float q_sh[Q_SMEM ? 8 * DEC_D : 1];   // [warp][D]: launches use at most 8 warps
   for (int head = warp; head < h; head += nwarps) {
-    float qv[DEC_D];
+    float qreg[QR];
+    float* qv = Q_SMEM ? q_sh + warp * DEC_D : qreg;
     {
       const uint4* qp = reinterpret_cast<const uint4*>(q + (size_t)b * ldq + head * DEC_D);
 #pragma unroll
@@ -61,6 +65,7 @@ mqa_attn_decode_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const
         qv[i * 8 + 6] = bf16_lo(u.w) * scale_log2; qv[i * 8 + 7] = bf16_hi(u.w) * scale_log2;
       }
     }
+    if constexpr (Q_SMEM) __syncwarp();
     float m = -INFINITY, l = 0.f, acc[DEC_D];
 #pragma unroll
     for (int d = 0; d < DEC_D; ++d) acc[d] = 0.f;
@@ -95,28 +100,38 @@ mqa_attn_decode_kernel(const __nv_bfloat16* __restrict__ q, long long ldq, const
     const float m_all = warp_max(m);
     const float f = (m == -INFINITY) ? 0.f : exp2f(m - m_all);
     const float l_all = warp_sum(l * f);
-    float mine0 = 0.f, mine1 = 0.f;
+    // lane l keeps channels 64 r + 2 l + {0, 1} of every 64-channel group r (lanes 16.. hold nothing at D = 32)
+    constexpr int GROUPS = (DEC_D + 63) / 64;
+    float mine0[GROUPS], mine1[GROUPS];
+#pragma unroll
+    for (int r = 0; r < GROUPS; ++r) mine0[r] = mine1[r] = 0.f;
 #pragma unroll
     for (int d = 0; d < DEC_D; ++d) {
       const float t = warp_sum(acc[d] * f);
-      if ((d >> 1) == lane) { if (d & 1) mine1 = t; else mine0 = t; }
+      if (((d & 63) >> 1) == lane) { if (d & 1) mine1[d >> 6] = t; else mine0[d >> 6] = t; }
     }
+    const bool owner = 2 * lane < DEC_D;
     if (partial != nullptr) {
       float* ps = partial + (((size_t)b * splits + split) * h + head) * (DEC_D + 2);
       if (lane == 0) { ps[0] = m_all; ps[1] = l_all; }
-      ps[2 + 2 * lane] = mine0;
-      ps[3 + 2 * lane] = mine1;
+#pragma unroll
+      for (int r = 0; r < GROUPS; ++r)
+        if (owner) { ps[2 + 64 * r + 2 * lane] = mine0[r]; ps[3 + 64 * r + 2 * lane] = mine1[r]; }
     } else {
       const float inv = l_all > 0.f ? 1.f / l_all : 0.f;  // fully masked row -> zeros (as alm_mqa_attn_fwd)
-      __nv_bfloat162 out2 = __floats2bfloat162_rn(mine0 * inv, mine1 * inv);
-      *reinterpret_cast<__nv_bfloat162*>(o + (size_t)b * ldo + head * DEC_D + 2 * lane) = out2;
+#pragma unroll
+      for (int r = 0; r < GROUPS; ++r)
+        if (owner)
+          *reinterpret_cast<__nv_bfloat162*>(o + (size_t)b * ldo + head * DEC_D + 64 * r + 2 * lane) =
+              __floats2bfloat162_rn(mine0[r] * inv, mine1[r] * inv);
     }
+    if constexpr (Q_SMEM) __syncwarp();  // the next head of this warp overwrites its q_sh row
   }
 }
 
 // o[b, head, :] = sum_s acc_s 2^(m_s - m) / sum_s l_s 2^(m_s - m): one thread per (head, channel)
 __global__ void mqa_attn_decode_combine_kernel(const float* __restrict__ partial, __nv_bfloat16* __restrict__ o,
-                                               long long ldo, int h, int splits) {
+                                               long long ldo, int h, int splits, int DEC_D) {
   const int b = blockIdx.x;
   for (int i = threadIdx.x; i < h * DEC_D; i += blockDim.x) {
     const int head = i / DEC_D, d = i % DEC_D;
@@ -216,23 +231,32 @@ gemv_bf16_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, const __nv_
 
 using namespace alm;
 
-extern "C" int alm_kv_append(const void* kv_new, int64_t ld, void* k_cache, void* v_cache, int64_t cache_bstride,
-                             const int32_t* len, int max_len, int b, alm_stream_t stream_) {
+extern "C" int alm_kv_append_dh(const void* kv_new, int64_t ld, void* k_cache, void* v_cache, int64_t cache_bstride,
+                                const int32_t* len, int max_len, int b, int dim_head, alm_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ALM_REQUIRE(dim_head == 32 || dim_head == 64 || dim_head == 128, ALM_ERR_UNSUPPORTED);
   ALM_REQUIRE(kv_new && k_cache && v_cache && len && b > 0 && max_len > 0, ALM_ERR_ARG);
-  const int n = b * 2 * DEC_D;
+  const int n = b * 2 * dim_head;
   kv_append_kernel<<<ceil_div(n, 256), 256, 0, stream>>>((const __nv_bfloat16*)kv_new, ld, (__nv_bfloat16*)k_cache,
-                                                         (__nv_bfloat16*)v_cache, cache_bstride, len, max_len, b);
+                                                         (__nv_bfloat16*)v_cache, cache_bstride, len, max_len, b,
+                                                         dim_head);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);
   return ALM_OK;
 }
 
-extern "C" int alm_mqa_attn_decode(const void* q, int64_t ldq, const void* k_cache, const void* v_cache,
-                                   int64_t cache_bstride, const int32_t* len, int max_len, const void* key_mask,
-                                   int64_t mask_bstride, const float* bias, int64_t bias_ld, void* o, int64_t ldo,
-                                   float* workspace, int splits, int b, int h, float scale, alm_stream_t stream_) {
+extern "C" int alm_kv_append(const void* kv_new, int64_t ld, void* k_cache, void* v_cache, int64_t cache_bstride,
+                             const int32_t* len, int max_len, int b, alm_stream_t stream_) {
+  return alm_kv_append_dh(kv_new, ld, k_cache, v_cache, cache_bstride, len, max_len, b, 64, stream_);
+}
+
+extern "C" int alm_mqa_attn_decode_dh(const void* q, int64_t ldq, const void* k_cache, const void* v_cache,
+                                      int64_t cache_bstride, const int32_t* len, int max_len, const void* key_mask,
+                                      int64_t mask_bstride, const float* bias, int64_t bias_ld, void* o, int64_t ldo,
+                                      float* workspace, int splits, int b, int h, float scale, int dim_head,
+                                      alm_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ALM_REQUIRE(dim_head == 32 || dim_head == 64 || dim_head == 128, ALM_ERR_UNSUPPORTED);
   ALM_REQUIRE(q && k_cache && v_cache && len && o && b > 0 && h > 0 && max_len > 0, ALM_ERR_ARG);
   ALM_REQUIRE(splits >= 1 && splits <= 64 && (splits == 1 || workspace != nullptr), ALM_ERR_ARG);
   ALM_REQUIRE(bias == nullptr || bias_ld >= max_len, ALM_ERR_ARG);
@@ -241,18 +265,28 @@ extern "C" int alm_mqa_attn_decode(const void* q, int64_t ldq, const void* k_cac
                   (reinterpret_cast<uintptr_t>(v_cache) & 15u) == 0, ALM_ERR_ALIGN);
   const int threads = 32 * min(h, 8);
   dim3 grid(b, splits);
-  auto kernel = bias ? mqa_attn_decode_kernel<true> : mqa_attn_decode_kernel<false>;
+  auto kernel = dim_head == 32    ? (bias ? mqa_attn_decode_kernel<32, true> : mqa_attn_decode_kernel<32, false>)
+                : dim_head == 64  ? (bias ? mqa_attn_decode_kernel<64, true> : mqa_attn_decode_kernel<64, false>)
+                                  : (bias ? mqa_attn_decode_kernel<128, true> : mqa_attn_decode_kernel<128, false>);
   kernel<<<grid, threads, 0, stream>>>((const __nv_bfloat16*)q, ldq, (const __nv_bfloat16*)k_cache,
                                        (const __nv_bfloat16*)v_cache, cache_bstride, len, max_len,
                                        (const uint8_t*)key_mask, mask_bstride, bias, bias_ld, (__nv_bfloat16*)o, ldo,
                                        splits > 1 ? workspace : nullptr, h, scale * 1.4426950408889634f);
   ALM_CHECK_LAUNCH();
   if (splits > 1) {
-    mqa_attn_decode_combine_kernel<<<b, 256, 0, stream>>>(workspace, (__nv_bfloat16*)o, ldo, h, splits);
+    mqa_attn_decode_combine_kernel<<<b, 256, 0, stream>>>(workspace, (__nv_bfloat16*)o, ldo, h, splits, dim_head);
     ALM_CHECK_LAUNCH();
   }
   ALM_LAUNCHED(splits > 1 ? 2 : 1);
   return ALM_OK;
+}
+
+extern "C" int alm_mqa_attn_decode(const void* q, int64_t ldq, const void* k_cache, const void* v_cache,
+                                   int64_t cache_bstride, const int32_t* len, int max_len, const void* key_mask,
+                                   int64_t mask_bstride, const float* bias, int64_t bias_ld, void* o, int64_t ldo,
+                                   float* workspace, int splits, int b, int h, float scale, alm_stream_t stream_) {
+  return alm_mqa_attn_decode_dh(q, ldq, k_cache, v_cache, cache_bstride, len, max_len, key_mask, mask_bstride, bias,
+                                bias_ld, o, ldo, workspace, splits, b, h, scale, 64, stream_);
 }
 
 extern "C" int alm_decode_bias_row(const float* table, int rows, const float* override_h, const int32_t* u,

@@ -1020,6 +1020,11 @@ extern "C" int alm_decode_stack_plan(int b, int d, int heads, int inner, int n_l
   return ALM_OK;
 }
 
+extern "C" int alm_decode_stack_plan_dh(int b, int d, int heads, int inner, int n_layers, int dim_head, int32_t* staged) {
+  if (dim_head != dstep::DH) return ALM_ERR_UNSUPPORTED;   // the one-kernel step is built for one head width
+  return alm_decode_stack_plan(b, d, heads, inner, n_layers, staged);
+}
+
 extern "C" int alm_decode_stack_step(const void* layer_table, int n_layers, const float* x, void* out,
                                      const float* final_gamma, int32_t* len, int max_len, int64_t cache_bstride,
                                      const void* key_mask, int64_t mask_bstride, void* scratch, int64_t scratch_bytes,

@@ -342,22 +342,25 @@ ce_fwd_bwd_kernel(const float* __restrict__ logits, long long ldl, const long lo
   }
 }
 
-// ---- delta[b,h,i] = sum_d dO[b,i,h,d] * O[b,i,h,d]   (one warp per (token, head), d = 64) --------
+// ---- delta[b,h,i] = sum_d dO[b,i,h,d] * O[b,i,h,d]   (one warp per (token, head), D = 32 / 64 / 128: lane l takes columns 2 l + {0, 1} of every 64)
 // also zeroes the same (token, head) row of the fp32 dQ workspace of the attention backward (when given)
 __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ o, long long ldo,
                                   const __nv_bfloat16* __restrict__ d_o, long long lddo, float* __restrict__ delta,
-                                  long long dstride, float* __restrict__ dq_acc, int b, int h, int n) {
+                                  long long dstride, float* __restrict__ dq_acc, int b, int h, int n, int D) {
   const int gw = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   const int total = b * n * h;
   if (gw >= total) return;
   const int head = gw % h;
   const int tok = gw / h;  // b*n + i
-  const uint32_t uo = *reinterpret_cast<const uint32_t*>(o + (size_t)tok * ldo + head * 64 + lane * 2);
-  const uint32_t ud = *reinterpret_cast<const uint32_t*>(d_o + (size_t)tok * lddo + head * 64 + lane * 2);
-  float v = bf16_lo(uo) * bf16_lo(ud) + bf16_hi(uo) * bf16_hi(ud);
-  if (dq_acc != nullptr)
-    *reinterpret_cast<float2*>(dq_acc + ((size_t)tok * h + head) * 64 + lane * 2) = make_float2(0.f, 0.f);
+  float v = 0.f;
+  for (int c = lane * 2; c < D; c += 64) {
+    const uint32_t uo = *reinterpret_cast<const uint32_t*>(o + (size_t)tok * ldo + head * D + c);
+    const uint32_t ud = *reinterpret_cast<const uint32_t*>(d_o + (size_t)tok * lddo + head * D + c);
+    v += bf16_lo(uo) * bf16_lo(ud) + bf16_hi(uo) * bf16_hi(ud);
+    if (dq_acc != nullptr)
+      *reinterpret_cast<float2*>(dq_acc + ((size_t)tok * h + head) * D + c) = make_float2(0.f, 0.f);
+  }
   v = warp_sum(v);
   if (lane == 0) {
     const int bi = tok / n, i = tok - bi * n;
@@ -703,18 +706,26 @@ extern "C" int alm_ce_fwd_bwd(const float* logits, int64_t ldl, const int64_t* l
   return ALM_OK;
 }
 
-extern "C" int alm_attn_delta(const void* o, int64_t ldo, const void* d_o, int64_t lddo, float* delta,
-                              int64_t delta_stride, float* dq_acc, int b, int h, int n, alm_stream_t stream_) {
+extern "C" int alm_attn_delta_dh(const void* o, int64_t ldo, const void* d_o, int64_t lddo, float* delta,
+                                 int64_t delta_stride, float* dq_acc, int b, int h, int n, int dim_head,
+                                 alm_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ALM_REQUIRE(dim_head == 32 || dim_head == 64 || dim_head == 128, ALM_ERR_UNSUPPORTED);
   ALM_REQUIRE(b > 0 && h > 0 && n > 0, ALM_ERR_ARG);
   const long long warps = (long long)b * h * n;
   const int threads = 256;
   const long long blocks = ceil_div(warps * 32, (long long)threads);
   attn_delta_kernel<<<(unsigned)blocks, threads, 0, stream>>>((const __nv_bfloat16*)o, ldo,
-                                                              (const __nv_bfloat16*)d_o, lddo, delta, delta_stride, dq_acc, b, h, n);
+                                                              (const __nv_bfloat16*)d_o, lddo, delta, delta_stride, dq_acc, b, h, n,
+                                                              dim_head);
   ALM_CHECK_LAUNCH();
   ALM_LAUNCHED(1);
   return ALM_OK;
+}
+
+extern "C" int alm_attn_delta(const void* o, int64_t ldo, const void* d_o, int64_t lddo, float* delta,
+                              int64_t delta_stride, float* dq_acc, int b, int h, int n, alm_stream_t stream_) {
+  return alm_attn_delta_dh(o, ldo, d_o, lddo, delta, delta_stride, dq_acc, b, h, n, 64, stream_);
 }
 
 extern "C" int alm_axpby_bf16(const void* x, int64_t ldx, float alpha, const void* y, int64_t ldy, float beta,

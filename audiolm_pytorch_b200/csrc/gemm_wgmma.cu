@@ -423,7 +423,7 @@ static int gemm_common(const void* A, int a_mn, int64_t lda, int64_t strideA, co
     dims[2] = (uint64_t)batch; box[2] = 1;
     strides[0] = 2; strides[1] = (uint64_t)lda * 2;
     strides[2] = batch > 1 ? (uint64_t)strideA * 2 : dims[1] * strides[1];
-    int rc = make_tensor_map(&tmA, A, 2, 3, dims, strides, box, true);
+    int rc = make_tensor_map(&tmA, A, 2, 3, dims, strides, box, 128);
     if (rc != ALM_OK) return rc;
   }
   {
@@ -439,7 +439,7 @@ static int gemm_common(const void* A, int a_mn, int64_t lda, int64_t strideA, co
     dims[2] = (uint64_t)batch; box[2] = 1;
     strides[0] = 2; strides[1] = (uint64_t)ldb * 2;
     strides[2] = batch > 1 ? (uint64_t)strideB * 2 : dims[1] * strides[1];
-    int rc = make_tensor_map(&tmB, B, 2, 3, dims, strides, box, true);
+    int rc = make_tensor_map(&tmB, B, 2, 3, dims, strides, box, 128);
     if (rc != ALM_OK) return rc;
   }
 
@@ -452,7 +452,7 @@ static int gemm_common(const void* A, int a_mn, int64_t lda, int64_t strideA, co
     const uint64_t dims[3] = {(uint64_t)N, (uint64_t)M, (uint64_t)batch};
     const uint64_t strides[3] = {2, (uint64_t)ldc * 2, batch > 1 ? (uint64_t)strideC * 2 : (uint64_t)M * ldc * 2};
     const uint32_t box[3] = {64, 64, 1};
-    int rc = make_tensor_map(&tmC, C, 2, 3, dims, strides, box, true);
+    int rc = make_tensor_map(&tmC, C, 2, 3, dims, strides, box, 128);
     if (rc != ALM_OK) return rc;
   }
 

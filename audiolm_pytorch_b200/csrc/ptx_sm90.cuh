@@ -149,6 +149,34 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr, uint32_
   uint32_t hi = ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 30);
   return (static_cast<uint64_t>(hi) << 32) | lo;
 }
+// The same with SWIZZLE_64B (layout 2): tile rows of 32 bf16 (64 B), an 8-row group is 512 B (SBO); K-major advance K by
+// 16: +32 B; MN-major atoms are [8 k rows][32 bf16 along MN], advance K by 16: +1024 B.
+__device__ __forceinline__ uint64_t wgmma_desc_sw64(uint32_t smem_addr, uint32_t sbo_bytes, uint32_t lbo_bytes) {
+  uint32_t lo = ((smem_addr >> 4) & 0x3FFFu) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
+  uint32_t hi = ((sbo_bytes >> 4) & 0x3FFFu) | (2u << 30);
+  return (static_cast<uint64_t>(hi) << 32) | lo;
+}
+// A [rows][W] bf16 operand tile as TMA writes it for the attention kernels: W / HW column halves of [rows][HW], HW =
+// min(W, 64), each half swizzled over its own row width (128 B, or 64 B at W = 32) and `half_bytes` apart.
+template <int W>
+struct SwizzledTile {
+  static constexpr int HW = W < 64 ? W : 64;   // columns of one half
+  static constexpr int HALVES = W / HW;
+  static constexpr int ROW_BYTES = HW * 2;
+  static constexpr int SWIZZLE = ROW_BYTES;    // 64 or 128: the TMA swizzle mode and the descriptor layout
+  static_assert(W == 32 || W == 64 || W == 128, "tile widths of the attention kernels");
+  static __device__ __forceinline__ uint64_t desc(uint32_t addr, uint32_t lbo) {
+    return SWIZZLE == 128 ? wgmma_desc_sw128(addr, 8 * ROW_BYTES, lbo) : wgmma_desc_sw64(addr, 8 * ROW_BYTES, lbo);
+  }
+  // K-major (contraction over the W columns): k16 step k of the tile whose first row is at `addr`
+  static __device__ __forceinline__ uint64_t kmajor(uint32_t addr, int k, uint32_t half_bytes) {
+    return desc(addr + (k / (HW / 16)) * half_bytes + (k % (HW / 16)) * 32, 16);
+  }
+  // MN-major (contraction over the rows): k16 step kk = rows [16 kk, 16 kk + 16); N = W spans the halves through LBO
+  static __device__ __forceinline__ uint64_t mnmajor(uint32_t addr, int kk, uint32_t half_bytes) {
+    return desc(addr + kk * 16 * ROW_BYTES, half_bytes);
+  }
+};
 // No-swizzle K-major operand: core matrix = 8 rows x 16 B stored contiguously (128 B); SBO = byte distance between 8-row
 // groups along M/N, LBO = byte distance between the two core matrices of one K=16 step along K.
 // With SBO = 128 every row sits 16 B after the previous one, so the start address may point at ANY row (16-B aligned):
@@ -227,6 +255,23 @@ __device__ __forceinline__ void wgmma_ss_n256(float (&d)[128], uint64_t da, uint
       : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
 }
 
+template <int TB>
+__device__ __forceinline__ void wgmma_rs_n32(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, %22;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate), "n"(TB));
+}
+template <int TB>
+__device__ __forceinline__ void wgmma_rs_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, %70;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate), "n"(TB));
+}
+
 // dispatch on the accumulator width: d holds N / 2 fp32 per thread (the m64nNk16 fragment layout)
 template <int N, int TA = 0, int TB = 0>
 __device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
@@ -237,8 +282,10 @@ __device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t da, uint64_
 }
 template <int N, int TB = 0>
 __device__ __forceinline__ void wgmma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
-  static_assert(N == 64, "the register-A form is only instantiated for N = 64");
-  wgmma_rs_n64<TB>(d, a, db, accumulate);
+  static_assert(N == 32 || N == 64 || N == 128, "the register-A form is instantiated for N = 32, 64 and 128");
+  if constexpr (N == 32) wgmma_rs_n32<TB>(d, a, db, accumulate);
+  else if constexpr (N == 64) wgmma_rs_n64<TB>(d, a, db, accumulate);
+  else wgmma_rs_n128<TB>(d, a, db, accumulate);
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {

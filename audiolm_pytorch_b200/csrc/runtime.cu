@@ -25,7 +25,7 @@ static EncodeTiledFn resolve_encode() {
 }
 
 int make_tensor_map(CUtensorMap* out, const void* base, int elem_bytes, int rank, const uint64_t* dims,
-                    const uint64_t* strides_bytes, const uint32_t* box, bool swizzle128) {
+                    const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes) {
   EncodeTiledFn enc = resolve_encode();
   if (!enc) {
     fprintf(stderr, "[alm] cuTensorMapEncodeTiled unavailable (no CUDA driver?)\n");
@@ -52,9 +52,13 @@ int make_tensor_map(CUtensorMap* out, const void* base, int elem_bytes, int rank
       }
     }
   }
+  if (swizzle_bytes != 0 && swizzle_bytes != 64 && swizzle_bytes != 128) return ALM_ERR_ARG;
+  const CUtensorMapSwizzle swz = swizzle_bytes == 128  ? CU_TENSOR_MAP_SWIZZLE_128B
+                                 : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                                       : CU_TENSOR_MAP_SWIZZLE_NONE;
   CUtensorMapDataType dt = elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   CUresult r = enc(out, dt, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bdim, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     fprintf(stderr, "[alm] cuTensorMapEncodeTiled failed with %d (rank %d dims %llu,%llu,%llu box %u,%u,%u)\n", (int)r,

@@ -8,7 +8,7 @@ than GPU work.  Here one decode step
     embed(last token) -> 6 x [hyper-connection pre, q/kv GEMMs, kv append, decode attention, out GEMM,
                               hyper-connection pre, W1 GEMM, GEGLU+LN, W2 GEMM] -> post + LN -> head -> top-k Gumbel
 
-works on STATIC buffers: the K/V cache is a preallocated [depth, b, max_len, 64] pair whose fill level lives in
+works on STATIC buffers: the K/V cache is a preallocated [depth, b, max_len, dim_head] pair whose fill level lives in
 a device int32 (`alm_kv_append`, `alm_mqa_attn_decode` read it at run time), the token goes in and out through a
 device buffer.  The step is therefore captured ONCE per sampling position class in a CUDA graph and replayed per
 token; the host only replays the graph and polls for EOS.
@@ -43,7 +43,7 @@ class StackDecoder:
     def __init__(self, tr: Transformer, batch: int, max_len: int):
         dev = next(tr.parameters()).device
         self.tr, self.b, self.max_len = tr, batch, max_len
-        self.kc = torch.zeros(tr.depth, batch, max_len, 64, device=dev, dtype=bf16)
+        self.kc = torch.zeros(tr.depth, batch, max_len, tr.dim_head, device=dev, dtype=bf16)
         self.vc = torch.zeros_like(self.kc)
         self.len = torch.zeros(1, device=dev, dtype=torch.int32)
         # key mask (1 = attend): a STATIC buffer so that captured graphs keep pointing at it; all ones by default
@@ -86,12 +86,13 @@ class StackDecoder:
         return self._fused
 
     def fused_ok(self):
-        """the one-kernel step covers the 4-stream stack without an attention bias, at the sizes its kernel takes
-        (ops.decode_stack_plan); everything else runs the multi-kernel step"""
+        """the one-kernel step covers the 4-stream stack of head width 64 without an attention bias, at the sizes its
+        kernel takes (ops.decode_stack_plan); everything else runs the multi-kernel step"""
         tr = self.tr
         return (FUSED_STACK_STEP and self.b <= ops.DECODE_STEP_MAX_ROWS and tr.num_residual_streams == 4
                 and self.bias is None
-                and ops.decode_stack_plan(self.b, tr.dim, tr.heads, tr.layers[0][2].branch.inner, tr.depth) is not None)
+                and ops.decode_stack_plan(self.b, tr.dim, tr.heads, tr.layers[0][2].branch.inner, tr.depth,
+                                          dim_head=tr.dim_head) is not None)
 
     def barrier_timeouts(self) -> int:
         """sticky error flag of the one-kernel step (a device-wide barrier gave up waiting); 0 when healthy"""
@@ -100,7 +101,7 @@ class StackDecoder:
         return int(self._fused[2][256:260].view(torch.int32).item())
 
     def load_cache(self, kv):
-        """kv: [depth, 2, b, n, 64] as returned by Transformer(..., return_kv_cache=True)"""
+        """kv: [depth, 2, b, n, dim_head] as returned by Transformer(..., return_kv_cache=True)"""
         n = kv.shape[-2]
         assert n <= self.max_len and kv.shape[2] == self.b
         self.kc[:, :, :n] = kv[:, 0].to(bf16)
@@ -143,7 +144,7 @@ class StackDecoder:
     def step(self, x):
         """x [b, d] (embedding of the new token) -> normed output [b, d] bf16; appends to the cache, len += 1."""
         tr = self.tr
-        b, d, H = self.b, tr.dim, tr.heads
+        b, d, H, D = self.b, tr.dim, tr.heads, tr.dim_head
         if tr.rel_pos_bias is not None and self.bias is None:
             raise ops._lib.AlmError("this stack has a relative position bias: set it with StackDecoder.set_bias "
                                     "(the models' decode_bias) before decoding")
@@ -175,12 +176,12 @@ class StackDecoder:
             W = tr._weights(i)
             f = ff_hc.branch
             inner, ip = f.inner, _pad8(f.inner)
-            q = mm(xn, W["wq"])                      # [b, H*64]
-            kv = mm(bin_, W["wkv"])                  # [b, 128]
+            q = mm(xn, W["wq"])                      # [b, H*D]
+            kv = mm(bin_, W["wkv"])                  # [b, 2*D]
             if tr.add_value_residual and v_first is not None:
-                ops.axpby(kv[:, 64:], 0.5, v_first, 0.5, out=kv[:, 64:])
+                ops.axpby(kv[:, D:], 0.5, v_first, 0.5, out=kv[:, D:])
             elif tr.add_value_residual:
-                v_first = kv[:, 64:].clone()
+                v_first = kv[:, D:].clone()
             ops.kv_append(kv, self.kc[i], self.vc[i], self.len)
             o = ops.mqa_attn_decode(q, self.kc[i], self.vc[i], self.len, heads=H, key_mask=self.mask, bias=brow)
             Y = mm(o, W["wo"])

@@ -206,26 +206,38 @@ def dropout_(x, p, seed, site):
     return x
 
 
+ATTN_HEAD_WIDTHS = (32, 64, 128)
+
+
+def _head_width(k):
+    """dim_head of an attention call = the width of its shared key head; the kernels are built for three widths"""
+    D = k.shape[-1]
+    if D not in ATTN_HEAD_WIDTHS:
+        raise NotImplementedError(f"the sm_90a attention kernels are built for dim_head in {ATTN_HEAD_WIDTHS}, got {D}")
+    return D
+
+
 def mqa_attn_fwd(q, k, v, *, heads, key_mask=None, causal=True, scale=None, return_lse=True, bias=None,
                  dropout=None):
     """Multi-query attention forward (attend.py:69-146).
 
-    q: [b, n_q, heads*64] bf16 (last dim contiguous; may be a column slice of a wider buffer)
-    k, v: [b, n_k, 64] bf16 (one shared head);  key_mask: [b, n_k] bool/uint8 (True = attend) or None.
+    q: [b, n_q, heads*D] bf16 (last dim contiguous; may be a column slice of a wider buffer)
+    k, v: [b, n_k, D] bf16 (one shared head of width D = dim_head in {32, 64, 128}, read from k);  key_mask: [b, n_k] bool/uint8 (True = attend) or None.
     Queries are right-aligned against keys (query i sees keys <= i + n_k - n_q) when causal.
     bias: optional fp32 [heads, n_q, >=n_k] additive score bias shared by the batch (attend.py:122-124).
     dropout: optional (p, seed, site): dropout on the attention probabilities (attend.py:139-140); the mask element
     of (batch, head, query i, key j) is keep(seed, site, (batch*heads + head) * n_q_pad + i, j), n_q_pad = n_q
-    rounded up to 128.  The returned lse is that of the un-dropped probabilities.
+    rounded up to 128 (the same mask at every D).  The returned lse is that of the un-dropped probabilities.
     Accepted sizes: 1 <= n_q <= n_k and b * heads * n_q_pad < 2**32 (the 32-bit dropout counter), for any batch b:
     the local attention calls this with b = batch * heads * windows, which passes 65535 on long clips.
-    Returns o [b, n_q, heads*64] bf16 and lse [b, heads, n_q] fp32.
+    scale defaults to D ** -0.5.  Returns o [b, n_q, heads*D] bf16 and lse [b, heads, n_q] fp32.
     """
     _check_cuda(q, k, v, bias)
     assert q.dtype == bf16 and k.dtype == bf16 and v.dtype == bf16
     b, n_q, hd = q.shape
     n_k = k.shape[1]
-    assert hd == heads * 64 and k.shape[-1] == 64 and v.shape[-1] == 64, "dim_head must be 64"
+    D = _head_width(k)
+    assert hd == heads * D and v.shape[-1] == D, "q must be [b, n_q, heads * dim_head] and v as wide as k"
     assert q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1
     assert q.stride(0) == n_q * q.stride(1)
     o = torch.empty(b, n_q, hd, device=q.device, dtype=bf16)
@@ -236,23 +248,23 @@ def mqa_attn_fwd(q, k, v, *, heads, key_mask=None, causal=True, scale=None, retu
         assert key_mask.n_k == n_k and key_mask.bits.shape[0] == b
         key_mask = key_mask.bits
     if scale is None:
-        scale = 64 ** -0.5
+        scale = D ** -0.5
     # algorithmic FLOPs: QK^T + PV over the visible (lower-triangle) part only
     vis = (n_q * n_k - n_q * (n_q - 1) / 2) if causal else n_q * n_k
     bhs, brs = _check_bias(bias, heads, n_q, n_k) if bias is not None else (0, 0)
-    with _timed("mqa_attn_fwd_wgmma", 4.0 * b * heads * 64 * vis):
+    with _timed("mqa_attn_fwd_wgmma", 4.0 * b * heads * D * vis):
         _lib.call(
-            "alm_mqa_attn_fwd",
+            "alm_mqa_attn_fwd_dh",
             q, q.stride(1), k, k.stride(1), k.stride(0), v, v.stride(1), v.stride(0), key_mask,
             o, o.stride(1), lse, n_q_pad, bias, bhs, brs, b, heads, n_q, n_k, int(causal), float(scale),
-            *_drop_args(dropout),
+            *_drop_args(dropout), D,
         )
     return o, lse
 
 
 def mqa_attn_bwd(q, k, v, o, d_o, lse, *, heads, key_mask=None, causal=True, scale=None, bias=None, dbias=None,
                  dropout=None):
-    """Backward of mqa_attn_fwd: returns dq [b,n_q,h*64], dk [b,n_k,64], dv [b,n_k,64] (bf16).
+    """Backward of mqa_attn_fwd: returns dq [b,n_q,h*D], dk [b,n_k,D], dv [b,n_k,D] (bf16), D = k.shape[-1].
     dropout: the (p, seed, site) of the forward call; its mask is regenerated.
 
     lse is the padded [b, heads, n_q_pad] tensor returned by the forward.  With a bias, d(bias) is ACCUMULATED
@@ -262,6 +274,8 @@ def mqa_attn_bwd(q, k, v, o, d_o, lse, *, heads, key_mask=None, causal=True, sca
     b, n_q, hd = q.shape
     n_k = k.shape[1]
     n_q_pad = lse.shape[-1]
+    D = _head_width(k)
+    assert hd == heads * D and v.shape[-1] == D
     assert d_o.dtype == bf16 and d_o.stride(-1) == 1 and o.stride(-1) == 1
     assert d_o.stride(0) == n_q * d_o.stride(1)
     key_mask = pack_key_mask(key_mask)
@@ -269,24 +283,24 @@ def mqa_attn_bwd(q, k, v, o, d_o, lse, *, heads, key_mask=None, causal=True, sca
         assert key_mask.n_k == n_k
         key_mask = key_mask.bits
     if scale is None:
-        scale = 64 ** -0.5
+        scale = D ** -0.5
     dq = torch.empty(b, n_q, hd, device=q.device, dtype=bf16)
     delta = torch.empty(b, heads, n_q_pad, device=q.device, dtype=f32)
     dq_acc = torch.empty(b, n_q, hd, device=q.device, dtype=f32)  # fp32 dQ workspace, zeroed by alm_attn_delta
-    dk = torch.empty(b, n_k, 64, device=q.device, dtype=bf16)
-    dv = torch.empty(b, n_k, 64, device=q.device, dtype=bf16)
+    dk = torch.empty(b, n_k, D, device=q.device, dtype=bf16)
+    dv = torch.empty(b, n_k, D, device=q.device, dtype=bf16)
     bhs, brs = _check_bias(bias, heads, n_q, n_k) if bias is not None else (0, 0)
     if dbias is not None:
         assert bias is not None and dbias.dtype == f32 and dbias.shape == bias.shape and dbias.stride() == bias.stride()
     vis = (n_q * n_k - n_q * (n_q - 1) / 2) if causal else n_q * n_k
     # 5 matmuls, each executed once; the timed region also covers delta + workspace zeroing and the dq conversion
-    with _timed("mqa_attn_bwd_wgmma", 10.0 * b * heads * 64 * vis):
-        _lib.call("alm_attn_delta", o, o.stride(1), d_o, d_o.stride(1), delta, n_q_pad, dq_acc, b, heads, n_q)
+    with _timed("mqa_attn_bwd_wgmma", 10.0 * b * heads * D * vis):
+        _lib.call("alm_attn_delta_dh", o, o.stride(1), d_o, d_o.stride(1), delta, n_q_pad, dq_acc, b, heads, n_q, D)
         _lib.call(
-            "alm_mqa_attn_bwd",
+            "alm_mqa_attn_bwd_dh",
             q, q.stride(1), k, k.stride(1), k.stride(0), v, v.stride(1), v.stride(0), d_o, d_o.stride(1), key_mask,
             lse, delta, n_q_pad, dq, dq.stride(1), dq_acc, dk, dk.stride(1), dv, dv.stride(1),
-            bias, dbias, bhs, brs, b, heads, n_q, n_k, int(causal), float(scale), *_drop_args(dropout),
+            bias, dbias, bhs, brs, b, heads, n_q, n_k, int(causal), float(scale), *_drop_args(dropout), D,
         )
     return dq, dk, dv
 
@@ -305,33 +319,38 @@ def gemv(x, w, *, out_dtype=bf16, bias=None):
 
 
 def kv_append(kv_new, k_cache, v_cache, cache_len):
-    """k_cache[b, len] = kv_new[b, :64]; v_cache[b, len] = kv_new[b, 64:]  (len: int32 device scalar)."""
+    """k_cache[b, len] = kv_new[b, :D]; v_cache[b, len] = kv_new[b, D:]  (len: int32 device scalar; D = dim_head =
+    k_cache.shape[-1])."""
     _check_cuda(kv_new, k_cache, v_cache, cache_len)
-    b, max_len, dh = k_cache.shape
-    assert dh == 64 and v_cache.shape == k_cache.shape and kv_new.shape == (b, 128) and kv_new.dtype == bf16
+    b, max_len, _ = k_cache.shape
+    D = _head_width(k_cache)
+    assert v_cache.shape == k_cache.shape and kv_new.shape == (b, 2 * D) and kv_new.dtype == bf16
     assert k_cache.dtype == bf16 and v_cache.dtype == bf16 and cache_len.dtype == torch.int32
-    assert k_cache.stride(1) == 64 and v_cache.stride() == k_cache.stride() and kv_new.stride(1) == 1
-    _lib.call("alm_kv_append", kv_new, kv_new.stride(0), k_cache, v_cache, k_cache.stride(0), cache_len, max_len, b)
+    assert k_cache.stride(1) == D and v_cache.stride() == k_cache.stride() and kv_new.stride(1) == 1
+    _lib.call("alm_kv_append_dh", kv_new, kv_new.stride(0), k_cache, v_cache, k_cache.stride(0), cache_len, max_len, b,
+              D)
 
 
 def mqa_attn_decode(q, k_cache, v_cache, cache_len, *, heads, key_mask=None, scale=None, splits=None, bias=None):
-    """one new query per sequence against the static cache: q [b, heads*64] bf16 -> o [b, heads*64] bf16.
+    """one new query per sequence against the static cache [b, max_len, D]: q [b, heads*D] bf16 -> o [b, heads*D] bf16.
     Attends keys 0..cache_len (inclusive: the new token has just been appended at position cache_len).
     bias: fp32 [heads, >= max_len] added to the scores of every sequence (row j of head h: bias[h, j]) or None."""
     _check_cuda(q, k_cache, v_cache, cache_len, key_mask, bias)
     b, max_len, _ = k_cache.shape
-    assert q.shape == (b, heads * 64) and q.dtype == bf16 and q.stride(1) == 1
-    o = torch.empty(b, heads * 64, device=q.device, dtype=bf16)
+    D = _head_width(k_cache)
+    assert q.shape == (b, heads * D) and q.dtype == bf16 and q.stride(1) == 1
+    assert v_cache.shape == k_cache.shape and k_cache.stride(1) == D and v_cache.stride() == k_cache.stride()
+    o = torch.empty(b, heads * D, device=q.device, dtype=bf16)
     if key_mask is not None:
         assert key_mask.dtype == torch.uint8 and key_mask.shape[0] == b and key_mask.shape[1] >= max_len
     if bias is not None:
         assert bias.dtype == f32 and bias.shape[0] == heads and bias.shape[1] >= max_len and bias.stride(1) == 1
     if splits is None:  # enough CTAs to spread a long cache over the SMs, fixed per cache size (static launch)
         splits = max(1, min(32, max_len // 128, num_sms(q.device) // max(1, b)))
-    ws = torch.empty(b, splits, heads, 66, device=q.device, dtype=f32) if splits > 1 else None
-    _lib.call("alm_mqa_attn_decode", q, q.stride(0), k_cache, v_cache, k_cache.stride(0), cache_len, max_len, key_mask,
+    ws = torch.empty(b, splits, heads, D + 2, device=q.device, dtype=f32) if splits > 1 else None
+    _lib.call("alm_mqa_attn_decode_dh", q, q.stride(0), k_cache, v_cache, k_cache.stride(0), cache_len, max_len, key_mask,
               0 if key_mask is None else key_mask.stride(0), bias, 0 if bias is None else bias.stride(0), o, o.stride(0),
-              ws, splits, b, heads, float(64 ** -0.5 if scale is None else scale))
+              ws, splits, b, heads, float(D ** -0.5 if scale is None else scale), D)
     return o
 
 
@@ -402,11 +421,12 @@ def decode_stack_grid():
 
 
 @functools.lru_cache(maxsize=None)
-def decode_stack_plan(b, d, heads, inner, n_layers):
-    """None if alm_decode_stack_step refuses this shape on the current device, else for phases A, C, D, E (q|kv, out,
-    W1, W2 projections) whether the weight rows are staged in shared memory (True) or read from L2 (False)."""
+def decode_stack_plan(b, d, heads, inner, n_layers, dim_head=64):
+    """None if alm_decode_stack_step refuses this shape on the current device (it is built for dim_head 64 alone), else
+    for phases A, C, D, E (q|kv, out, W1, W2 projections) whether the weight rows are staged in shared memory (True)
+    or read from L2 (False)."""
     staged = (ctypes.c_int32 * 4)()
-    if _lib.load().alm_decode_stack_plan(b, d, heads, inner, n_layers, staged) != 0:
+    if _lib.load().alm_decode_stack_plan_dh(b, d, heads, inner, n_layers, dim_head, staged) != 0:
         return None
     return tuple(bool(s) for s in staged)
 

@@ -72,7 +72,8 @@ class Attend(nn.Module):
         self.flash = flash
 
     def forward(self, q, k, v, mask=None, attn_bias=None):
-        """q [b h n 64], k/v [b j 64] -> [b h n 64] (inference helper; training goes through Transformer)."""
+        """q [b h n d], k/v [b j d] -> [b h n d], d = dim_head in {32, 64, 128} (inference helper; training goes
+        through Transformer)."""
         b, h, n, d = q.shape
         if exists(attn_bias):
             assert not self.flash, "attention bias not supported for flash attention"  # attend.py:112
@@ -86,16 +87,18 @@ class Attend(nn.Module):
 
 
 class Attention(nn.Module):
-    """Parameter holder for audiolm_pytorch.py:264-406 (self-attention, multi-query, dim_head 64)."""
+    """Parameter holder for audiolm_pytorch.py:264-406 (self-attention, multi-query, dim_head 32, 64 or 128)."""
 
     def __init__(self, dim, causal=False, dim_head=64, dim_context=None, heads=8, norm_context=False,
                  num_null_kv=0, dropout=0.1, scale=8, flash=False):
         super().__init__()
-        if dim_head != 64:
-            raise NotImplementedError("the sm_90a attention kernels are built for dim_head=64")
+        if dim_head not in ops.ATTN_HEAD_WIDTHS:
+            raise NotImplementedError(f"the sm_90a attention kernels are built for dim_head in {ops.ATTN_HEAD_WIDTHS}, "
+                                      f"got {dim_head}")
         if num_null_kv > 0 or exists(dim_context) and dim_context != dim:
             raise NotImplementedError("cross attention / null kv (text conditioning) is out of scope")
         self.heads = heads
+        self.dim_head = dim_head
         self.causal = causal
         inner = dim_head * heads
         self.norm = LayerNorm(dim)
@@ -413,6 +416,7 @@ class Transformer(nn.Module):
                 None,
                 wrap(FeedForward(dim=dim, dropout=ff_dropout)),
             ]))
+        self.dim_head = kwargs.get("dim_head", 64)
         self.norm = LayerNorm(dim)
         self._packed = _PackedWeights()
         # called with the layer index once that layer's parameter gradients are complete in the backward
@@ -547,7 +551,7 @@ class Transformer(nn.Module):
 
     def _walk_forward(self, x, mask, bias, drop, *, save, want_kv, kv_cache=None):
         """The stack's forward over the kernels, for both residual modes.  Returns (out, kv, saved):
-        kv is the [depth, 2, b, cache_len + n, 64] cache tensor when `want_kv` (stacking it is a copy a training step
+        kv is the [depth, 2, b, cache_len + n, dim_head] cache tensor when `want_kv` (stacking it is a copy a training step
         does not need), else an empty tensor; `saved` is what `_walk_backward` reads when `save`, else None.
         `kv_cache`: keys / values of the positions before x."""
         b, n, d = x.shape
@@ -574,7 +578,7 @@ class Transformer(nn.Module):
             if i + 1 < self.depth:
                 xn, bin_ = res.step(Y, P[i + 1][0], P[i + 1][1]["ln"], want_bin=True)
         out = res.exit(Y, self.norm.gamma)
-        # kv cache tensor [depth, 2, b, n, 64] as the reference returns it (audiolm_pytorch.py:370, 560)
+        # kv cache tensor [depth, 2, b, n, dim_head] as the reference returns it (audiolm_pytorch.py:370, 560)
         kv = torch.stack(kvs).unflatten(0, (self.depth, 2)) if want_kv else torch.empty(0, device=x.device, dtype=bf16)
         if not save:
             return out.view(b, n, d), kv, None
@@ -586,22 +590,22 @@ class Transformer(nn.Module):
         rec["xn_a"] / rec["bin_a"]; records q, kv, o, lse in `rec`.  Returns (Y, k, v, v_first), k / v including
         the cached positions."""
         b, n, _ = S["shape"]
-        H = self.heads
-        q = ops.gemm(rec["xn_a"], W["wq"])                 # [M, H*64]
-        kv = ops.gemm(rec["bin_a"], W["wkv"])              # [M, 128]  (k | v) from the UN-normalised input
+        H, D = self.heads, self.dim_head
+        q = ops.gemm(rec["xn_a"], W["wq"])                 # [M, H*D]
+        kv = ops.gemm(rec["bin_a"], W["wkv"])              # [M, 2*D]  (k | v) from the UN-normalised input
         if self.add_value_residual and v_first is not None:
-            ops.axpby(kv[:, 64:], 0.5, v_first, 0.5, out=kv[:, 64:])
+            ops.axpby(kv[:, D:], 0.5, v_first, 0.5, out=kv[:, D:])
         elif self.add_value_residual:
-            v_first = kv[:, 64:].clone()                   # layer-0 values before any mixing (:355-358)
-        k = kv[:, :64].unflatten(0, (b, n))
-        v = kv[:, 64:].unflatten(0, (b, n))
+            v_first = kv[:, D:].clone()                    # layer-0 values before any mixing (:355-358)
+        k = kv[:, :D].unflatten(0, (b, n))
+        v = kv[:, D:].unflatten(0, (b, n))
         if cache is not None:
             k = torch.cat((cache[0].to(bf16), k), dim=1).contiguous()
             v = torch.cat((cache[1].to(bf16), v), dim=1).contiguous()
         # without a backward to feed, the kernel skips writing the row LSE
-        o, lse = ops.mqa_attn_fwd(q.view(b, n, H * 64), k, v, heads=H, key_mask=S["mask"], causal=True,
+        o, lse = ops.mqa_attn_fwd(q.view(b, n, H * D), k, v, heads=H, key_mask=S["mask"], causal=True,
                                   return_lse=save, bias=S["bias"], dropout=d_attn)
-        o = o.view(b * n, H * 64)
+        o = o.view(b * n, H * D)
         Y = ops.gemm(o, W["wo"])
         if d_out:
             ops.dropout_(Y, *d_out)
@@ -663,28 +667,28 @@ class Transformer(nn.Module):
         dv_first: gradient of layer 0's values from the layers above (value residual).  Returns (dxn, dbin, dv_first)."""
         b, n, _ = S["shape"]
         M = b * n
-        H = self.heads
+        H, D = self.heads, self.dim_head
         if d_out:
             ops.dropout_(dY, *d_out)  # dY is read by nothing else
-        dO = ops.gemm(dY, W["wo"], b_mn=True)              # [M, H*64]
+        dO = ops.gemm(dY, W["wo"], b_mn=True)              # [M, H*D]
         wgrad(dY, rec["o"], g["wo"])
         kv = rec["kv"]
-        k3 = kv[:, :64].unflatten(0, (b, n))
-        v3 = kv[:, 64:].unflatten(0, (b, n))
-        dq, dk, dv = ops.mqa_attn_bwd(rec["q"].view(b, n, H * 64), k3, v3, rec["o"].view(b, n, H * 64),
-                                      dO.view(b, n, H * 64), rec["lse"], heads=H, key_mask=S["mask"], causal=True,
+        k3 = kv[:, :D].unflatten(0, (b, n))
+        v3 = kv[:, D:].unflatten(0, (b, n))
+        dq, dk, dv = ops.mqa_attn_bwd(rec["q"].view(b, n, H * D), k3, v3, rec["o"].view(b, n, H * D),
+                                      dO.view(b, n, H * D), rec["lse"], heads=H, key_mask=S["mask"], causal=True,
                                       bias=S["bias"], dbias=S["dbias"], dropout=d_attn)
-        dkv = torch.empty(M, 128, device=dY.device, dtype=bf16)
-        ops.axpby(dk.view(M, 64), 1.0, None, 0.0, out=dkv[:, :64])
-        dv2 = dv.view(M, 64)
+        dkv = torch.empty(M, 2 * D, device=dY.device, dtype=bf16)
+        ops.axpby(dk.view(M, D), 1.0, None, 0.0, out=dkv[:, :D])
+        dv2 = dv.view(M, D)
         if self.add_value_residual and i > 0:
-            ops.axpby(dv2, 0.5, None, 0.0, out=dkv[:, 64:])
+            ops.axpby(dv2, 0.5, None, 0.0, out=dkv[:, D:])
             dv_first = ops.axpby(dv2, 0.5, dv_first, 1.0) if dv_first is not None else ops.axpby(dv2, 0.5, None, 0.0)
         elif self.add_value_residual and dv_first is not None:
-            ops.axpby(dv2, 1.0, dv_first, 1.0, out=dkv[:, 64:])
+            ops.axpby(dv2, 1.0, dv_first, 1.0, out=dkv[:, D:])
         else:
-            ops.axpby(dv2, 1.0, None, 0.0, out=dkv[:, 64:])
-        dq2 = dq.view(M, H * 64)
+            ops.axpby(dv2, 1.0, None, 0.0, out=dkv[:, D:])
+        dq2 = dq.view(M, H * D)
         dxn = ops.gemm(dq2, W["wq"], b_mn=True)
         dbin = ops.gemm(dkv, W["wkv"], b_mn=True)
         wgrad(dq2, rec["xn_a"], g["wq"])

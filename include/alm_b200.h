@@ -102,6 +102,18 @@ int alm_mqa_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int
                      alm_stream_t stream);
 
 /*
+ * alm_mqa_attn_fwd for a head width dim_head in {32, 64, 128} (any other value: ALM_ERR_UNSUPPORTED): every "64" of
+ * the shapes above reads dim_head, i.e. q / o [b, n_q, h*dim_head], k / v [b, n_k, dim_head]; everything else,
+ * including the dropout mask of a given seed (its counter addresses (row, key) only), is as in alm_mqa_attn_fwd, which
+ * is this call with dim_head = 64.  `scale` is passed by the caller (dim_head^-1/2 in the models).
+ */
+int alm_mqa_attn_fwd_dh(const void* q, int64_t ldq, const void* k, int64_t ldk, int64_t k_bstride, const void* v,
+                        int64_t ldv, int64_t v_bstride, const void* key_mask, void* o, int64_t ldo, float* lse,
+                        int64_t lse_stride, const float* bias, int64_t bias_hstride, int64_t bias_rstride, int b,
+                        int h, int n_q, int n_k, int causal, float scale, float dropout_p, uint64_t seed,
+                        uint32_t site, int dim_head, alm_stream_t stream);
+
+/*
  * Backward of alm_mqa_attn_fwd (one wgmma kernel per (batch, 128-key block): dK/dV accumulate over all heads in
  * registers, partial dQ products are reduce-added into dq_acc by TMA; a second kernel converts dq_acc to bf16 dq).
  * lse/delta are [b, h, n_q_pad] with n_q_pad a multiple of 128; delta = rowsum(dO * O) from alm_attn_delta.
@@ -121,6 +133,23 @@ int alm_mqa_attn_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, int
 /* delta[b, h, i] = rowsum(dO * O); also zeroes dq_acc ([b, n, h*64] fp32, contiguous) unless it is null */
 int alm_attn_delta(const void* o, int64_t ldo, const void* d_o, int64_t lddo, float* delta /* [b,h,stride] */,
                    int64_t delta_stride, float* dq_acc, int b, int h, int n, alm_stream_t stream);
+
+/*
+ * alm_mqa_attn_bwd and alm_attn_delta for a head width dim_head in {32, 64, 128} (any other value:
+ * ALM_ERR_UNSUPPORTED); the calls above are these with dim_head = 64.  Shapes: q / d_o / o / dq [b, n_q, h*dim_head],
+ * k / v / dk / dv [b, n_k, dim_head], dq_acc fp32 [b, n_q, h*dim_head] contiguous; lse / delta / bias / dbias and the
+ * dropout mask as above.  One CTA per (batch, 128-key block) at every width; an iteration covers 128 queries at
+ * dim_head 32 and 64, and 64 queries at 128, where dK and dV alone take 128 registers per thread.  dk and dv are
+ * bitwise reproducible at every width (registers, no atomics); dq is not.
+ */
+int alm_mqa_attn_bwd_dh(const void* q, int64_t ldq, const void* k, int64_t ldk, int64_t k_bstride, const void* v,
+                        int64_t ldv, int64_t v_bstride, const void* d_o, int64_t lddo, const void* key_mask,
+                        const float* lse, const float* delta, int n_q_pad, void* dq, int64_t lddq, float* dq_acc,
+                        void* dk, int64_t lddk, void* dv, int64_t lddv, const float* bias, float* dbias,
+                        int64_t bias_hstride, int64_t bias_rstride, int b, int h, int n_q, int n_k, int causal,
+                        float scale, float dropout_p, uint64_t seed, uint32_t site, int dim_head, alm_stream_t stream);
+int alm_attn_delta_dh(const void* o, int64_t ldo, const void* d_o, int64_t lddo, float* delta /* [b,h,stride] */,
+                      int64_t delta_stride, float* dq_acc, int b, int h, int n, int dim_head, alm_stream_t stream);
 
 /*
  * Dense attention bias from a learned table (HBM-bound gather, scatter-add backward):
@@ -165,6 +194,15 @@ int alm_mqa_attn_decode(const void* q, int64_t ldq, const void* k_cache, const v
                         int64_t bias_ld, void* o, int64_t ldo,
                         float* workspace /* [b, splits, h, 66] fp32 when splits > 1 */, int splits, int b, int h,
                         float scale, alm_stream_t stream);
+/* alm_kv_append / alm_mqa_attn_decode for a head width dim_head in {32, 64, 128} (any other value: ALM_ERR_UNSUPPORTED;
+ * the calls above are these with dim_head = 64): kv_new [b, 2*dim_head] = [k | v] (row stride ld), k_cache / v_cache
+ * bf16 [b, max_len, dim_head], q / o [b, h*dim_head], workspace fp32 [b, splits, h, dim_head + 2] when splits > 1. */
+int alm_kv_append_dh(const void* kv_new, int64_t ld, void* k_cache, void* v_cache, int64_t cache_bstride,
+                     const int32_t* len, int max_len, int b, int dim_head, alm_stream_t stream);
+int alm_mqa_attn_decode_dh(const void* q, int64_t ldq, const void* k_cache, const void* v_cache, int64_t cache_bstride,
+                           const int32_t* len, int max_len, const void* key_mask, int64_t mask_bstride,
+                           const float* bias, int64_t bias_ld, void* o, int64_t ldo, float* workspace, int splits,
+                           int b, int h, float scale, int dim_head, alm_stream_t stream);
 int alm_decode_bias_row(const float* table, int rows, const float* override_h, const int32_t* u, const int32_t* cls,
                         int c, const int32_t* len, int max_len, float* out, int64_t ld, int h, alm_stream_t stream);
 
@@ -209,6 +247,9 @@ int alm_decode_stack_grid(void);
  * the step applies).  For an accepted shape, staged[0..3] (may be null) tells for phases A, C, D, E ([to_q ; to_kv],
  * to_out, W1, W2) whether a CTA's weight rows are staged in shared memory (1) or read from L2 (0). */
 int alm_decode_stack_plan(int b, int d, int heads, int inner, int n_layers, int32_t* staged);
+/* The same question for a stack of head width dim_head: alm_decode_stack_step is built for dim_head 64 alone, so any other
+ * width is ALM_ERR_UNSUPPORTED (those models decode with the multi-kernel step); 64 is alm_decode_stack_plan. */
+int alm_decode_stack_plan_dh(int b, int d, int heads, int inner, int n_layers, int dim_head, int32_t* staged);
 int64_t alm_decode_stack_scratch_bytes(int b, int d, int heads, int inner);
 int64_t alm_decode_stack_trace_offset(int b, int d, int heads, int inner); /* debugging: phase stamps of -DALM_DSTEP_TRACE builds */
 int alm_decode_stack_step(const void* layer_table, int n_layers, const float* x, void* out, const float* final_gamma,
