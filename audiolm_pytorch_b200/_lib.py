@@ -68,6 +68,8 @@ SIGNATURES: dict[str, list] = {
     "alm_causal_convT1d_fwd": [P, P, P, P, I, I, I, I, I, P],
     "alm_codec_first_conv": [P, P, P, P, I, I, I, I, I, P],
     "alm_codec_ru_tc": [P, P, P, P, P, I, I, I, I, I, I, P],
+    "alm_codec_ru_se_tc": [P, P, P, P, P, P, P, I, I, I, I, I, I, I, P],
+    "alm_codec_se_fp32": [P, P, P, P, P, P, P, I, I, I, I, P],
     "alm_codec_conv_tc": [P, P, P, P, I, I, I, I, I, I, I, I, I, I, P],
     "alm_codec_pack_c8s": [P, P, I, I, I, P],
     "alm_codec_last_conv": [P, P, P, P, I, I, I, I, I, P],

@@ -440,6 +440,40 @@ __global__ void rvq_decode_kernel(const long long* __restrict__ indices, long lo
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// SqueezeExcite of a ResidualUnit (soundstream.py:145-169, 362-369), fp32 on CUDA cores:
+//   out[b, c, t] = x[b, c, t] + y[b, c, t] * sigmoid(b2[c] + sum_i W2[c, i] silu(b1[i] + sum_c' W1'[i, c'] y[b, c', t]))
+// y = the unit's ELU(conv1(...)) output, x its input; W1' is the first 1x1 conv with the reference's channel-wise
+// cumulative mean folded in (ops.se_fold_weight), so every time step is independent.  One CTA = SE_T time steps of one
+// clip; the y tile and the inner activations stay in shared memory, weights are warp-uniform loads.
+// ------------------------------------------------------------------------------------------------
+constexpr int SE_T = 64;
+
+__global__ void __launch_bounds__(SE_T)
+se_fp32_kernel(const float* __restrict__ y, const float* __restrict__ x, const float* __restrict__ w1,
+               const float* __restrict__ b1, const float* __restrict__ w2, const float* __restrict__ b2,
+               float* __restrict__ out, int C, int Ci, int T) {
+  extern __shared__ float smem[];
+  float* ys = smem;               // [C][SE_T]
+  float* ss = smem + C * SE_T;    // [Ci][SE_T]
+  const int b = blockIdx.y, tid = threadIdx.x;
+  const int t = blockIdx.x * SE_T + tid;
+  const bool ok = t < T;
+  const size_t base = (size_t)b * C * T;
+  for (int c = 0; c < C; ++c) ys[c * SE_T + tid] = ok ? y[base + (size_t)c * T + t] : 0.f;
+  for (int i = 0; i < Ci; ++i) {
+    float acc = __ldg(b1 + i);
+    for (int c = 0; c < C; ++c) acc = fmaf(__ldg(w1 + (size_t)i * C + c), ys[c * SE_T + tid], acc);
+    ss[i * SE_T + tid] = acc / (1.f + expf(-acc));
+  }
+  if (!ok) return;
+  for (int c = 0; c < C; ++c) {
+    float acc = __ldg(b2 + c);
+    for (int i = 0; i < Ci; ++i) acc = fmaf(__ldg(w2 + (size_t)c * Ci + i), ss[i * SE_T + tid], acc);
+    out[base + (size_t)c * T + t] = x[base + (size_t)c * T + t] + ys[c * SE_T + tid] / (1.f + expf(-acc));
+  }
+}
+
 }  // namespace alm
 
 using namespace alm;
@@ -490,6 +524,26 @@ extern "C" int alm_residual_unit_fwd(const float* x, const float* w7_packed, con
               ALM_ERR_ALIGN);
   const int rc = cvt::dispatch_ru(x, w7_packed, b7, w1_packed, b1, y, B, C, T, dilation, pad_mode, stream);
   return rc == -1 ? ALM_ERR_UNSUPPORTED : rc;
+}
+
+extern "C" int alm_codec_se_fp32(const float* y, const float* x, const float* w1_folded, const float* b1,
+                                 const float* w2, const float* b2, float* out, int B, int C, int Ci, int T,
+                                 alm_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ALM_REQUIRE(y && x && w1_folded && b1 && w2 && b2 && out && B > 0 && C > 0 && Ci > 0 && T > 0 && B <= 65535,
+              ALM_ERR_ARG);
+  const size_t smem = (size_t)(C + Ci) * SE_T * sizeof(float);
+  ALM_REQUIRE(smem <= 200 * 1024, ALM_ERR_UNSUPPORTED);
+  static size_t attr = 0;
+  if (smem > 48 * 1024 && smem > attr) {
+    ALM_CUDA_OK(cudaFuncSetAttribute(se_fp32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr = smem;
+  }
+  dim3 grid(ceil_div(T, SE_T), B);
+  se_fp32_kernel<<<grid, SE_T, smem, stream>>>(y, x, w1_folded, b1, w2, b2, out, C, Ci, T);
+  ALM_CHECK_LAUNCH();
+  ALM_LAUNCHED(1);
+  return ALM_OK;
 }
 
 extern "C" int alm_causal_convT1d_fwd(const float* x, const float* w, const float* bias, float* y, int B, int Cin,

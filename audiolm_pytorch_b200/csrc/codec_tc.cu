@@ -19,8 +19,9 @@
 //
 // Kernels
 //   first_conv_kernel      fp32 wave [B][T] (C_in = 1) -> C8S, CUDA cores (7 FMAs per output, HBM-bound on the write)
-//   ru_tc_kernel<C>        fused ResidualUnit: y = x + ELU(W1 ELU(W7 *_d x + b7) + b1); the k=7 result goes
-//                          registers -> (bias, ELU, split) -> shared memory as the bf16 A operand of the 1x1 conv
+//   ru_tc_kernel<C, SE>    fused ResidualUnit: y = x + ELU(W1 ELU(W7 *_d x + b7) + b1); the k=7 result goes
+//                          registers -> (bias, ELU, split) -> shared memory as the bf16 A operand of the 1x1 conv.
+//                          SE = true adds the unit's SqueezeExcite (soundstream.py:145-169) as two more GEMMs per tile
 //   conv_tc_kernel<..>     strided / plain causal conv as a pipelined implicit GEMM over (tap, k-step) units
 // Activation tiles are staged with 16-B cp.async by whole producer warps, weights with large bulk copies.
 #include "alm_common.cuh"
@@ -33,6 +34,8 @@ constexpr int TILE_M = 128;
 constexpr int MAX_HALO = 54;  // 6 * dilation 9
 
 __device__ __forceinline__ float elu1(float v) { return v > 0.f ? v : (__expf(v) - 1.f); }
+__device__ __forceinline__ float silu1(float v) { return v / (1.f + __expf(-v)); }
+__device__ __forceinline__ float sigmoid1(float v) { return 1.f / (1.f + __expf(-v)); }
 
 // 8 fp32 -> hi uint4, lo uint4 (bf16 pairs, channel e in the low half of word e/2 for even e)
 __device__ __forceinline__ void split8(const float (&v)[8], uint4& hi, uint4& lo) {
@@ -184,6 +187,16 @@ __device__ __forceinline__ RowAddr c8s_row(int b, int t, int nch, int P, int T) 
 // writes the split bf16 activation to shared memory in the no-swizzle K-major layout, which is the A operand of the
 // 1x1 conv (D2); E2 adds b1, applies ELU, adds the skip input and stores C8S.  One warpgroup per CTA keeps the
 // register budget at 255 per thread, which the C = 256 layer (two 128-register accumulators in sequence) needs.
+//
+// SE = true (ResidualUnit(squeeze_excite=True), soundstream.py:362-369): the unit's output is x + y * gate(y) with
+// y = ELU(D2 + b1).  The reference's "cumulative mean" runs over channels (SqueezeExcite.forward cumsums dim -2 of
+// [B, C, T]), so the gate is pointwise in time and the mean folds into the first SE weight (ops.pack_ru_se_weights):
+//   gate = sigmoid(W2 SiLU(W1' y + bs1) + bs2),  W1'[i, c'] = sum_{c >= c'} W1[i, c] / (c + 1).
+// E2 writes split y to sA2 (as E1 does); D3 = y W1'^T (N = NS, the inner width zero-padded to >= 32, A from sA2);
+// E3 adds bs1, applies SiLU and splits the accumulators straight into register A fragments (the m64nNk16 accumulator
+// and the k16 register-A layouts coincide); D4 = s W2^T (N = C, K = NS, A from registers); E4 re-reads y from sA2,
+// adds the skip input and stores.  Re-reading y keeps the C = 256 layer at one 128-register accumulator.  The SE
+// weights stream through the same ring (or stay resident) after the conv units: KSTEPS W1' units, NS / 16 W2 units.
 // ---------------------------------------------------------------------------------------------
 constexpr int RU_TILE_M = 64;
 constexpr int RU_THREADS = 256;
@@ -198,9 +211,12 @@ struct RuParams {
   int tiles_per_clip, total_tiles;
   int ar;      // rows of one staged chunk: RU_TILE_M + 6 d
   int na, nw;  // staged activation tiles (1 or 2), weight ring stages (streamed mode)
+  const float* se_b1 = nullptr;  // SE only: biases of the two 1x1 convs ([se_ci], [C])
+  const float* se_b2 = nullptr;
+  int se_ci = 0;
 };
 
-template <int C>
+template <int C, bool SE = false>
 struct RuCfg {
   static constexpr int NCHUNK = C / 8;
   static constexpr int KSTEPS = C / 16;
@@ -209,18 +225,34 @@ struct RuCfg {
   static constexpr int NUNITS = 8 * KSTEPS;
   static constexpr int MAX_NW = 16;
   static constexpr int A2_BYTES = 2 * NCHUNK * RU_TILE_M * 16;  // E1 output: [hi / lo][chunk][64 rows][16 B]
-  static constexpr int FIXED_BYTES = A2_BYTES + 2 * C * 4 + 512 + 128;  // A2, biases, barriers, alignment slack
+  // squeeze-excite: inner width padded to NS (a multiple of 16, >= 32 for the smallest wgmma tile in use)
+  static constexpr int NS = SE ? (C / 4 > 32 ? C / 4 : 32) : 0;
+  static constexpr int SE1_UNIT_BYTES = 2 * 2 * NS * 16;  // one k-step of W1': hi / lo [2 chunks][NS][16 B]
+  static constexpr int SE_BYTES = KSTEPS * SE1_UNIT_BYTES + (NS / 16) * UNIT_BYTES;
+  static constexpr int W_BYTES = NUNITS * UNIT_BYTES + SE_BYTES;  // the packed weights of one unit (resident image)
+  static constexpr int BIAS_FLOATS = 2 * C + (SE ? NS + C : 0);  // b7, b1 (, bs1 padded to NS, bs2)
+  static constexpr int FIXED_BYTES = A2_BYTES + BIAS_FLOATS * 4 + 512 + 128;  // A2, biases, barriers, alignment slack
   static constexpr int MAX_SMEM = 232448;
   // two CTAs per SM only where shared memory allows it at every dilation (resident weights, largest halo); the
   // occupancy hint of the kernel and the grid size of launch_ru both follow from it
   static constexpr int RESIDENT_MAX_SMEM =
-      2 * (2 * NCHUNK * (RU_TILE_M + MAX_HALO) * 16) + NUNITS * UNIT_BYTES + FIXED_BYTES;
+      2 * (2 * NCHUNK * (RU_TILE_M + MAX_HALO) * 16) + W_BYTES + FIXED_BYTES;
   static constexpr int CTAS_PER_SM = RESIDENT && RESIDENT_MAX_SMEM <= 113 * 1024 ? 2 : 1;
+  // weight unit u of the packed image: 8 KSTEPS conv units, then KSTEPS W1' units, then NS / 16 W2 units
+  static constexpr int ALL_UNITS = NUNITS + (SE ? KSTEPS + NS / 16 : 0);
+  __host__ __device__ static constexpr int unit_off(int u) {
+    return u < NUNITS            ? u * UNIT_BYTES
+           : u < NUNITS + KSTEPS ? NUNITS * UNIT_BYTES + (u - NUNITS) * SE1_UNIT_BYTES
+                                 : NUNITS * UNIT_BYTES + KSTEPS * SE1_UNIT_BYTES + (u - NUNITS - KSTEPS) * UNIT_BYTES;
+  }
+  __host__ __device__ static constexpr int unit_bytes(int u) {
+    return u >= NUNITS && u < NUNITS + KSTEPS ? SE1_UNIT_BYTES : UNIT_BYTES;
+  }
 };
 
-template <int C>
-__global__ void __launch_bounds__(RU_THREADS, RuCfg<C>::CTAS_PER_SM) ru_tc_kernel(const RuParams p) {
-  using Cfg = RuCfg<C>;
+template <int C, bool SE>
+__global__ void __launch_bounds__(RU_THREADS, RuCfg<C, SE>::CTAS_PER_SM) ru_tc_kernel(const RuParams p) {
+  using Cfg = RuCfg<C, SE>;
   constexpr int NCHUNK = Cfg::NCHUNK, KSTEPS = Cfg::KSTEPS;
   constexpr bool RESIDENT = Cfg::RESIDENT;
   const int NA = p.na, NW = p.nw, A_ROWS = p.ar;
@@ -230,8 +262,8 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C>::CTAS_PER_SM) ru_tc_kerne
   uint8_t* sA2 = smem;
   uint8_t* sA = sA2 + Cfg::A2_BYTES;
   uint8_t* sW = sA + NA * A_BYTES;
-  float* sBias = reinterpret_cast<float*>(sW + (RESIDENT ? Cfg::NUNITS : NW) * Cfg::UNIT_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + 2 * C);
+  float* sBias = reinterpret_cast<float*>(sW + (RESIDENT ? Cfg::W_BYTES : NW * Cfg::UNIT_BYTES));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sBias + Cfg::BIAS_FLOATS);
   uint64_t* a_full = bars;              // [2]
   uint64_t* a_empty = bars + 2;         // [2]
   uint64_t* w_full = bars + 4;          // [<= 16] (resident: [0] only)
@@ -253,6 +285,10 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C>::CTAS_PER_SM) ru_tc_kerne
     sBias[i] = p.b7 ? p.b7[i] : 0.f;
     sBias[C + i] = p.b1 ? p.b1[i] : 0.f;
   }
+  if constexpr (SE) {
+    for (int i = threadIdx.x; i < Cfg::NS; i += blockDim.x) sBias[2 * C + i] = i < p.se_ci ? p.se_b1[i] : 0.f;
+    for (int i = threadIdx.x; i < C; i += blockDim.x) sBias[2 * C + Cfg::NS + i] = p.se_b2[i];
+  }
   __syncthreads();
 
   const int halo = 6 * p.d;
@@ -266,11 +302,11 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C>::CTAS_PER_SM) ru_tc_kerne
     // Resident-weight layers (C <= 64) run TWO producer warps, warp 0 owning staging buffer 0 (even tiles) and warp 3
     // buffer 1 (odd tiles).
     if (RESIDENT && warp == 0 && lane == 0) {
-      mbar_arrive_expect_tx(&w_full[0], Cfg::NUNITS * Cfg::UNIT_BYTES);
+      mbar_arrive_expect_tx(&w_full[0], Cfg::W_BYTES);
       constexpr int PIECE = 16384;  // few large copies
-      for (int off = 0; off < Cfg::NUNITS * Cfg::UNIT_BYTES; off += PIECE)
-        bulk_copy_g2s(sW + off, reinterpret_cast<const uint8_t*>(p.w) + off,
-                      min(PIECE, Cfg::NUNITS * Cfg::UNIT_BYTES - off), &w_full[0]);
+      for (int off = 0; off < Cfg::W_BYTES; off += PIECE)
+        bulk_copy_g2s(sW + off, reinterpret_cast<const uint8_t*>(p.w) + off, min(PIECE, Cfg::W_BYTES - off),
+                      &w_full[0]);
     }
     int wstage = 0;
     uint32_t wphase = 0;
@@ -280,6 +316,15 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C>::CTAS_PER_SM) ru_tc_kerne
         mbar_arrive_expect_tx(&w_full[wstage], Cfg::UNIT_BYTES);
         bulk_copy_g2s(sW + wstage * Cfg::UNIT_BYTES, p.w + (size_t)u * (Cfg::UNIT_BYTES / 2), Cfg::UNIT_BYTES,
                       &w_full[wstage]);
+        if (++wstage == NW) { wstage = 0; wphase ^= 1u; }
+      }
+    };
+    auto stream_se_units = [&](int u0, int u1) {  // lane 0 only; the W1' units are smaller than a ring slot
+      for (int u = u0; u < u1; ++u) {
+        mbar_wait(&w_empty[wstage], wphase ^ 1u);
+        mbar_arrive_expect_tx(&w_full[wstage], Cfg::unit_bytes(u));
+        bulk_copy_g2s(sW + wstage * Cfg::UNIT_BYTES, reinterpret_cast<const uint8_t*>(p.w) + Cfg::unit_off(u),
+                      Cfg::unit_bytes(u), &w_full[wstage]);
         if (++wstage == NW) { wstage = 0; wphase ^= 1u; }
       }
     };
@@ -345,7 +390,11 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C>::CTAS_PER_SM) ru_tc_kerne
         if (lane == 0) mbar_arrive(&a_full[i % NA]);
         // publish tile i BEFORE staging tile i + 1: the staging waits for a_empty and takes ~1 k clk of issue
         if (NA == 2 && has(i + 1)) issue_a(i + 1);
-        if (lane == 0) stream_units(0, 8 * KSTEPS);
+        if constexpr (SE) {
+          if (lane == 0) stream_se_units(0, Cfg::ALL_UNITS);
+        } else {
+          if (lane == 0) stream_units(0, 8 * KSTEPS);
+        }
         __syncwarp();
         if (NA == 1 && has(i + 1)) issue_a(i + 1);
       }
@@ -370,6 +419,12 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C>::CTAS_PER_SM) ru_tc_kerne
     if (RESIDENT) return b0 + (uint64_t)(u * (Cfg::UNIT_BYTES / 16));
     mbar_wait(&w_full[wstage], wphase);
     return b0 + (uint64_t)(wstage * (Cfg::UNIT_BYTES / 16));
+  };
+  // SE units: resident at their packed offset, else the next ring slot; `base` carries the operand's LBO
+  auto se_unit = [&](int u, uint64_t base) -> uint64_t {
+    if (RESIDENT) return base + (uint64_t)(Cfg::unit_off(u) / 16);
+    mbar_wait(&w_full[wstage], wphase);
+    return base + (uint64_t)(wstage * (Cfg::UNIT_BYTES / 16));
   };
   auto unit_done = [&]() {
     wgmma_commit();
@@ -445,45 +500,133 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C>::CTAS_PER_SM) ru_tc_kerne
     }
     drain();
     wgmma_fence_acc(d);
-    // ---- E2: D2 (+b1, ELU, + skip) -> split -> global (C8S) ----
     const int tile = tile_of(i);
     const int b = tile / p.tiles_per_clip;
     const int t0 = (tile - b * p.tiles_per_clip) * RU_TILE_M;
+    if constexpr (SE) {
+      constexpr int NS = Cfg::NS;
+      // ---- E2: y = ELU(D2 + b1) -> split -> sA2 (A operand of D3, re-read by E4) ----
+      asm volatile("bar.sync 1, 128;" ::: "memory");  // every warp's D2 reads of sA2 have retired
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int t = t0 + rl + 8 * h;
-      if (t >= p.T) continue;
-      const __nv_bfloat16* xrow = p.x + ((size_t)b * 2 * NCHUNK * p.T + t) * 8 + c_lane;
-      const RowAddr ya = c8s_row(b, t, 2 * NCHUNK, p.out_phases, p.T);
+      for (int j = 0; j < C / 8; ++j)
 #pragma unroll
-      for (int j = 0; j < C / 8; ++j) {
-        const int col = 8 * j + c_lane;
-        const uint32_t hw = __ldg(reinterpret_cast<const uint32_t*>(xrow + (size_t)j * p.T * 8));
-        const uint32_t lw = __ldg(reinterpret_cast<const uint32_t*>(xrow + (size_t)(NCHUNK + j) * p.T * 8));
-        const float v0 = bf16_lo(hw) + bf16_lo(lw) + elu1(d[4 * j + 2 * h] + sBias[C + col]);
-        const float v1 = bf16_hi(hw) + bf16_hi(lw) + elu1(d[4 * j + 2 * h + 1] + sBias[C + col + 1]);
-        uint32_t oh, ol;
-        split_bf16x2(v0, v1, oh, ol);
-        *reinterpret_cast<uint32_t*>(p.y + ya.off + (size_t)j * ya.chunk_stride + c_lane) = oh;
-        *reinterpret_cast<uint32_t*>(p.y + ya.off + (size_t)(NCHUNK + j) * ya.chunk_stride + c_lane) = ol;
+        for (int h = 0; h < 2; ++h) {
+          const int col = 8 * j + c_lane;
+          uint32_t hi, lo;
+          split_bf16x2(elu1(d[4 * j + 2 * h] + sBias[C + col]), elu1(d[4 * j + 2 * h + 1] + sBias[C + col + 1]), hi,
+                       lo);
+          const uint32_t off = (uint32_t)(j * RU_TILE_M + rl + 8 * h) * 16 + c_lane * 2;
+          *reinterpret_cast<uint32_t*>(sA2 + off) = hi;
+          *reinterpret_cast<uint32_t*>(sA2 + NCHUNK * RU_TILE_M * 16 + off) = lo;
+        }
+      fence_proxy_async_smem();
+      asm volatile("bar.sync 1, 128;" ::: "memory");
+      // ---- D3 = W1' y: N = NS, K = C, A from sA2 ----
+      float s[NS / 2];
+      const uint64_t b3 = wgmma_desc_nosw(sw_addr, 128, NS * 16);
+#pragma unroll
+      for (int kk = 0; kk < KSTEPS; ++kk) {
+        const uint64_t b_hi = se_unit(8 * KSTEPS + kk, b3);
+        const uint64_t b_lo = b_hi + (uint64_t)(2 * NS);
+        const uint32_t a_off = a2_addr + kk * 2 * (RU_TILE_M * 16);
+        const uint64_t a_hi = wgmma_desc_nosw(a_off, 128, RU_TILE_M * 16);
+        const uint64_t a_lo = wgmma_desc_nosw(a_off + NCHUNK * (RU_TILE_M * 16), 128, RU_TILE_M * 16);
+        wgmma_fence();
+        wgmma_ss<NS>(s, a_hi, b_hi, kk > 0 ? 1u : 0u);
+        wgmma_ss<NS>(s, a_lo, b_hi, 1u);
+        wgmma_ss<NS>(s, a_hi, b_lo, 1u);
+        unit_done();
       }
+      drain();
+      wgmma_fence_acc(s);
+      // ---- E3: SiLU(D3 + bs1) -> split register A fragments of D4: a[q] of k-step kk is accumulator group
+      // j = 2 kk + q / 2, row half q % 2 (padded inner channels are SiLU(0) = 0) ----
+      uint32_t s_hi[NS / 16][4], s_lo[NS / 16][4];
+#pragma unroll
+      for (int kk = 0; kk < NS / 16; ++kk)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int j = 2 * kk + q / 2, h = q % 2;
+          const int col = 8 * j + c_lane;
+          split_bf16x2(silu1(s[4 * j + 2 * h] + sBias[2 * C + col]), silu1(s[4 * j + 2 * h + 1] + sBias[2 * C + col + 1]),
+                       s_hi[kk][q], s_lo[kk][q]);
+        }
+      // ---- D4 = W2 s: N = C, K = NS ----
+#pragma unroll
+      for (int kk = 0; kk < NS / 16; ++kk) {
+        const uint64_t b_hi = se_unit(9 * KSTEPS + kk, b0);
+        const uint64_t b_lo = b_hi + (uint64_t)(2 * C);
+        wgmma_fence();
+        wgmma_rs<C>(d, s_hi[kk], b_hi, kk > 0 ? 1u : 0u);
+        wgmma_rs<C>(d, s_lo[kk], b_hi, 1u);
+        wgmma_rs<C>(d, s_hi[kk], b_lo, 1u);
+        unit_done();
+      }
+      drain();
+      wgmma_fence_acc(d);
+      // ---- E4: skip + y * sigmoid(D4 + bs2) -> split -> global (C8S); each thread re-reads the y it wrote ----
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int t = t0 + rl + 8 * h;
+        if (t >= p.T) continue;
+        const __nv_bfloat16* xrow = p.x + ((size_t)b * 2 * NCHUNK * p.T + t) * 8 + c_lane;
+        const RowAddr ya = c8s_row(b, t, 2 * NCHUNK, p.out_phases, p.T);
+#pragma unroll
+        for (int j = 0; j < C / 8; ++j) {
+          const int col = 8 * j + c_lane;
+          const uint32_t hw = __ldg(reinterpret_cast<const uint32_t*>(xrow + (size_t)j * p.T * 8));
+          const uint32_t lw = __ldg(reinterpret_cast<const uint32_t*>(xrow + (size_t)(NCHUNK + j) * p.T * 8));
+          const uint32_t off = (uint32_t)(j * RU_TILE_M + rl + 8 * h) * 16 + c_lane * 2;
+          const uint32_t yh = *reinterpret_cast<const uint32_t*>(sA2 + off);
+          const uint32_t yl = *reinterpret_cast<const uint32_t*>(sA2 + NCHUNK * RU_TILE_M * 16 + off);
+          const float v0 = bf16_lo(hw) + bf16_lo(lw) +
+                           (bf16_lo(yh) + bf16_lo(yl)) * sigmoid1(d[4 * j + 2 * h] + sBias[2 * C + NS + col]);
+          const float v1 = bf16_hi(hw) + bf16_hi(lw) +
+                           (bf16_hi(yh) + bf16_hi(yl)) * sigmoid1(d[4 * j + 2 * h + 1] + sBias[2 * C + NS + col + 1]);
+          uint32_t oh, ol;
+          split_bf16x2(v0, v1, oh, ol);
+          *reinterpret_cast<uint32_t*>(p.y + ya.off + (size_t)j * ya.chunk_stride + c_lane) = oh;
+          *reinterpret_cast<uint32_t*>(p.y + ya.off + (size_t)(NCHUNK + j) * ya.chunk_stride + c_lane) = ol;
+        }
+      }
+    } else {
+      // ---- E2: D2 (+b1, ELU, + skip) -> split -> global (C8S) ----
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int t = t0 + rl + 8 * h;
+        if (t >= p.T) continue;
+        const __nv_bfloat16* xrow = p.x + ((size_t)b * 2 * NCHUNK * p.T + t) * 8 + c_lane;
+        const RowAddr ya = c8s_row(b, t, 2 * NCHUNK, p.out_phases, p.T);
+#pragma unroll
+        for (int j = 0; j < C / 8; ++j) {
+          const int col = 8 * j + c_lane;
+          const uint32_t hw = __ldg(reinterpret_cast<const uint32_t*>(xrow + (size_t)j * p.T * 8));
+          const uint32_t lw = __ldg(reinterpret_cast<const uint32_t*>(xrow + (size_t)(NCHUNK + j) * p.T * 8));
+          const float v0 = bf16_lo(hw) + bf16_lo(lw) + elu1(d[4 * j + 2 * h] + sBias[C + col]);
+          const float v1 = bf16_hi(hw) + bf16_hi(lw) + elu1(d[4 * j + 2 * h + 1] + sBias[C + col + 1]);
+          uint32_t oh, ol;
+          split_bf16x2(v0, v1, oh, ol);
+          *reinterpret_cast<uint32_t*>(p.y + ya.off + (size_t)j * ya.chunk_stride + c_lane) = oh;
+          *reinterpret_cast<uint32_t*>(p.y + ya.off + (size_t)(NCHUNK + j) * ya.chunk_stride + c_lane) = ol;
+        }
     }
-    // every thread's sA2 reads by the D2 wgmmas have retired (drain above); E1 of the next tile may overwrite it
+    }
+    // every thread's sA2 reads by the D2 (D3) wgmmas have retired (drain above); E1 of the next tile may overwrite it
     asm volatile("bar.sync 1, 128;" ::: "memory");
   }
 }
 
-template <int C>
+template <int C, bool SE = false>
 static int launch_ru(RuParams p, cudaStream_t stream) {
-  using Cfg = RuCfg<C>;
-  auto kfn = ru_tc_kernel<C>;
+  using Cfg = RuCfg<C, SE>;
+  auto kfn = ru_tc_kernel<C, SE>;
   p.ar = RU_TILE_M + 6 * p.d;
   const int a_bytes = 2 * Cfg::NCHUNK * p.ar * 16;
   int smem;
   if (Cfg::RESIDENT) {
     p.na = 2;
     p.nw = 0;
-    smem = 2 * a_bytes + Cfg::NUNITS * Cfg::UNIT_BYTES + Cfg::FIXED_BYTES;
+    smem = 2 * a_bytes + Cfg::W_BYTES + Cfg::FIXED_BYTES;
   } else {
     // the weight ring must cover the L2 latency of the streamed units: as many stages as fit; a second staged
     // activation tile only if that still leaves at least 48 KB of ring
@@ -780,6 +923,37 @@ extern "C" int alm_codec_ru_tc(const void* x, void* y, const void* w_units, cons
     case 64: return ctc::launch_ru<64>(p, stream);
     case 128: return ctc::launch_ru<128>(p, stream);
     case 256: return ctc::launch_ru<256>(p, stream);
+    default: return ALM_ERR_UNSUPPORTED;
+  }
+}
+
+extern "C" int alm_codec_ru_se_tc(const void* x, void* y, const void* w_units, const float* b7, const float* b1,
+                                  const float* se_b1, const float* se_b2, int B, int C, int se_ci, int T, int dilation,
+                                  int pad_mode, int out_phases, alm_stream_t stream_) {
+  using namespace alm;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ALM_REQUIRE(x && y && w_units && se_b1 && se_b2 && B > 0 && T > 0, ALM_ERR_ARG);
+  ALM_REQUIRE(dilation >= 1 && 6 * dilation <= ctc::MAX_HALO && pad_mode >= 0 && pad_mode <= 2, ALM_ERR_UNSUPPORTED);
+  ALM_REQUIRE(T > 6 * dilation, ALM_ERR_ARG);
+  ALM_REQUIRE(out_phases >= 1 && T % out_phases == 0, ALM_ERR_ARG);
+  ctc::RuParams p;
+  p.x = reinterpret_cast<const __nv_bfloat16*>(x);
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.w = reinterpret_cast<const __nv_bfloat16*>(w_units);
+  p.b7 = b7;
+  p.b1 = b1;
+  p.se_b1 = se_b1;
+  p.se_b2 = se_b2;
+  p.se_ci = se_ci;
+  p.B = B; p.T = T; p.d = dilation; p.pad_mode = pad_mode; p.out_phases = out_phases;
+  p.tiles_per_clip = ceil_div(T, ctc::RU_TILE_M);
+  p.total_tiles = p.tiles_per_clip * B;
+  auto inner_ok = [&](int ns) { return se_ci >= 1 && se_ci <= ns; };
+  switch (C) {
+    case 32: return inner_ok(ctc::RuCfg<32, true>::NS) ? ctc::launch_ru<32, true>(p, stream) : ALM_ERR_UNSUPPORTED;
+    case 64: return inner_ok(ctc::RuCfg<64, true>::NS) ? ctc::launch_ru<64, true>(p, stream) : ALM_ERR_UNSUPPORTED;
+    case 128: return inner_ok(ctc::RuCfg<128, true>::NS) ? ctc::launch_ru<128, true>(p, stream) : ALM_ERR_UNSUPPORTED;
+    case 256: return inner_ok(ctc::RuCfg<256, true>::NS) ? ctc::launch_ru<256, true>(p, stream) : ALM_ERR_UNSUPPORTED;
     default: return ALM_ERR_UNSUPPORTED;
   }
 }

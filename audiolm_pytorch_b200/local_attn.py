@@ -54,8 +54,8 @@ class LocalMHA(nn.Module):
         super().__init__()
         if not (causal and prenorm and qk_rmsnorm and use_xpos and use_rotary_pos_emb and gate_values_per_head):
             raise NotImplementedError("LocalMHA is built for the configuration soundstream.py:418-427 uses")
-        if dim_head != 64:
-            raise NotImplementedError("the sm_90a attention kernel is built for dim_head=64")
+        if dim_head not in ops.ATTN_HEAD_WIDTHS:
+            raise NotImplementedError(f"the sm_90a attention kernels are built for dim_head in {ops.ATTN_HEAD_WIDTHS}")
         if dim % 8 != 0:
             raise ValueError("dim must be a multiple of 8")
         inner = dim_head * heads

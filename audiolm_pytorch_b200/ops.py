@@ -687,6 +687,34 @@ def residual_unit(x, w7_packed, b7, w1_packed, b1, *, dilation, pad_mode="reflec
     return y
 
 
+def se_fold_weight(w1):
+    """SqueezeExcite's first 1x1 conv [Ci, C, 1] with the reference's cumulative mean folded in -> fp32 [Ci, C].
+
+    SqueezeExcite.forward (soundstream.py:156-169) receives [B, C, T] but cumsums dim -2, so its "cumulative mean" runs
+    over channels: m[c] = mean_{c' <= c} y[c'].  That is linear, so W1 m = W1' y with
+    W1'[i, c'] = sum_{c >= c'} W1[i, c] / (c + 1), computed here in fp64."""
+    w = w1.detach()[..., 0].double()
+    C = w.shape[1]
+    scaled = w / torch.arange(1, C + 1, device=w.device, dtype=torch.float64)
+    return scaled.flip(-1).cumsum(-1).flip(-1).float().contiguous()
+
+
+def codec_se_fp32(y, x, w1_folded, b1, w2, b2):
+    """SqueezeExcite residual tail out = x + y * gate(y) on fp32 [B, C, T] (csrc/codec.cu); w1_folded from
+    se_fold_weight, w2 [C, Ci(, 1)]."""
+    _check_cuda(y, x, w1_folded, b1, w2, b2)
+    y, x = y.contiguous(), x.contiguous()
+    B, C, T = y.shape
+    Ci = w1_folded.shape[0]
+    assert x.shape == y.shape and y.dtype == f32 and x.dtype == f32 and w1_folded.shape == (Ci, C)
+    w2 = w2.detach().reshape(C, Ci).float().contiguous()
+    out = torch.empty_like(y)
+    with _timed("codec_se_fp32", 2.0 * B * T * 2 * C * Ci):
+        _lib.call("alm_codec_se_fp32", y, x, w1_folded, b1.detach().float().contiguous(), w2,
+                  b2.detach().float().contiguous(), out, B, C, Ci, T)
+    return out
+
+
 def causal_conv_transpose1d(x, weight, bias=None, *, stride):
     """CausalConvTranspose1d forward (soundstream.py:347-360): weight [Cin, Cout, 2*stride]."""
     _check_cuda(x, weight, bias)
@@ -741,6 +769,26 @@ def _split_units(w, bn=None):
 def pack_ru_weights(w7, w1):
     """ResidualUnit weights [C, C, 7], [C, C, 1] -> the unit layout alm_codec_ru_tc streams (tap 7 = the 1x1 conv)."""
     return _split_units(torch.cat((w7.detach().float(), w1.detach().float()), dim=2))
+
+
+def se_inner_pad(C):
+    """inner width of the tensor-core SqueezeExcite GEMMs: the reference's max(8, C // 4), zero-padded to >= 32"""
+    return max(32, C // 4)
+
+
+def pack_ru_se_weights(w7, w1, se_w1, se_w2):
+    """ResidualUnit(squeeze_excite=True) weights -> the unit layout alm_codec_ru_se_tc streams: pack_ru_weights, then the
+    folded first SE conv (se_fold_weight) as [C/16] k-steps with NS rows and the second SE conv as [NS/16] k-steps with C
+    rows, NS = se_inner_pad(C), zero-padded."""
+    C = w7.shape[0]
+    Ci = se_w1.shape[0]
+    ns = se_inner_pad(C)
+    assert se_w1.shape[:2] == (Ci, C) and se_w2.shape[:2] == (C, Ci) and Ci <= ns
+    w1f = torch.zeros(ns, C, 1, device=w7.device, dtype=f32)
+    w1f[:Ci, :, 0] = se_fold_weight(se_w1)
+    w2p = torch.zeros(C, ns, 1, device=w7.device, dtype=f32)
+    w2p[:, :Ci, 0] = se_w2.detach().reshape(C, Ci).float()
+    return torch.cat((pack_ru_weights(w7, w1).flatten(), _split_units(w1f).flatten(), _split_units(w2p).flatten()))
 
 
 def conv_tc_bn(cout):
@@ -812,6 +860,26 @@ def codec_ru_tc(x, w_units, b7, b1, *, dilation, pad_mode="reflect", out_phases=
     with _timed(cls, 2.0 * B * C * T * 4, "byte"):
         _lib.call("alm_codec_ru_tc", x, y, w_units, b7, b1, B, C, T, int(dilation), PAD_MODES[pad_mode],
                   int(out_phases))
+    return y
+
+
+def codec_ru_se_tc(x, w_units, b7, b1, se_b1, se_b2, *, dilation, pad_mode="reflect", out_phases=1):
+    """fused ResidualUnit with SqueezeExcite on C8S activations; w_units from pack_ru_se_weights."""
+    _check_cuda(x, w_units, b7, b1, se_b1, se_b2)
+    B, nch2, P, T, _ = x.shape
+    C = nch2 * 4
+    ns = se_inner_pad(C)
+    assert P == 1 and x.dtype == bf16 and x.is_contiguous() and w_units.dtype == bf16 and w_units.is_contiguous()
+    assert w_units.numel() == (8 * (C // 16) * C + (C // 16) * ns + (ns // 16) * C) * 2 * 2 * 8
+    se_b1, se_b2 = se_b1.detach().float().contiguous(), se_b2.detach().float().contiguous()
+    assert se_b2.numel() == C and 1 <= se_b1.numel() <= ns
+    y = torch.empty(B, nch2, out_phases, T // out_phases, 8, device=x.device, dtype=bf16)
+    cls = "codec_ru_se_tc"
+    if _PROFILE is not None and PROFILE_SHAPES:
+        cls += f" C{C} T{T} d{dilation} P{out_phases}"
+    with _timed(cls, 2.0 * B * C * T * 4, "byte"):
+        _lib.call("alm_codec_ru_se_tc", x, y, w_units, b7, b1, se_b1, se_b2, B, C, se_b1.numel(), T, int(dilation),
+                  PAD_MODES[pad_mode], int(out_phases))
     return y
 
 

@@ -71,26 +71,54 @@ class CausalConvTranspose1d(nn.Module):
         return ops.causal_conv_transpose1d(x, self.conv.weight, self.conv.bias, stride=self.upsample_factor)
 
 
-class _RUBody(nn.Module):
-    """holds the two convs under the reference's Sequential indices 0 and 2 (1, 3 are ELUs)."""
+class SqueezeExcite(nn.Module):
+    """soundstream.py:145-169: y * sigmoid(W2 SiLU(W1 m + b1) + b2), m the cumulative mean over CHANNELS (the reference
+    cumsums dim -2 of [B, C, T]); keys `net.0.*` [Ci, C, 1] and `net.2.*` [C, Ci, 1], Ci = max(8, C // 4).  Applied by
+    ResidualUnit, which adds the skip input in the same kernel."""
 
-    def __init__(self, chan_in, chan_out, dilation, kernel_size, pad_mode):
+    def __init__(self, dim, reduction_factor=4, dim_minimum=8):
+        super().__init__()
+        inner = max(dim_minimum, dim // reduction_factor)
+        self.net = nn.Sequential(nn.Conv1d(dim, inner, 1), nn.SiLU(), nn.Conv1d(inner, dim, 1), nn.Sigmoid())
+
+    def folded_weight(self):
+        """[Ci, C] first-conv weight with the cumulative mean folded in (ops.se_fold_weight), cached per weight version"""
+        return SoundStream._cached(self, "_folded", [self.net[0].weight], lambda: ops.se_fold_weight(self.net[0].weight))
+
+    def residual(self, y, x):
+        """x + SqueezeExcite(y) on fp32 [B, C, T] (csrc/codec.cu)"""
+        return ops.codec_se_fp32(y, x, self.folded_weight(), self.net[0].bias, self.net[2].weight, self.net[2].bias)
+
+
+class _RUBody(nn.Module):
+    """holds the two convs under the reference's Sequential indices 0 and 2 (1, 3 are ELUs) and, with squeeze_excite,
+    the SqueezeExcite under index 4."""
+
+    def __init__(self, chan_in, chan_out, dilation, kernel_size, pad_mode, squeeze_excite=False):
         super().__init__()
         self.add_module("0", CausalConv1d(chan_in, chan_out, kernel_size, dilation=dilation, pad_mode=pad_mode))
         self.add_module("2", CausalConv1d(chan_out, chan_out, 1, pad_mode=pad_mode))
+        if squeeze_excite:
+            self.add_module("4", SqueezeExcite(chan_out))
+
+
+def _se_of(ru):
+    return getattr(ru.fn, "4", None)
 
 
 class ResidualUnit(nn.Module):
-    """x + ELU(conv1(ELU(conv7_dil(x)))) (soundstream.py:362-369) in two fused launches; keys `fn.{0,2}.conv.*`."""
+    """x + SE(ELU(conv1(ELU(conv7_dil(x))))) (soundstream.py:362-369), SE = identity unless squeeze_excite; keys
+    `fn.{0,2}.conv.*` (and `fn.4.net.{0,2}.*`).  Two fused launches without SE, three with it."""
 
     def __init__(self, chan_in, chan_out, dilation, kernel_size=7, squeeze_excite=False, pad_mode="reflect"):
         super().__init__()
-        if squeeze_excite:
-            raise NotImplementedError("squeeze_excite=True is not built")
-        self.fn = _RUBody(chan_in, chan_out, dilation, kernel_size, pad_mode)
+        self.fn = _RUBody(chan_in, chan_out, dilation, kernel_size, pad_mode, squeeze_excite)
 
     def forward(self, x):
         c7, c1 = getattr(self.fn, "0"), getattr(self.fn, "2")
+        se = _se_of(self)
+        if se is not None:
+            return se.residual(c1(c7(x, elu=True), elu=True), x)
         C = x.shape[1]
         if (FUSE_RESIDUAL_UNITS and C in ops.RU_FUSED_CHANNELS and c7.dilation in ops.RU_FUSED_DILATIONS
                 and c7.conv.kernel_size[0] == 7 and c1.conv.kernel_size[0] == 1 and c7.conv.out_channels == C
@@ -279,7 +307,8 @@ class SoundStream(nn.Module):
     # ---- encoder on the tensor cores (csrc/codec_tc.cu) ------------------------------------------------
     def _tc_plan(self):
         """layer list for the split-bf16 tensor-core encoder, or None when this configuration is outside what those
-        kernels are built for (then the fp32 CUDA-core kernels run).  Structure follows soundstream.py:519-531."""
+        kernels are built for (then the fp32 CUDA-core kernels run).  Structure follows soundstream.py:519-531.  Units with
+        a SqueezeExcite take alm_codec_ru_se_tc."""
         if not (ENCODER_ON_TENSOR_CORES and self.single_channel):
             return None
         enc = list(self.encoder)
@@ -294,7 +323,8 @@ class SoundStream(nn.Module):
                 c7, c1 = getattr(ru.fn, "0"), getattr(ru.fn, "2")
                 C = c7.conv.in_channels
                 ok = ok and (C in (32, 64, 128, 256) and c7.conv.out_channels == C and c7.conv.kernel_size[0] == 7
-                             and c1.conv.kernel_size[0] == 1 and 6 * c7.dilation <= 54 and c7.stride == 1)
+                             and c1.conv.kernel_size[0] == 1 and 6 * c7.dilation <= 54 and c7.stride == 1
+                             and (_se_of(ru) is None or _se_of(ru).net[0].out_channels <= ops.se_inner_pad(C)))
             ok = ok and down.dilation == 1 and down.conv.in_channels % 16 == 0 and down.conv.out_channels % 64 == 0
             plan.append((rus, down))
         return (first, plan, last) if ok else None
@@ -309,6 +339,21 @@ class SoundStream(nn.Module):
             mod.__dict__[name] = hit
         return hit[1]
 
+    def _ru_tc(self, ru, h, out_phases=1):
+        """one residual unit on the tensor cores (C8S in and out); SE units take alm_codec_ru_se_tc"""
+        c7, c1 = getattr(ru.fn, "0"), getattr(ru.fn, "2")
+        se = _se_of(ru)
+        if se is None:
+            wu = self._cached(ru, "_tc_units", [c7.conv.weight, c1.conv.weight],
+                              lambda: ops.pack_ru_weights(c7.conv.weight, c1.conv.weight))
+            return ops.codec_ru_tc(h, wu, c7.conv.bias, c1.conv.bias, dilation=c7.dilation, pad_mode=c7.pad_mode,
+                                   out_phases=out_phases)
+        w1, w2 = se.net[0], se.net[2]
+        wu = self._cached(ru, "_tc_units_se", [c7.conv.weight, c1.conv.weight, w1.weight, w2.weight],
+                          lambda: ops.pack_ru_se_weights(c7.conv.weight, c1.conv.weight, w1.weight, w2.weight))
+        return ops.codec_ru_se_tc(h, wu, c7.conv.bias, c1.conv.bias, w1.bias, w2.bias, dilation=c7.dilation,
+                                  pad_mode=c7.pad_mode, out_phases=out_phases)
+
     def _encode_tc(self, wave, plan):
         """wave fp32 [B, T] -> encoder output fp32 [B, n, codebook_dim] (channels-last, what the RVQ consumes).
         Activations stay in the C8S split-bf16 layout between layers; every layer is one kernel launch."""
@@ -316,11 +361,7 @@ class SoundStream(nn.Module):
         h = ops.codec_first_conv(wave, first.conv.weight, first.conv.bias, pad_mode=first.pad_mode)
         for rus, down in blocks:
             for i, ru in enumerate(rus):
-                c7, c1 = getattr(ru.fn, "0"), getattr(ru.fn, "2")
-                wu = self._cached(ru, "_tc_units", [c7.conv.weight, c1.conv.weight],
-                                  lambda c7=c7, c1=c1: ops.pack_ru_weights(c7.conv.weight, c1.conv.weight))
-                h = ops.codec_ru_tc(h, wu, c7.conv.bias, c1.conv.bias, dilation=c7.dilation, pad_mode=c7.pad_mode,
-                                    out_phases=down.stride if i == len(rus) - 1 else 1)
+                h = self._ru_tc(ru, h, out_phases=down.stride if i == len(rus) - 1 else 1)
             if not rus:
                 raise NotImplementedError  # (guarded by _tc_plan: every block has residual units)
             wu = self._cached(down, "_tc_units", [down.conv.weight], lambda d=down: ops.pack_conv_weights(d.conv.weight))
@@ -349,7 +390,8 @@ class SoundStream(nn.Module):
                 c7, c1 = getattr(ru.fn, "0"), getattr(ru.fn, "2")
                 C = c7.conv.in_channels
                 ok = ok and (C in (32, 64, 128, 256) and c7.conv.out_channels == C and c7.conv.kernel_size[0] == 7
-                             and c1.conv.kernel_size[0] == 1 and 6 * c7.dilation <= 54 and c7.stride == 1)
+                             and c1.conv.kernel_size[0] == 1 and 6 * c7.dilation <= 54 and c7.stride == 1
+                             and (_se_of(ru) is None or _se_of(ru).net[0].out_channels <= ops.se_inner_pad(C)))
             plan.append((up, rus))
         return (first, plan, last) if ok else None
 
@@ -369,10 +411,7 @@ class SoundStream(nn.Module):
             h = ops.codec_conv_tc(h, wu, bias_up, cout=s_ * up.conv.out_channels, kernel_size=2, stride=1,
                                   pad_mode="constant", upsample=s_)
             for ru in rus:
-                c7, c1 = getattr(ru.fn, "0"), getattr(ru.fn, "2")
-                wr = self._cached(ru, "_tc_units", [c7.conv.weight, c1.conv.weight],
-                                  lambda c7=c7, c1=c1: ops.pack_ru_weights(c7.conv.weight, c1.conv.weight))
-                h = ops.codec_ru_tc(h, wr, c7.conv.bias, c1.conv.bias, dilation=c7.dilation, pad_mode=c7.pad_mode)
+                h = self._ru_tc(ru, h)
         return ops.codec_last_conv(h, last.conv.weight, last.conv.bias, pad_mode=last.pad_mode)
 
     def decode_frames(self, x):

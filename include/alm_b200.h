@@ -382,6 +382,15 @@ int alm_residual_unit_fwd(const float* x, const float* w7_packed, const float* b
                           const float* b1, float* y, int B, int C, int T, int dilation, int pad_mode,
                           alm_stream_t stream);
 /*
+ * SqueezeExcite of a ResidualUnit (soundstream.py:145-169, 362-369) on CUDA cores, for the configurations the
+ * tensor-core path does not cover.  y [B,C,T] = the unit's ELU(conv1(...)) output, x [B,C,T] its input:
+ *   out = x + y * sigmoid(w2 . silu(w1_folded . y + b1) + b2)   per time step,
+ * w1_folded [Ci,C] = the first 1x1 conv with the channel-wise cumulative mean folded in (ops.se_fold_weight),
+ * b1 [Ci], w2 [C,Ci], b2 [C]; all contiguous fp32.  (C + Ci) * 256 B of shared memory must fit in 200 KB.
+ */
+int alm_codec_se_fp32(const float* y, const float* x, const float* w1_folded, const float* b1, const float* w2,
+                      const float* b2, float* out, int B, int C, int Ci, int T, alm_stream_t stream);
+/*
  * SoundStream encoder on the tensor cores (csrc/codec_tc.cu): split-bf16 ("bf16x3": x_hi w_hi + x_lo w_hi + x_hi w_lo,
  * fp32 accumulation) implicit-GEMM causal convs.  Activations travel between these three calls in the "C8S" layout
  *   bf16 [B][2C/8][P][T/P][8]   (chunk c < C/8: hi halves of channels 8c..8c+7, chunk C/8 + c: their lo halves;
@@ -404,6 +413,17 @@ int alm_codec_ru_tc(const void* x, void* y, const void* w_units, const float* b7
                     int dilation, int pad_mode, int out_phases, alm_stream_t stream);
 int alm_codec_conv_tc(const void* x, void* y, const void* w_units, const float* bias, int B, int Cin, int Cout, int Tin,
                       int K, int stride, int pad_mode, int out_phases, int out_fp32, int upsample, alm_stream_t stream);
+/*
+ * alm_codec_ru_se_tc: ResidualUnit(squeeze_excite=True) (soundstream.py:145-169, 362-369), same operands and layout as
+ *   alm_codec_ru_tc plus the SqueezeExcite:  y = ELU(W1 ELU(W7 *_dil x + b7) + b1),
+ *   out = x + y * sigmoid(Ws2 SiLU(Ws1' y + se_b1) + se_b2),  Ws1'[i, c'] = sum_{c >= c'} Ws1[i, c] / (c + 1)
+ *   (the reference's cumulative mean runs over channels, so it folds into the first SE weight).  se_ci = the inner
+ *   width max(8, C / 4); se_b1 [se_ci], se_b2 [C] fp32.  w_units (ops.pack_ru_se_weights): the alm_codec_ru_tc units,
+ *   then Ws1' as [C/16][hi, lo][2][NS][8] and Ws2 as [NS/16][hi, lo][2][C][8], NS = max(32, C / 4) (zero-padded).
+ */
+int alm_codec_ru_se_tc(const void* x, void* y, const void* w_units, const float* b7, const float* b1, const float* se_b1,
+                       const float* se_b2, int B, int C, int se_ci, int T, int dilation, int pad_mode, int out_phases,
+                       alm_stream_t stream);
 /*
  * Decoder side (soundstream.py:347-360, 615-627).  CausalConvTranspose1d(Cin, C', 2s, stride s) runs as
  * alm_codec_conv_tc with K = 2, stride 1, constant padding, Cout = s * C' (ops.pack_convT_weights) and upsample = s:
