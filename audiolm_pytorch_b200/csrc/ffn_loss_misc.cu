@@ -303,6 +303,7 @@ geglu_ln_bwd_kernel(const __nv_bfloat16* __restrict__ h, long long ldh, int gate
 // ---- cross entropy: one CTA per row -----------------------------------------------------------
 // loss_rows[r] = lse - logit[label]  (0 when label == ignore)
 // dlogits[r, c] = (softmax - onehot) * (*scale_num) / (*scale_den)   as bf16 (0 row when ignored)
+// a label outside [0, V) that is not ignore_index gives a NaN loss and a NaN gradient row (columns < V)
 __global__ void __launch_bounds__(FF_THREADS)
 ce_fwd_bwd_kernel(const float* __restrict__ logits, long long ldl, const long long* __restrict__ labels,
                   long long ignore_index, float* __restrict__ loss_rows, __nv_bfloat16* __restrict__ dlogits,
@@ -313,6 +314,7 @@ ce_fwd_bwd_kernel(const float* __restrict__ logits, long long ldl, const long lo
   const float* row = logits + (size_t)r * ldl;
   const long long label = labels[r];
   const bool ignored = (label == ignore_index);
+  const bool bad_label = !ignored && (label < 0 || label >= V);
   float mx[1] = {-INFINITY};
   for (int c = threadIdx.x; c < V; c += FF_THREADS) mx[0] = fmaxf(mx[0], row[c]);
   // block max via the sum helper's buffer
@@ -330,9 +332,10 @@ ce_fwd_bwd_kernel(const float* __restrict__ logits, long long ldl, const long lo
   for (int c = threadIdx.x; c < V; c += FF_THREADS) sm[0] += __expf(row[c] - mx[0]);
   block_sum256<1>(sm, buf);
   const float lse = mx[0] + logf(sm[0]);
-  if (threadIdx.x == 0) loss_rows[r] = ignored ? 0.f : (lse - row[label]);
+  const float nan = __int_as_float(0x7fc00000);
+  if (threadIdx.x == 0) loss_rows[r] = ignored ? 0.f : bad_label ? nan : (lse - row[label]);
   if (dlogits != nullptr) {
-    const float sc = ignored ? 0.f : (*scale_num) / (*scale_den);
+    const float sc = ignored ? 0.f : bad_label ? nan : (*scale_num) / (*scale_den);
     __nv_bfloat16* drow = dlogits + (size_t)r * ldd;
     for (int c = threadIdx.x; c < Vpad; c += FF_THREADS) {
       float g = 0.f;

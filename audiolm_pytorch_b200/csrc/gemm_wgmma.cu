@@ -223,6 +223,8 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
     }
 
     // ===================== epilogue from the accumulator fragment =====================
+    // split-K: the bias is added once, by the split that owns k block 0
+    const float* bias = s == 0 ? p.bias : nullptr;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int gm = mb * GEMM_BLOCK_M + r_base + 8 * h;
@@ -230,16 +232,24 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
       const long long row_off = (long long)b * p.strideC + (long long)gm * p.ldc;
       // fused head + cross entropy: this row's state for the tile
       [[maybe_unused]] float ce_lse2 = 0.f, ce_scale = 0.f;
-      [[maybe_unused]] long long ce_label = -1;
+      [[maybe_unused]] long long ce_label = -1;  // the label's column, -1 when the label is not a column
       if constexpr (CE) {
+        bool bad_label = false;  // outside [0, N) and not ignore_index: its loss and gradient row are NaN
         if (row_ok) {
-          ce_label = p.ce_labels[gm];
+          const long long label = p.ce_labels[gm];
+          const bool in_range = label >= 0 && label < p.N;
+          ce_label = in_range ? label : -1;
+          bad_label = !in_range && label != p.ce_ignore;
           if (p.ce_mode == 2) {
             ce_lse2 = p.ce_lse[gm] * 1.4426950408889634f;
-            ce_scale = ce_label == p.ce_ignore ? 0.f : __ldg(p.ce_num) / __ldg(p.ce_den);
+            ce_scale = label == p.ce_ignore ? 0.f
+                       : bad_label      ? __int_as_float(0x7fc00000)
+                                        : __ldg(p.ce_num) / __ldg(p.ce_den);
           }
         }
         if (p.ce_mode == 1) {
+          // no tile holds a bad label's column: the first tile writes its NaN, so every row keeps exactly one writer
+          if (bad_label && nb == 0 && (lane & 3) == 0) p.ce_lab[gm] = __int_as_float(0x7fc00000);
           // row max / sum over the tile: each thread covers 2 columns per 8-column group, the 4 lanes of a quad the row
           float cm = -INFINITY;
 #pragma unroll
@@ -248,7 +258,7 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
             for (int c = 0; c < 2; ++c) {
               const int col = n0 + 8 * j + c_lane + c;
               float v = acc[4 * j + 2 * h + c] * p.alpha;
-              if (p.bias != nullptr && col < p.N) v += __ldg(p.bias + col);
+              if (bias != nullptr && col < p.N) v += __ldg(bias + col);
               if (row_ok && col == ce_label) p.ce_lab[gm] = v;
               v = col < p.N ? v * 1.4426950408889634f : -INFINITY;
               acc[4 * j + 2 * h + c] = v;
@@ -278,9 +288,9 @@ gemm_bf16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_con
         if (col >= p.N) break;
         float v0 = acc[4 * j + 2 * h] * p.alpha, v1 = acc[4 * j + 2 * h + 1] * p.alpha;
         const bool pair = col + 1 < p.N;
-        if (p.bias != nullptr) {
-          v0 += __ldg(p.bias + col);
-          if (pair) v1 += __ldg(p.bias + col + 1);
+        if (bias != nullptr) {
+          v0 += __ldg(bias + col);
+          if (pair) v1 += __ldg(bias + col + 1);
         }
         if constexpr (CE) {
           v0 = (exp2f(v0 * 1.4426950408889634f - ce_lse2) - (col == ce_label ? 1.f : 0.f)) * ce_scale;
@@ -344,6 +354,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUt
   return ALM_OK;
 }
 
+// (transformer.gemm_block_n keeps a host copy for best_split_k; tests/test_gemm_ce_envelope_gpu.py checks they agree)
 static int pick_block_n(int N) {
   if (N <= 64) return 64;
   if (N <= 128) return 128;

@@ -207,13 +207,17 @@ def pack_w1(w, inner):
     return out
 
 
+def gemm_block_n(N):
+    """BLOCK_N of alm_gemm_bf16 for N output columns: a copy of pick_block_n in csrc/gemm_wgmma.cu"""
+    return 64 if N <= 64 else (128 if N <= 128 or (-(-N // 128) * 128) * 10 < (-(-N // 256) * 256) * 9 else 256)
+
+
 def best_split_k(M, N, K, n_sm=None):
     """split-K factor for weight-gradient GEMMs (few output tiles, very long K); n_sm: SMs of the current device (132,
     the H100 SXM's count, when no device is present: the heuristic itself is host logic)."""
     if n_sm is None:
         n_sm = ops.num_sms() if torch.cuda.is_available() else 132
-    bn = 64 if N <= 64 else (128 if N <= 128 or (-(-N // 128) * 128) * 10 < (-(-N // 256) * 256) * 9 else 256)
-    tiles = -(-M // 128) * -(-N // bn)
+    tiles = -(-M // 128) * -(-N // gemm_block_n(N))
     kb = -(-K // 64)
     best, best_t = 1, None
     for s in range(1, min(64, kb) + 1):

@@ -46,6 +46,7 @@ void alm_reset_launch_count(void);
  *   a_mn = 1: A(m,k) = A[b*strideA + k*lda + m]   ("MN-major", e.g. dy^T for weight gradients)
  *   b_mn likewise for B(n,k).   c_fp32: 0 -> bf16 output, 1 -> fp32 output.
  *   acc_mode: 0 overwrite, 1 C += (read-modify-write), 2 C += with fp32 atomics (required when split_k > 1).
+ *   With split_k > 1 the bias is added once, by the split that owns the first k block.
  * Replaces every nn.Linear / einsum on the transformer path: audiolm_pytorch.py:255,259 (FFN),
  * :293-294,303 (q/kv/out projections), :621,798 (logit Linear), :972,979,1335,1350,1357 (grouped
  * logit einsums), and their autograd backward (dgrad: b_mn=1, wgrad: a_mn=b_mn=1).
@@ -211,11 +212,14 @@ int alm_decode_bias_row(const float* table, int rows, const float* override_h, c
  * (audiolm_pytorch.py:621, 798, 965-983, 1325-1361 heads; :1561-1565, 1836-1854, 2119-2137 losses).
  *   alm_gemm_head_ce mode 1 : X [M, K] bf16 (row stride ldx) times W [V, K] bf16 (row stride ldw) (+ bias [V] fp32); the GEMM
  *       epilogue reduces every (row, n tile) to {max, sum 2^(t - max)} of t = logit * log2(e) -> part [M, tiles, 2]
- *       (tiles = alm_gemm_head_ce_tiles(V)) and writes logit[label] -> lab_logit [M] (rows whose label is never a column,
- *       e.g. ignore_index = -1, are left untouched)
- *   alm_ce_finish           : part, lab_logit -> lse [M] (natural log), loss_rows [M] = lse - logit[label] (0 when ignored)
+ *       (tiles = alm_gemm_head_ce_tiles(V)) and writes logit[label] -> lab_logit [M].  A label outside [0, V) writes NaN
+ *       there unless it equals ignore_index (then lab_logit[r] is left untouched: alm_ce_finish does not read it)
+ *   alm_ce_finish           : part, lab_logit -> lse [M] (natural log), loss_rows [M] = lse - logit[label] (0 when ignored,
+ *       NaN for a label outside [0, V))
  *   alm_gemm_head_ce mode 2 : recomputes the GEMM and writes d loss / d logits = (softmax - onehot) * (*scale_num / *scale_den)
- *       as bf16 [M, ldd] (zero rows where label == ignore_index; columns >= V are not written: pre-zero the padding). */
+ *       as bf16 [M, ldd] (zero rows where label == ignore_index, NaN rows for a label outside [0, V); columns >= V are
+ *       not written: pre-zero the padding).
+ * alm_ce_fwd_bwd below treats labels the same way. */
 int alm_gemm_head_ce_tiles(int V);
 int alm_gemm_head_ce(const void* X, int64_t ldx, const void* W, int64_t ldw, const float* bias, const int64_t* labels,
                      int64_t ignore_index, int mode, float* part, float* lab_logit, const float* lse,
