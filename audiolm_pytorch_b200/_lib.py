@@ -78,6 +78,8 @@ SIGNATURES: dict[str, list] = {
     "alm_rvq_prepare": [P, L, P, P, L, P, I, I, P],
     "alm_rvq_select": [P, L, P, P, P, P, L, P, P, L, I, I, I, I, P],
     "alm_rvq_decode": [P, L, P, P, L, I, I, I, I, P],
+    "alm_sq_encode": [P, L, I, I, I, I, P, P, P, P, P, P, I, I, P, L, P, I, P],
+    "alm_sq_decode": [P, I, I, I, I, I, I, P, P, P, P, I, I, P, L, P],
 }
 
 

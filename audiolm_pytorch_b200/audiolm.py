@@ -734,7 +734,7 @@ class CoarseTransformerWrapper(nn.Module):
         with torch.inference_mode():
             self.codec.eval()
             _, indices, _ = self.codec(wave, return_encoded=True, input_sample_hz=input_sample_hz)
-        return indices
+        return indices.long()   # FSQ codecs emit int32 ids; labels and sampled sequences are int64
 
     @_eval_no_grad
     def generate(self, *, semantic_token_ids, prime_wave=None, prime_wave_input_sample_hz=None,
@@ -745,7 +745,7 @@ class CoarseTransformerWrapper(nn.Module):
         semantic_token_ids = semantic_token_ids.to(dev)
         assert not (exists(prime_wave) and exists(prime_coarse_token_ids))
         if exists(prime_coarse_token_ids):
-            coarse = prime_coarse_token_ids
+            coarse = prime_coarse_token_ids.long()
         elif exists(prime_wave):
             assert exists(self.codec)
             coarse = self._codec_ids(prime_wave, prime_wave_input_sample_hz)[..., :self.num_coarse_quantizers]
@@ -804,7 +804,7 @@ class CoarseTransformerWrapper(nn.Module):
             coarse_token_ids = indices[..., :self.num_coarse_quantizers]
         b = semantic_token_ids.shape[0]
         sem = semantic_token_ids.reshape(b, -1)
-        coarse = coarse_token_ids.reshape(b, -1)
+        coarse = coarse_token_ids.reshape(b, -1).long()
         if self.training:
             sem = append_eos_id(sem, self.transformer.semantic_eos_id)
             coarse = append_eos_id(coarse, self.transformer.coarse_eos_id)
@@ -868,16 +868,16 @@ class FineTransformerWrapper(nn.Module):
                  **kwargs):
         dev = self.device
         batch = coarse_token_ids.shape[0]
-        coarse = coarse_token_ids.reshape(batch, -1).to(dev)
+        coarse = coarse_token_ids.reshape(batch, -1).to(dev).long()
         assert not (exists(prime_wave) and exists(prime_fine_token_ids))
         if exists(prime_fine_token_ids):
-            fine = prime_fine_token_ids
+            fine = prime_fine_token_ids.long()
         elif exists(prime_wave):
             assert exists(self.codec)
             with torch.inference_mode():
                 self.codec.eval()
                 _, ids, _ = self.codec(prime_wave, return_encoded=True, input_sample_hz=prime_wave_input_sample_hz)
-            fine = ids[..., self.num_coarse_quantizers:].reshape(batch, -1)
+            fine = ids[..., self.num_coarse_quantizers:].reshape(batch, -1).long()
         else:
             fine = torch.empty((batch, 0), device=dev, dtype=torch.long)
         first = fine.shape[-1] // self.num_fine_quantizers
@@ -933,8 +933,8 @@ class FineTransformerWrapper(nn.Module):
             coarse_token_ids = token_ids[..., :self.num_coarse_quantizers]
             fine_token_ids = token_ids[..., self.num_coarse_quantizers:]
         b = coarse_token_ids.shape[0]
-        coarse = coarse_token_ids.reshape(b, -1)
-        fine = fine_token_ids.reshape(b, -1)
+        coarse = coarse_token_ids.reshape(b, -1).long()
+        fine = fine_token_ids.reshape(b, -1).long()
         if return_loss:
             coarse_labels, fine_labels = coarse, fine
             fine = fine[:, :-1]

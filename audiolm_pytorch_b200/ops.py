@@ -978,6 +978,75 @@ def rvq_decode(indices, codebooks):
     return out
 
 
+SQ_MODES = {"fsq": 0, "lfq": 1}
+
+
+def fsq_constants(levels, num_quantizers):
+    """per-dimension constants of residual FSQ as vector-quantize-pytorch computes them, in torch fp32 on the CPU:
+    (consts fp32 [4 + Q, dc] = half_l, offset, shift, L // 2, then scale[q] = (L - 1) ** -q; ints int32 [2, dc] =
+    levels, basis = cumprod([1, L_0, ..., L_{dc-2}])).  The kernels take these as they are, so the rounding boundaries
+    they quantize against are bit-identical to the quantizer's."""
+    lv = torch.tensor(levels, dtype=torch.int32)
+    half_l = (lv - 1) * (1 + 1e-3) / 2
+    offset = torch.where(lv % 2 == 0, 0.5, 0.0)
+    shift = (offset / half_l).atanh()
+    scales = torch.stack([(torch.tensor(levels, dtype=f32) - 1) ** -q for q in range(num_quantizers)])
+    basis = torch.cumprod(torch.tensor([1] + list(levels[:-1])), dim=0, dtype=torch.int32)
+    consts = torch.cat((torch.stack((half_l, offset, shift, (lv // 2).to(f32))), scales)).to(f32).contiguous()
+    return consts, torch.stack((lv, basis)).contiguous()
+
+
+def lfq_constants(codebook_dim, num_quantizers):
+    """the same layout for residual LFQ: scale[q] = 2 ** -q in every dimension, basis_j = 2 ** (dc - 1 - j) (most
+    significant bit first); the FSQ rows are unused (zero) and every level is 2."""
+    dc = codebook_dim
+    scales = torch.tensor([2.0 ** -q for q in range(num_quantizers)], dtype=f32)[:, None].expand(-1, dc)
+    consts = torch.cat((torch.zeros(4, dc, dtype=f32), scales)).contiguous()
+    basis = 2 ** torch.arange(dc - 1, -1, -1, dtype=torch.int32)
+    return consts, torch.stack((torch.full((dc,), 2, dtype=torch.int32), basis)).contiguous()
+
+
+def _sq_args(mode, groups, Dg, weights, consts, ints):
+    assert mode in SQ_MODES and consts.dtype == f32 and ints.dtype == torch.int32
+    dc, Q = consts.shape[1], consts.shape[0] - 4
+    assert weights is not None or Dg == dc, "the projections (Dg != dc) need their weights"
+    w_in, b_in, w_out_t, b_out = weights if Dg != dc else (None,) * 4
+    return dc, Q, w_in, b_in, w_out_t, b_out
+
+
+def sq_encode(x, *, mode, groups, weights, consts, ints, index_dtype):
+    """residual FSQ / LFQ (csrc/scalar_quant.cu): x [N, groups * Dg] fp32 (row stride free) -> (quantized [N, groups * Dg]
+    fp32, indices [groups, N, Q] of index_dtype, int32 or int64).  consts / ints from fsq_constants / lfq_constants on
+    x's device; weights = (w_in [g, dc, Dg], b_in [g, dc], w_out_t [g, dc, Dg], b_out [g, Dg]) fp32 contiguous, ignored
+    when Dg == dc (identity projections)."""
+    _check_cuda(x, consts, ints)
+    assert x.dtype == f32 and x.stride(-1) == 1 and x.shape[1] % groups == 0 and index_dtype in (torch.int32, torch.int64)
+    N, D = x.shape
+    Dg = D // groups
+    dc, Q, w_in, b_in, w_out_t, b_out = _sq_args(mode, groups, Dg, weights, consts, ints)
+    quant = torch.empty(N, D, device=x.device, dtype=f32)
+    idx = torch.empty(groups, N, Q, device=x.device, dtype=index_dtype)
+    with _timed("sq_encode", 4.0 * N * D * dc if Dg != dc else 0.0):
+        _lib.call("alm_sq_encode", x, x.stride(0), N, groups, Dg, SQ_MODES[mode], w_in, b_in, w_out_t, b_out, consts,
+                  ints, dc, Q, quant, D, idx, int(index_dtype == torch.int64))
+    return quant, idx
+
+
+def sq_decode(indices, *, mode, Dg, weights, consts, ints):
+    """get_output_from_indices of sq_encode's quantizer: indices [groups, N, q'] int32 / int64, q' <= Q, -1 = dropped
+    -> fp32 [N, groups * Dg] = project_out(sum of the codes).  Bit-identical to sq_encode's quantized on its own
+    indices."""
+    _check_cuda(indices, consts, ints)
+    assert indices.dtype in (torch.int32, torch.int64)
+    indices = indices.contiguous()
+    groups, N, Qi = indices.shape
+    dc, Q, _, _, w_out_t, b_out = _sq_args(mode, groups, Dg, weights, consts, ints)
+    out = torch.empty(N, groups * Dg, device=indices.device, dtype=f32)
+    _lib.call("alm_sq_decode", indices, int(indices.dtype == torch.int64), Qi, N, groups, Dg, SQ_MODES[mode], w_out_t,
+              b_out, consts, ints, dc, Q, out, groups * Dg)
+    return out
+
+
 def topk_gumbel_sample(logits, uniform, *, k, temperature=1.0):
     """ids [R] = Gumbel-max sample over the k largest logits of each row (noise supplied by the caller)."""
     _check_cuda(logits, uniform)

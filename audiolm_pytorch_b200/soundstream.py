@@ -1,14 +1,17 @@
-"""SoundStream codec inference path on libalm_b200 (sm_90a): causal conv encoder -> residual VQ -> decoder.
+"""SoundStream codec inference path on libalm_b200 (sm_90a): causal conv encoder -> residual quantizer -> decoder.
 
 Drop-in surface of /root/reference/audiolm_pytorch/soundstream.py:314-395, 451-866 for the calls the AudioLM
 hot path makes: `forward(x, return_encoded=True | return_codes_only=True | return_recons_only=True)`,
 `tokenize`, `decode_from_codebook_indices`, `decode`, with the reference's constructor kwargs and
-state_dict keys for `encoder.*`, `decoder.*`, `rq.*`.  GAN / mel training losses, LFQ / FSQ quantizers and
-FiLM denoising are outside this build; the local-attention bottleneck lives in local_attn.py.
+state_dict keys for `encoder.*`, `decoder.*`, `rq.*`.  The quantizer is the residual VQ, residual FSQ
+(`use_finite_scalar_quantizer`) or residual LFQ (`use_lookup_free_quantizer`), eval path only.  GAN / mel training
+losses, quantizer training and FiLM denoising are outside this build; the local-attention bottleneck lives in
+local_attn.py.
 """
 from __future__ import annotations
 
 import functools
+import math
 import pickle
 from itertools import cycle
 from pathlib import Path
@@ -209,6 +212,128 @@ class GroupedResidualVQ(nn.Module):
         return torch.cat([rvq.get_output_from_indices(i) for rvq, i in zip(self.rvqs, indices)], dim=-1)
 
 
+# ---- residual FSQ / LFQ (vector-quantize-pytorch GroupedResidualFSQ / GroupedResidualLFQ, eval path) -----------------
+# rq_kwargs that only shape training (quantize dropout, the LFQ losses); anything else changes what eval computes
+_SQ_TRAINING_KWARGS = {"quantize_dropout", "quantize_dropout_cutoff_index", "quantize_dropout_multiple_of"}
+_LFQ_TRAINING_KWARGS = _SQ_TRAINING_KWARGS | {"entropy_loss_weight", "commitment_loss_weight", "diversity_gamma"}
+
+
+class _ScalarQuantizerGroup(nn.Module):
+    """one group's ResidualFSQ / ResidualLFQ: `project_in` Linear(Dg, dc) and `project_out` Linear(dc, Dg), both
+    identities when Dg == dc.  They are its only persistent state."""
+
+    def __init__(self, dim, codebook_dim):
+        super().__init__()
+        proj = dim != codebook_dim
+        self.project_in = nn.Linear(dim, codebook_dim) if proj else nn.Identity()
+        self.project_out = nn.Linear(codebook_dim, dim) if proj else nn.Identity()
+
+
+class _GroupedScalarQuantizer(nn.Module):
+    """channels split into `groups`, each r = project_in(x); Q residual per-dimension quantizer stages; project_out.
+    All groups and stages run in one launch (ops.sq_encode, csrc/scalar_quant.cu)."""
+
+    mode = None
+    index_dtype = None
+
+    def __init__(self, *, dim, groups, num_quantizers, codebook_dim, constants, kwargs, allowed_kwargs):
+        super().__init__()
+        unknown = sorted(set(kwargs) - allowed_kwargs)
+        if unknown:
+            raise NotImplementedError(f"{type(self).__name__}: rq_kwargs {unknown} are outside this build")
+        if groups not in (1, 2, 4) or dim % groups:
+            raise NotImplementedError(f"{type(self).__name__}: groups={groups} with dim={dim} is outside this build "
+                                      "(groups 1, 2 or 4 dividing dim)")
+        if not 1 <= num_quantizers <= 32:
+            raise NotImplementedError(f"{type(self).__name__}: num_quantizers={num_quantizers} is outside this build (1..32)")
+        dg = dim // groups
+        if not (dg == codebook_dim or (dg % 4 == 0 and dg <= 1024)):
+            raise NotImplementedError(f"{type(self).__name__}: dim per group {dg} is outside this build (equal to the "
+                                      f"codebook dim {codebook_dim}, or a multiple of 4 up to 1024)")
+        self.groups = groups
+        self.num_quantizers = num_quantizers
+        self.codebook_dim = codebook_dim
+        self.dim_per_group = dg
+        self.rvqs = nn.ModuleList([_ScalarQuantizerGroup(dg, codebook_dim) for _ in range(groups)])
+        consts, ints = constants
+        self.register_buffer("sq_consts", consts, persistent=False)
+        self.register_buffer("sq_ints", ints, persistent=False)
+
+    def _weights(self):
+        """(w_in [g, dc, Dg], b_in [g, dc], w_out_t [g, dc, Dg], b_out [g, Dg]) fp32, cached per weight version"""
+        if self.dim_per_group == self.codebook_dim:
+            return None
+        params = [p_ for r in self.rvqs for p_ in (*r.project_in.parameters(), *r.project_out.parameters())]
+
+        def pack():
+            ins, outs = [r.project_in for r in self.rvqs], [r.project_out for r in self.rvqs]
+            return (torch.stack([m.weight.detach() for m in ins]).float().contiguous(),
+                    torch.stack([m.bias.detach() for m in ins]).float().contiguous(),
+                    torch.stack([m.weight.detach().t() for m in outs]).float().contiguous(),
+                    torch.stack([m.bias.detach() for m in outs]).float().contiguous())
+        return SoundStream._cached(self, "_sq_weights", params, pack)
+
+    def _encode(self, x):
+        if self.training:
+            raise NotImplementedError(f"{type(self).__name__} training (quantize dropout, aux losses) is outside this build")
+        b, n, d = x.shape
+        quant, idx = ops.sq_encode(x.reshape(b * n, d).to(f32), mode=self.mode, groups=self.groups,
+                                   weights=self._weights(), consts=self.sq_consts, ints=self.sq_ints,
+                                   index_dtype=self.index_dtype)
+        return quant.view(b, n, d), idx.view(self.groups, b, n, self.num_quantizers)
+
+    def get_output_from_indices(self, indices):
+        """indices [g, b, n, q'] (q' <= num_quantizers leading stages, -1 = dropped) -> [b, n, dim]"""
+        g, b, n, q = indices.shape
+        out = ops.sq_decode(indices.reshape(g, b * n, q), mode=self.mode, Dg=self.dim_per_group,
+                            weights=self._weights(), consts=self.sq_consts, ints=self.sq_ints)
+        return out.view(b, n, -1)
+
+
+class GroupedResidualFSQ(_GroupedScalarQuantizer):
+    """residual finite scalar quantization (arXiv 2309.15505) as soundstream.py:576-587 builds it; forward returns
+    (quantized, indices int32 [g, b, n, Q]), no loss.  codebook_size = prod(levels)."""
+
+    mode = "fsq"
+    index_dtype = torch.int32
+
+    def __init__(self, *, dim, levels, num_quantizers, groups=1, **kwargs):
+        levels = [int(l_) for l_ in levels]
+        if not 1 <= len(levels) <= 16 or min(levels) < 2 or math.prod(levels) >= 2 ** 31:
+            raise NotImplementedError(f"GroupedResidualFSQ: levels={levels} are outside this build (1 to 16 levels, each "
+                                      ">= 2, product below 2^31)")
+        super().__init__(dim=dim, groups=groups, num_quantizers=num_quantizers, codebook_dim=len(levels),
+                         constants=ops.fsq_constants(levels, num_quantizers), kwargs=kwargs,
+                         allowed_kwargs=_SQ_TRAINING_KWARGS)
+        self.levels = levels
+        self.codebook_size = math.prod(levels)
+
+    def forward(self, x):
+        return self._encode(x)
+
+
+class GroupedResidualLFQ(_GroupedScalarQuantizer):
+    """residual lookup-free quantization (arXiv 2310.05737) as soundstream.py:561-572 builds it; forward returns
+    (quantized, indices int64 [g, b, n, Q], aux losses [g, Q], zero in eval)."""
+
+    mode = "lfq"
+    index_dtype = torch.int64
+
+    def __init__(self, *, dim, num_quantizers, codebook_size, groups=1, **kwargs):
+        dc = int(codebook_size).bit_length() - 1
+        if codebook_size != 2 ** dc or not 1 <= dc <= 16:
+            raise NotImplementedError(f"GroupedResidualLFQ: codebook_size={codebook_size} is outside this build (a power "
+                                      "of two from 2 to 2^16)")
+        super().__init__(dim=dim, groups=groups, num_quantizers=num_quantizers, codebook_dim=dc,
+                         constants=ops.lfq_constants(dc, num_quantizers), kwargs=kwargs,
+                         allowed_kwargs=_LFQ_TRAINING_KWARGS)
+        self.codebook_size = codebook_size
+
+    def forward(self, x):
+        quant, idx = self._encode(x)
+        return quant, idx, torch.zeros(self.groups, self.num_quantizers, device=x.device)
+
+
 class SoundStream(nn.Module):
     """soundstream.py:451-866 (inference path)."""
 
@@ -231,9 +356,8 @@ class SoundStream(nn.Module):
         cfg.pop("self", None)
         cfg.pop("__class__", None)
         self._configs = pickle.dumps(cfg)
-        if use_lookup_free_quantizer or use_finite_scalar_quantizer or use_gate_loop_layers:
-            raise NotImplementedError("LFQ / FSQ / gate-loop variants are outside this build")
-        assert exists(codebook_size)
+        if use_gate_loop_layers:
+            raise NotImplementedError("gate-loop layers are outside this build")
         self.target_sample_hz = target_sample_hz
         self.single_channel = input_channels == 1
         self.strides = strides
@@ -251,12 +375,32 @@ class SoundStream(nn.Module):
         self.decoder_attn = LocalTransformer(**attn_kwargs) if use_local_attn else None
         self.num_quantizers = rq_num_quantizers
         self.codebook_dim = codebook_dim
-        self.codebook_size = codebook_size
         self.rq_groups = rq_groups
-        self.use_lookup_free_quantizer = False
-        self.use_finite_scalar_quantizer = False
-        self.rq = GroupedResidualVQ(dim=codebook_dim, num_quantizers=rq_num_quantizers, codebook_size=codebook_size,
-                                    groups=rq_groups)
+        # quantizer choice and its asserts as soundstream.py:555-609
+        assert not (use_lookup_free_quantizer and use_finite_scalar_quantizer)
+        self.use_lookup_free_quantizer = use_lookup_free_quantizer
+        self.use_finite_scalar_quantizer = use_finite_scalar_quantizer
+        rq_common = dict(dim=codebook_dim, num_quantizers=rq_num_quantizers, groups=rq_groups, quantize_dropout=True,
+                         quantize_dropout_cutoff_index=quantize_dropout_cutoff_index)
+        if use_lookup_free_quantizer:
+            assert exists(codebook_size) and not exists(finite_scalar_quantizer_levels), \
+                "if use_finite_scalar_quantizer is set to False, `codebook_size` must be set (and not " \
+                "`finite_scalar_quantizer_levels`)"
+            self.rq = GroupedResidualLFQ(codebook_size=codebook_size, **rq_common, **rq_kwargs)
+            self.codebook_size = codebook_size
+        elif use_finite_scalar_quantizer:
+            assert not exists(codebook_size) and exists(finite_scalar_quantizer_levels), \
+                "if use_finite_scalar_quantizer is set to True, `finite_scalar_quantizer_levels` must be set (and not " \
+                "`codebook_size`). the effective codebook size is the cumulative product of all the FSQ levels"
+            self.rq = GroupedResidualFSQ(levels=finite_scalar_quantizer_levels, **rq_common, **rq_kwargs)
+            self.codebook_size = self.rq.codebook_size
+        else:
+            assert exists(codebook_size) and not exists(finite_scalar_quantizer_levels), \
+                "if use_finite_scalar_quantizer is set to False, `codebook_size` must be set (and not " \
+                "`finite_scalar_quantizer_levels`)"
+            self.rq = GroupedResidualVQ(dim=codebook_dim, num_quantizers=rq_num_quantizers,
+                                        codebook_size=codebook_size, groups=rq_groups)
+            self.codebook_size = codebook_size
         self.decoder = nn.Sequential(
             CausalConv1d(codebook_dim, layer_channels[-1], 7, pad_mode=pad_mode),
             *[DecoderBlock(co, ci, s, dec_cycle_dilations, squeeze_excite, pad_mode)
@@ -452,7 +596,7 @@ class SoundStream(nn.Module):
         if quantized_indices.ndim == 3:
             b, n, gq = quantized_indices.shape
             quantized_indices = quantized_indices.reshape(b, n, self.rq_groups, -1).permute(2, 0, 1, 3)
-        return self.decode(self.rq.get_output_from_indices(quantized_indices.long()))
+        return self.decode(self.rq.get_output_from_indices(quantized_indices))
 
     def decode(self, x, quantize=False):
         if quantize:
@@ -475,7 +619,11 @@ class SoundStream(nn.Module):
         h = self.encode_frames(x)                                      # b n c
         if exists(self.encoder_attn):
             h = self.encoder_attn(h)
-        quantized, indices, commit_loss = self.rq(h)
+        if self.use_finite_scalar_quantizer:   # FSQ has no aux loss (soundstream.py:839-845)
+            quantized, indices = self.rq(h)
+            commit_loss = self.zero
+        else:
+            quantized, indices, commit_loss = self.rq(h)
         if return_codes_only:
             return indices
         if return_encoded:

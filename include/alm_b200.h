@@ -469,6 +469,34 @@ int alm_rvq_select(const float* scores, int64_t lds, const float* e2, const floa
 int alm_rvq_decode(const int64_t* indices, int64_t ldi, const float* codebooks, float* out, int64_t ldo, int N, int D,
                    int C, int Q, alm_stream_t stream);
 
+/*
+ * Residual FSQ / LFQ, eval path (vector-quantize-pytorch GroupedResidualFSQ / GroupedResidualLFQ as built at
+ * soundstream.py:563-587 and called at :839-845), csrc/scalar_quant.cu; mode 0 = FSQ, 1 = LFQ.  Per group g of width
+ * Dg (x [N, groups * Dg], row stride ldx): r = project_in(x_g); for q < Q: c = stage_q(r); r -= c; acc += c;
+ * quantized_g = project_out(acc); indices [groups, N, Q], int64 when idx64 else int32.
+ *   FSQ stage, per dimension j: z' = rint(tanh(r / scale[q][j] + shift) * half_l - offset), c = z' / (L // 2) * scale,
+ *       index = sum_j (z'_j + L_j // 2) * basis_j.
+ *   LFQ stage: c = r > 0 ? scale[q][j] : -scale[q][j], index = sum_j [r_j > 0] * basis_j (basis_j = 2^(dc-1-j)).
+ * consts fp32 [4 + Q, dc] = half_l, offset, shift, L // 2, scale[0..Q-1]; ints int32 [2, dc] = levels, basis (the
+ * caller computes both; FSQ levels must be >= 2 with a product below 2^31).  The projections exist iff Dg != dc:
+ * w_in [groups, dc, Dg], b_in [groups, dc], w_out_t [groups, dc, Dg] (project_out.weight transposed), b_out
+ * [groups, Dg]; with Dg == dc they are identities and may be null.
+ * Envelope: dc in 1..16, Q in 1..32, groups in {1, 2, 4}, Dg == dc or a multiple of 4 up to 1024; anything else is
+ * ALM_ERR_UNSUPPORTED.
+ */
+int alm_sq_encode(const float* x, int64_t ldx, int N, int groups, int Dg, int mode, const float* w_in, const float* b_in,
+                  const float* w_out_t, const float* b_out, const float* consts, const int32_t* ints, int dc, int Q,
+                  float* quantized, int64_t ldq, void* indices, int idx64, alm_stream_t stream);
+/*
+ * get_output_from_indices (soundstream.py:697) of the same quantizers: indices [groups, N, Qi] contiguous, int64 when
+ * idx64 else int32, the leading Qi <= Q stages (-1 = dropped; missing stages and -1 contribute no code) ->
+ * out [N, groups * Dg] (row stride ldo) = project_out(sum of codes).  The codes, their sum and project_out are the
+ * encoder's, so decoding alm_sq_encode's own indices returns its quantized output bit for bit.
+ */
+int alm_sq_decode(const void* indices, int idx64, int Qi, int N, int groups, int Dg, int mode, const float* w_out_t,
+                  const float* b_out, const float* consts, const int32_t* ints, int dc, int Q, float* out, int64_t ldo,
+                  alm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
