@@ -73,6 +73,8 @@ SIGNATURES: dict[str, list] = {
     "alm_codec_conv_tc": [P, P, P, P, I, I, I, I, I, I, I, I, I, I, P],
     "alm_codec_pack_c8s": [P, P, I, I, I, P],
     "alm_codec_last_conv": [P, P, P, P, I, I, I, I, I, P],
+    "alm_codec_gate_loop_fp32": [P, P, P, P, I, I, I, P],
+    "alm_codec_gate_loop_tc": [P, P, P, P, I, I, I, P],
     "alm_rvq_encode": [P, L, P, P, P, L, P, L, I, I, I, I, P],
     "alm_rvq_pack_codebooks": [P, P, P, L, I, P],
     "alm_rvq_prepare": [P, L, P, P, L, P, I, I, P],
@@ -110,6 +112,8 @@ def load() -> C.CDLL:
     lib.alm_decode_stack_scratch_bytes.argtypes = [I, I, I, I]
     lib.alm_gemm_head_ce_tiles.restype = I
     lib.alm_gemm_head_ce_tiles.argtypes = [I]
+    lib.alm_codec_gate_loop_workspace.restype = C.c_longlong
+    lib.alm_codec_gate_loop_workspace.argtypes = [I, I, I, I]
     lib.alm_decode_stack_grid.restype = I
     lib.alm_decode_stack_grid.argtypes = []
     lib.alm_decode_stack_plan.restype = I

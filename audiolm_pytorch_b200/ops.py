@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes
 import functools
+import math
 
 import torch
 
@@ -906,6 +907,67 @@ def codec_conv_tc(x, w_units, bias, *, cout, kernel_size, stride, pad_mode="refl
                   PAD_MODES[pad_mode], int(out_phases), int(out_fp32), int(upsample))
     return y
 
+
+
+# ---- gate-loop layer (csrc/codec_gate_loop.cu) --------------------------------------------------------
+def gate_loop_fold_weight(w, gamma):
+    """SimpleGateLoopLayer's to_qkva weight [3C, C] with its RMSNorm scale sqrt(C) * gamma folded into the columns ->
+    fp32 [3C, C], computed in fp64.  The norm's 1 / max(||u||, 1e-12) is per time step and stays in the kernel."""
+    w = w.detach().double()
+    C = w.shape[1]
+    return (w * (gamma.detach().double() * math.sqrt(C))[None, :]).float().contiguous()
+
+
+def gate_loop_slice(C):
+    """channels per CTA of alm_codec_gate_loop_tc (its q, kv and a are three m64nNSk16 accumulators)"""
+    return min(C, 64)
+
+
+def pack_gate_loop_weights(w_folded):
+    """folded [3C, C] -> the units alm_codec_gate_loop_tc streams: per channel slice of NS = gate_loop_slice(C), its q, kv
+    and a rows (3 NS) in the split-bf16 conv layout, bf16 [C/NS][C/16][hi, lo][2][3 NS][8]"""
+    C = w_folded.shape[1]
+    ns = gate_loop_slice(C)
+    rows = w_folded.detach().float().reshape(3, C // ns, ns, C).permute(1, 0, 2, 3).reshape(3 * C, C, 1)
+    return _split_units(rows, bn=3 * ns).reshape(C // ns, C // 16, 2, 2, 3 * ns, 8).contiguous()
+
+
+def _gate_loop_workspace(B, C, T, device, tc):
+    n = int(_lib.load().alm_codec_gate_loop_workspace(B, C, T, int(tc)))
+    return torch.empty(n, device=device, dtype=f32) if n else None
+
+
+def codec_gate_loop_fp32(x, w_folded):
+    """Residual(ChannelTranspose(SimpleGateLoopLayer)) on fp32 [B, C, T]: y = 2x + q * h.  The projection is
+    causal_conv1d with K = 1 on the folded weight; the norm, the gates and the scan are alm_codec_gate_loop_fp32."""
+    _check_cuda(x, w_folded)
+    x = x.contiguous()
+    B, C, T = x.shape
+    assert x.dtype == f32 and w_folded.shape == (3 * C, C)
+    proj = causal_conv1d(x, w_folded[:, :, None])
+    y = torch.empty_like(x)
+    with _timed("codec_gate_loop_fp32", 4.0 * B * T * 5 * C, "byte"):
+        _lib.call("alm_codec_gate_loop_fp32", x, proj, y, _gate_loop_workspace(B, C, T, x.device, False), B, C, T)
+    return y
+
+
+def codec_gate_loop_tc(x, w_units):
+    """Residual(ChannelTranspose(SimpleGateLoopLayer)) on C8S activations (P = 1 in and out), one fused kernel pair:
+    the split-bf16 projection on the tensor cores, the norm, the gates and the scan (alm_codec_gate_loop_tc);
+    w_units from pack_gate_loop_weights."""
+    _check_cuda(x, w_units)
+    B, nch2, P, T, _ = x.shape
+    C = nch2 * 4
+    ns = gate_loop_slice(C)
+    assert P == 1 and x.dtype == bf16 and x.is_contiguous()
+    assert w_units.dtype == bf16 and w_units.is_contiguous() and w_units.shape == (C // ns, C // 16, 2, 2, 3 * ns, 8)
+    y = torch.empty_like(x)
+    cls = "codec_gate_loop_tc"
+    if _PROFILE is not None and PROFILE_SHAPES:
+        cls += f" C{C} T{T}"
+    with _timed(cls, 8.0 * B * T * C, "byte"):
+        _lib.call("alm_codec_gate_loop_tc", x, w_units, y, _gate_loop_workspace(B, C, T, x.device, True), B, C, T)
+    return y
 
 def rvq_encode(x, codebooks):
     """x [N, D] fp32, codebooks [Q, C, D] fp32 -> (quantized [N, D] fp32, indices [N, Q] int64)."""

@@ -3,7 +3,7 @@
 Drop-in surface of /root/reference/audiolm_pytorch/soundstream.py:314-395, 451-866 for the calls the AudioLM
 hot path makes: `forward(x, return_encoded=True | return_codes_only=True | return_recons_only=True)`,
 `tokenize`, `decode_from_codebook_indices`, `decode`, with the reference's constructor kwargs and
-state_dict keys for `encoder.*`, `decoder.*`, `rq.*`.  The quantizer is the residual VQ, residual FSQ
+state_dict keys for `encoder.*`, `decoder.*`, `rq.*` (including the gate-loop layers of `use_gate_loop_layers`).  The quantizer is the residual VQ, residual FSQ
 (`use_finite_scalar_quantizer`) or residual LFQ (`use_lookup_free_quantizer`), eval path only.  GAN / mel training
 losses, quantizer training and FiLM denoising are outside this build; the local-attention bottleneck lives in
 local_attn.py.
@@ -28,6 +28,7 @@ f32 = torch.float32
 FUSE_RESIDUAL_UNITS = True  # False: conv7 + conv1 as two launches (A/B tests)
 RVQ_ON_TENSOR_CORES = True      # False: fp32 CUDA-core search kernel (A/B tests)
 ENCODER_ON_TENSOR_CORES = True  # False: fp32 CUDA-core conv kernels for the whole encoder (A/B tests)
+GATE_LOOP_TC_CHANNELS = (32, 64, 128, 256, 512)  # widths alm_codec_gate_loop_tc takes
 
 
 def exists(v):
@@ -144,6 +145,67 @@ def DecoderBlock(chan_in, chan_out, stride, cycle_dilations=(1, 3, 9), squeeze_e
     return nn.Sequential(CausalConvTranspose1d(chan_in, chan_out, 2 * stride, stride=stride),
                          *[ResidualUnit(chan_out, chan_out, next(it), squeeze_excite=squeeze_excite, pad_mode=pad_mode)
                            for _ in range(3)])
+
+
+class _RMSNorm(nn.Module):
+    """gateloop-transformer's RMSNorm: F.normalize(x, dim=-1) * sqrt(dim) * gamma; key `gamma` [dim]."""
+
+    def __init__(self, dim):
+        super().__init__()
+        self.gamma = nn.Parameter(torch.ones(dim))
+
+
+class GateLoop(nn.Module):
+    """SimpleGateLoopLayer(dim) of gateloop-transformer as the reference builds it (soundstream.py:29, 524-525, 620-621),
+    eval path: on u_t = x[:, :, t],  [q; kv; a]_t = W RMSNorm(u_t),  h_t = sigmoid(a_t) * h_{t-1} + kv_t,  out_t = q_t * h_t.
+    Keys `norm.gamma` [C] and `to_qkva.0.weight` [3C, C] (rows q, kv, a).  Runs only inside Residual(ChannelTranspose(.)),
+    whose two skip adds the kernels fuse: the block computes 2 x + q * h."""
+
+    def __init__(self, dim):
+        super().__init__()
+        self.norm = _RMSNorm(dim)
+        self.to_qkva = nn.Sequential(nn.Linear(dim, 3 * dim, bias=False))
+
+    def folded_weight(self):
+        """[3C, C] projection with sqrt(C) * gamma folded in (ops.gate_loop_fold_weight), cached per weight version"""
+        w = self.to_qkva[0].weight
+        return SoundStream._cached(self, "_folded", [w, self.norm.gamma],
+                                   lambda: ops.gate_loop_fold_weight(w, self.norm.gamma))
+
+    def block_fp32(self, x):
+        """Residual(ChannelTranspose(self)) on fp32 [B, C, T] (csrc/codec_gate_loop.cu)"""
+        return ops.codec_gate_loop_fp32(x.to(f32), self.folded_weight())
+
+    def block_tc(self, h):
+        """Residual(ChannelTranspose(self)) on C8S activations (P = 1), projection on the tensor cores"""
+        w = self.to_qkva[0].weight
+        units = SoundStream._cached(self, "_tc_units", [w, self.norm.gamma],
+                                    lambda: ops.pack_gate_loop_weights(ops.gate_loop_fold_weight(w, self.norm.gamma)))
+        return ops.codec_gate_loop_tc(h, units)
+
+
+class ChannelTranspose(nn.Module):
+    """soundstream.py:322-330 around a GateLoop: holds it under `fn`; its skip add runs in the gate-loop kernel."""
+
+    def __init__(self, fn):
+        super().__init__()
+        self.fn = fn
+
+
+class Residual(nn.Module):
+    """soundstream.py:314-320 around ChannelTranspose(GateLoop): keys `fn.fn.*`.  With ChannelTranspose's own skip add,
+    x enters the output twice (a reference quirk kept on purpose): Residual(ChannelTranspose(g))(x) = 2 x + g(x)."""
+
+    def __init__(self, fn):
+        super().__init__()
+        self.fn = fn
+
+    def forward(self, x):
+        return self.fn.fn.block_fp32(x)
+
+
+def _gate_loop_of(m):
+    return m.fn.fn if isinstance(m, Residual) else None
 
 
 # ---- residual VQ containers (state_dict keys of vector-quantize-pytorch) ---------------------------
@@ -356,16 +418,21 @@ class SoundStream(nn.Module):
         cfg.pop("self", None)
         cfg.pop("__class__", None)
         self._configs = pickle.dumps(cfg)
-        if use_gate_loop_layers:
-            raise NotImplementedError("gate-loop layers are outside this build")
         self.target_sample_hz = target_sample_hz
         self.single_channel = input_channels == 1
         self.strides = strides
         layer_channels = (channels, *[m * channels for m in channel_mults])
         pairs = tuple(zip(layer_channels[:-1], layer_channels[1:]))
+        # with use_gate_loop_layers a Residual(ChannelTranspose(GateLoop(C))) follows every block, on both sides
+        # (soundstream.py:522-525, 618-621), which shifts the later Sequential indices as in the reference
+        encoder_blocks = []
+        for (ci, co), s in zip(pairs, strides):
+            encoder_blocks.append(EncoderBlock(ci, co, s, enc_cycle_dilations, squeeze_excite, pad_mode))
+            if use_gate_loop_layers:
+                encoder_blocks.append(Residual(ChannelTranspose(GateLoop(co))))
         self.encoder = nn.Sequential(
             CausalConv1d(input_channels, channels, 7, pad_mode=pad_mode),
-            *[EncoderBlock(ci, co, s, enc_cycle_dilations, squeeze_excite, pad_mode) for (ci, co), s in zip(pairs, strides)],
+            *encoder_blocks,
             CausalConv1d(layer_channels[-1], codebook_dim, 3, pad_mode=pad_mode))
         attn_kwargs = dict(dim=codebook_dim, dim_head=attn_dim_head, heads=attn_heads, depth=attn_depth,
                            window_size=attn_window_size, xpos_scale_base=attn_xpos_scale_base,
@@ -401,10 +468,14 @@ class SoundStream(nn.Module):
             self.rq = GroupedResidualVQ(dim=codebook_dim, num_quantizers=rq_num_quantizers,
                                         codebook_size=codebook_size, groups=rq_groups)
             self.codebook_size = codebook_size
+        decoder_blocks = []
+        for (ci, co), s in zip(reversed(pairs), reversed(strides)):
+            decoder_blocks.append(DecoderBlock(co, ci, s, dec_cycle_dilations, squeeze_excite, pad_mode))
+            if use_gate_loop_layers:
+                decoder_blocks.append(Residual(ChannelTranspose(GateLoop(ci))))
         self.decoder = nn.Sequential(
             CausalConv1d(codebook_dim, layer_channels[-1], 7, pad_mode=pad_mode),
-            *[DecoderBlock(co, ci, s, dec_cycle_dilations, squeeze_excite, pad_mode)
-              for (ci, co), s in zip(reversed(pairs), reversed(strides))],
+            *decoder_blocks,
             CausalConv1d(channels, input_channels, 7, pad_mode=pad_mode))
         self.register_buffer("zero", torch.tensor(0.0), persistent=False)
 
@@ -452,7 +523,7 @@ class SoundStream(nn.Module):
     def _tc_plan(self):
         """layer list for the split-bf16 tensor-core encoder, or None when this configuration is outside what those
         kernels are built for (then the fp32 CUDA-core kernels run).  Structure follows soundstream.py:519-531.  Units with
-        a SqueezeExcite take alm_codec_ru_se_tc."""
+        a SqueezeExcite take alm_codec_ru_se_tc; a gate-loop layer after a block rides with that block's plan entry."""
         if not (ENCODER_ON_TENSOR_CORES and self.single_channel):
             return None
         enc = list(self.encoder)
@@ -462,6 +533,12 @@ class SoundStream(nn.Module):
               and last.conv.in_channels % 16 == 0 and last.conv.out_channels % 64 == 0)
         plan = []
         for blk in blocks if ok else ():
+            gl = _gate_loop_of(blk)
+            if gl is not None:
+                ok = ok and bool(plan) and plan[-1][2] is None and gl.norm.gamma.numel() in GATE_LOOP_TC_CHANNELS
+                if ok:
+                    plan[-1] = (*plan[-1][:2], gl)
+                continue
             *rus, down = list(blk)
             for ru in rus:
                 c7, c1 = getattr(ru.fn, "0"), getattr(ru.fn, "2")
@@ -470,7 +547,7 @@ class SoundStream(nn.Module):
                              and c1.conv.kernel_size[0] == 1 and 6 * c7.dilation <= 54 and c7.stride == 1
                              and (_se_of(ru) is None or _se_of(ru).net[0].out_channels <= ops.se_inner_pad(C)))
             ok = ok and down.dilation == 1 and down.conv.in_channels % 16 == 0 and down.conv.out_channels % 64 == 0
-            plan.append((rus, down))
+            plan.append((rus, down, None))
         return (first, plan, last) if ok else None
 
     @staticmethod
@@ -503,7 +580,7 @@ class SoundStream(nn.Module):
         Activations stay in the C8S split-bf16 layout between layers; every layer is one kernel launch."""
         first, blocks, last = plan
         h = ops.codec_first_conv(wave, first.conv.weight, first.conv.bias, pad_mode=first.pad_mode)
-        for rus, down in blocks:
+        for rus, down, gl in blocks:
             for i, ru in enumerate(rus):
                 h = self._ru_tc(ru, h, out_phases=down.stride if i == len(rus) - 1 else 1)
             if not rus:
@@ -511,6 +588,8 @@ class SoundStream(nn.Module):
             wu = self._cached(down, "_tc_units", [down.conv.weight], lambda d=down: ops.pack_conv_weights(d.conv.weight))
             h = ops.codec_conv_tc(h, wu, down.conv.bias, cout=down.conv.out_channels,
                                   kernel_size=down.conv.kernel_size[0], stride=down.stride, pad_mode=down.pad_mode)
+            if gl is not None:
+                h = gl.block_tc(h)
         wu = self._cached(last, "_tc_units", [last.conv.weight], lambda: ops.pack_conv_weights(last.conv.weight))
         return ops.codec_conv_tc(h, wu, last.conv.bias, cout=last.conv.out_channels,
                                  kernel_size=last.conv.kernel_size[0], stride=1, pad_mode=last.pad_mode, out_fp32=True)
@@ -527,6 +606,12 @@ class SoundStream(nn.Module):
               and last.conv.kernel_size[0] <= 8 and last.stride == 1 and last.dilation == 1)
         plan = []
         for blk in blocks if ok else ():
+            gl = _gate_loop_of(blk)
+            if gl is not None:
+                ok = ok and bool(plan) and plan[-1][2] is None and gl.norm.gamma.numel() in GATE_LOOP_TC_CHANNELS
+                if ok:
+                    plan[-1] = (*plan[-1][:2], gl)
+                continue
             up, *rus = list(blk)
             ok = ok and isinstance(up, CausalConvTranspose1d) and up.conv.in_channels % 16 == 0 \
                 and up.conv.out_channels % 16 == 0 and (up.upsample_factor * up.conv.out_channels) % 64 == 0
@@ -536,7 +621,7 @@ class SoundStream(nn.Module):
                 ok = ok and (C in (32, 64, 128, 256) and c7.conv.out_channels == C and c7.conv.kernel_size[0] == 7
                              and c1.conv.kernel_size[0] == 1 and 6 * c7.dilation <= 54 and c7.stride == 1
                              and (_se_of(ru) is None or _se_of(ru).net[0].out_channels <= ops.se_inner_pad(C)))
-            plan.append((up, rus))
+            plan.append((up, rus, None))
         return (first, plan, last) if ok else None
 
     def _decode_tc(self, x, plan):
@@ -546,7 +631,7 @@ class SoundStream(nn.Module):
         wu = self._cached(first, "_tc_units", [first.conv.weight], lambda: ops.pack_conv_weights(first.conv.weight))
         h = ops.codec_conv_tc(h, wu, first.conv.bias, cout=first.conv.out_channels,
                               kernel_size=first.conv.kernel_size[0], stride=1, pad_mode=first.pad_mode)
-        for up, rus in blocks:
+        for up, rus, gl in blocks:
             s_ = up.upsample_factor
             wu = self._cached(up, "_tc_units", [up.conv.weight],
                               lambda up=up, s_=s_: ops.pack_convT_weights(up.conv.weight, s_))
@@ -556,6 +641,8 @@ class SoundStream(nn.Module):
                                   pad_mode="constant", upsample=s_)
             for ru in rus:
                 h = self._ru_tc(ru, h)
+            if gl is not None:
+                h = gl.block_tc(h)
         return ops.codec_last_conv(h, last.conv.weight, last.conv.bias, pad_mode=last.pad_mode)
 
     def decode_frames(self, x):

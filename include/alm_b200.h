@@ -438,6 +438,24 @@ int alm_codec_ru_se_tc(const void* x, void* y, const void* w_units, const float*
 int alm_codec_pack_c8s(const float* x, void* y, int B, int n, int C, alm_stream_t stream);
 int alm_codec_last_conv(const void* x, const float* w, const float* bias, float* y, int B, int T, int Cin, int K,
                         int pad_mode, alm_stream_t stream);
+/*
+ * Gate-loop layer (SoundStream(use_gate_loop_layers=True): gateloop-transformer's SimpleGateLoopLayer inside the
+ * reference's Residual(ChannelTranspose(.)), soundstream.py:314-330, 524-525, 620-621), csrc/codec_gate_loop.cu.
+ * With u_t = x[:, :, t] and the folded weight W' = W diag(sqrt(C) gamma) [3C, C] (ops.gate_loop_fold_weight; rows q,
+ * kv, a) projecting P_t = W' u_t:
+ *   r_t = 1 / max(||u_t||_2, 1e-12),  h_t = sigmoid(r_t Pa_t) h_{t-1} + r_t Pkv_t (h_{-1} = 0),  y_t = 2 u_t + r_t Pq_t h_t.
+ * The scan is a fixed-order two-pass scan over time tiles: results are bitwise reproducible.  `workspace` holds
+ * alm_codec_gate_loop_workspace(B, C, T, tc) floats (0: may be null).
+ * alm_codec_gate_loop_tc:   x, y C8S (P = 1); the projection runs inside the kernel on the tensor cores (split bf16),
+ *                           w_units = ops.pack_gate_loop_weights(W'): bf16 [C/NS][C/16][hi, lo][2][3 NS][8], per
+ *                           channel slice of NS = min(C, 64) its q, kv and a rows; C in {32, 64, 128, 256, 512}, T >= 1.
+ * alm_codec_gate_loop_fp32: x, y fp32 [B][C][T], proj = P fp32 [B][3C][T] (alm_causal_conv1d_fwd, K = 1); C <= 1024.
+ */
+long long alm_codec_gate_loop_workspace(int B, int C, int T, int tc);
+int alm_codec_gate_loop_fp32(const float* x, const float* proj, float* y, float* workspace, int B, int C, int T,
+                             alm_stream_t stream);
+int alm_codec_gate_loop_tc(const void* x, const void* w_units, void* y, float* workspace, int B, int C, int T,
+                           alm_stream_t stream);
 int alm_causal_convT1d_fwd(const float* x, const float* w, const float* bias, float* y, int B, int Cin, int Cout,
                            int n, int stride, alm_stream_t stream);
 /*
