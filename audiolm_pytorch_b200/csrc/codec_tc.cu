@@ -69,39 +69,41 @@ __global__ void __launch_bounds__(128) first_conv_kernel(const float* __restrict
   for (int i = threadIdx.x; i < COUT * 8; i += blockDim.x) sw[i] = (i % 8) < K ? w[(i / 8) * K + (i % 8)] : 0.f;
   for (int i = threadIdx.x; i < COUT; i += blockDim.x) sb[i] = bias ? bias[i] : 0.f;
   __syncthreads();
-  const int b = blockIdx.y;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T) return;
   const int pad = K - 1;
-  float xv[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    xv[j] = 0.f;
-    if (j < K) {
-      int u = t + j - pad;  // x index of tap j
-      if (u < 0) {
-        if (pad_mode == 0) u = -u;                 // reflect (edge sample excluded)
-        else if (pad_mode == 2) u = 0;             // replicate
-        else u = -1;                               // constant zero
-      }
-      if (u >= 0) xv[j] = __ldg(x + (size_t)b * T + u);
-    }
-  }
   constexpr int NCH = COUT / 8;
-#pragma unroll 1
-  for (int c = 0; c < NCH; ++c) {
-    float v[8];
+  // grid.y is capped at 65535: a larger batch strides over it
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    float xv[8];
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      float acc = sb[c * 8 + e];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc = fmaf(sw[(c * 8 + e) * 8 + j], xv[j], acc);  // taps >= K: w = 0 and x = 0
-      v[e] = acc;
+    for (int j = 0; j < 8; ++j) {
+      xv[j] = 0.f;
+      if (j < K) {
+        int u = t + j - pad;  // x index of tap j
+        if (u < 0) {
+          if (pad_mode == 0) u = -u;                 // reflect (edge sample excluded)
+          else if (pad_mode == 2) u = 0;             // replicate
+          else u = -1;                               // constant zero
+        }
+        if (u >= 0) xv[j] = __ldg(x + (size_t)b * T + u);
+      }
     }
-    uint4 hi, lo;
-    split8(v, hi, lo);
-    *reinterpret_cast<uint4*>(y + c8s_off(b, c, t, 2 * NCH, 1, T)) = hi;
-    *reinterpret_cast<uint4*>(y + c8s_off(b, NCH + c, t, 2 * NCH, 1, T)) = lo;
+#pragma unroll 1
+    for (int c = 0; c < NCH; ++c) {
+      float v[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        float acc = sb[c * 8 + e];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc = fmaf(sw[(c * 8 + e) * 8 + j], xv[j], acc);  // taps >= K: w = 0 and x = 0
+        v[e] = acc;
+      }
+      uint4 hi, lo;
+      split8(v, hi, lo);
+      *reinterpret_cast<uint4*>(y + c8s_off(b, c, t, 2 * NCH, 1, T)) = hi;
+      *reinterpret_cast<uint4*>(y + c8s_off(b, NCH + c, t, 2 * NCH, 1, T)) = lo;
+    }
   }
 }
 
@@ -136,32 +138,34 @@ __global__ void __launch_bounds__(128) last_conv_kernel(const __nv_bfloat16* __r
   __shared__ float sw[CIN * 8];  // [ci][tap]
   for (int i = threadIdx.x; i < CIN * 8; i += blockDim.x) sw[i] = (i % 8) < K ? w[(i / 8) * K + (i % 8)] : 0.f;
   __syncthreads();
-  const int b = blockIdx.y;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= T) return;
   constexpr int NCH = CIN / 8;
   const int pad = K - 1;
-  float acc = bias ? bias[0] : 0.f;
-  for (int j = 0; j < K; ++j) {
-    int u = t + j - pad;
-    if (u < 0) {
-      if (pad_mode == 0) u = -u;
-      else if (pad_mode == 2) u = 0;
-      else continue;
-    }
+  // grid.y is capped at 65535: a larger batch strides over it
+  for (int b = blockIdx.y; b < B; b += gridDim.y) {
+    float acc = bias ? bias[0] : 0.f;
+    for (int j = 0; j < K; ++j) {
+      int u = t + j - pad;
+      if (u < 0) {
+        if (pad_mode == 0) u = -u;
+        else if (pad_mode == 2) u = 0;
+        else continue;
+      }
 #pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-      const uint4 h = __ldg(reinterpret_cast<const uint4*>(x + c8s_off(b, c, u, 2 * NCH, 1, T)));
-      const uint4 l = __ldg(reinterpret_cast<const uint4*>(x + c8s_off(b, NCH + c, u, 2 * NCH, 1, T)));
-      const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lw[4] = {l.x, l.y, l.z, l.w};
+      for (int c = 0; c < NCH; ++c) {
+        const uint4 h = __ldg(reinterpret_cast<const uint4*>(x + c8s_off(b, c, u, 2 * NCH, 1, T)));
+        const uint4 l = __ldg(reinterpret_cast<const uint4*>(x + c8s_off(b, NCH + c, u, 2 * NCH, 1, T)));
+        const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lw[4] = {l.x, l.y, l.z, l.w};
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        acc = fmaf(sw[(c * 8 + 2 * e) * 8 + j], bf16_lo(hw[e]) + bf16_lo(lw[e]), acc);
-        acc = fmaf(sw[(c * 8 + 2 * e + 1) * 8 + j], bf16_hi(hw[e]) + bf16_hi(lw[e]), acc);
+        for (int e = 0; e < 4; ++e) {
+          acc = fmaf(sw[(c * 8 + 2 * e) * 8 + j], bf16_lo(hw[e]) + bf16_lo(lw[e]), acc);
+          acc = fmaf(sw[(c * 8 + 2 * e + 1) * 8 + j], bf16_hi(hw[e]) + bf16_hi(lw[e]), acc);
+        }
       }
     }
+    y[(size_t)b * T + t] = acc;
   }
-  y[(size_t)b * T + t] = acc;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -891,7 +895,7 @@ extern "C" int alm_codec_first_conv(const float* x, const float* w, const float*
   ALM_REQUIRE(x && w && y && B > 0 && T > 0, ALM_ERR_ARG);
   ALM_REQUIRE(K >= 1 && K <= 8 && pad_mode >= 0 && pad_mode <= 2, ALM_ERR_UNSUPPORTED);
   ALM_REQUIRE(T > K - 1, ALM_ERR_ARG);
-  dim3 grid(ceil_div(T, 128), B);
+  dim3 grid(ceil_div(T, 128), min(B, 65535));
   __nv_bfloat16* yy = reinterpret_cast<__nv_bfloat16*>(y);
   if (Cout == 32) ctc::first_conv_kernel<32><<<grid, 128, 0, stream>>>(x, w, bias, yy, B, T, K, pad_mode);
   else if (Cout == 64) ctc::first_conv_kernel<64><<<grid, 128, 0, stream>>>(x, w, bias, yy, B, T, K, pad_mode);
@@ -1008,7 +1012,7 @@ extern "C" int alm_codec_last_conv(const void* x, const float* w, const float* b
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ALM_REQUIRE(x && w && y && B > 0 && T > 0, ALM_ERR_ARG);
   ALM_REQUIRE(K >= 1 && K <= 8 && pad_mode >= 0 && pad_mode <= 2 && T > K - 1, ALM_ERR_UNSUPPORTED);
-  dim3 grid(ceil_div(T, 128), B);
+  dim3 grid(ceil_div(T, 128), min(B, 65535));
   const __nv_bfloat16* xx = reinterpret_cast<const __nv_bfloat16*>(x);
   if (Cin == 32) ctc::last_conv_kernel<32><<<grid, 128, 0, stream>>>(xx, w, bias, y, B, T, K, pad_mode);
   else if (Cin == 64) ctc::last_conv_kernel<64><<<grid, 128, 0, stream>>>(xx, w, bias, y, B, T, K, pad_mode);

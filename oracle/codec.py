@@ -69,7 +69,8 @@ def encoder(st, x, strides=(2, 4, 5, 8), dilations=(1, 3, 9), pad_mode="reflect"
     for bi, s in enumerate(strides, start=1):
         for ri, d in enumerate(dilations):
             x = residual_unit(sub(st, f"{bi}.{ri}"), x, d, pad_mode)
-        x = causal_conv1d(x, st[f"{bi}.3.conv.weight"], st[f"{bi}.3.conv.bias"], stride=s, pad_mode=pad_mode)
+        # the reference's EncoderBlock builds its strided conv without pad_mode: always reflect
+        x = causal_conv1d(x, st[f"{bi}.3.conv.weight"], st[f"{bi}.3.conv.bias"], stride=s)
     last = len(strides) + 1
     return causal_conv1d(x, st[f"{last}.conv.weight"], st[f"{last}.conv.bias"], pad_mode=pad_mode)
 

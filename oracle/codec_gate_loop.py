@@ -82,7 +82,8 @@ def encoder(st, x, strides=(2, 4, 5, 8), dilations=(1, 3, 9), pad_mode="reflect"
         blk = sub(st, f"{2 * i + 1}")
         for ri, d in enumerate(dilations):
             x = ose.residual_unit(sub(blk, f"{ri}"), x, d, pad_mode)
-        x = oc.causal_conv1d(x, blk["3.conv.weight"], blk["3.conv.bias"], stride=s, pad_mode=pad_mode)
+        # the reference's EncoderBlock builds its strided conv without pad_mode: always reflect
+        x = oc.causal_conv1d(x, blk["3.conv.weight"], blk["3.conv.bias"], stride=s)
         x = gate_loop_block(sub(st, f"{2 * i + 2}"), x)
     last = 2 * len(strides) + 1
     return oc.causal_conv1d(x, st[f"{last}.conv.weight"], st[f"{last}.conv.bias"], pad_mode=pad_mode)

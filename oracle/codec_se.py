@@ -20,7 +20,7 @@ from .transformer import sub
 def squeeze_excite(st, y):
     """SqueezeExcite(C) on y [b, C, t] with keys net.0.{weight,bias} [Ci, C, 1], net.2.{weight,bias} [C, Ci, 1]."""
     C = y.shape[-2]
-    m = y.cumsum(dim=-2) / torch.arange(1, C + 1, dtype=y.dtype)[:, None]       # mean over channels 0..c
+    m = y.cumsum(dim=-2) / torch.arange(1, C + 1, dtype=y.dtype, device=y.device)[:, None]  # mean over channels 0..c
     s = F.silu(torch.einsum("ic,bct->bit", st["net.0.weight"][..., 0], m) + st["net.0.bias"][:, None])
     gate = torch.sigmoid(torch.einsum("ci,bit->bct", st["net.2.weight"][..., 0], s) + st["net.2.bias"][:, None])
     return y * gate
@@ -41,7 +41,8 @@ def encoder(st, x, strides=(2, 4, 5, 8), dilations=(1, 3, 9), pad_mode="reflect"
     for bi, s in enumerate(strides, start=1):
         for ri, d in enumerate(dilations):
             x = residual_unit(sub(st, f"{bi}.{ri}"), x, d, pad_mode)
-        x = oc.causal_conv1d(x, st[f"{bi}.3.conv.weight"], st[f"{bi}.3.conv.bias"], stride=s, pad_mode=pad_mode)
+        # the reference's EncoderBlock builds its strided conv without pad_mode: always reflect
+        x = oc.causal_conv1d(x, st[f"{bi}.3.conv.weight"], st[f"{bi}.3.conv.bias"], stride=s)
     last = len(strides) + 1
     return oc.causal_conv1d(x, st[f"{last}.conv.weight"], st[f"{last}.conv.bias"], pad_mode=pad_mode)
 
