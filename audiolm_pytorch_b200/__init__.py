@@ -8,10 +8,11 @@ __version__ = "0.2.0"
 
 from .audiolm import (AudioLM, CoarseTransformer, CoarseTransformerWrapper, FineTransformer,  # noqa: E402,F401
                       FineTransformerWrapper, SemanticTransformer, SemanticTransformerWrapper)
+from .hubert import HubertWithKmeans  # noqa: E402,F401
 from .parallel import FlatGradBucket  # noqa: E402,F401
 from .soundstream import AudioLMSoundStream, MusicLMSoundStream, SoundStream  # noqa: E402,F401
 from .transformer import Transformer  # noqa: E402,F401
 
 __all__ = ["AudioLM", "SemanticTransformer", "CoarseTransformer", "FineTransformer", "SemanticTransformerWrapper",
            "CoarseTransformerWrapper", "FineTransformerWrapper", "SoundStream", "AudioLMSoundStream",
-           "MusicLMSoundStream", "Transformer", "FlatGradBucket"]
+           "MusicLMSoundStream", "Transformer", "FlatGradBucket", "HubertWithKmeans"]

@@ -82,6 +82,13 @@ SIGNATURES: dict[str, list] = {
     "alm_rvq_decode": [P, L, P, P, L, I, I, I, I, P],
     "alm_sq_encode": [P, L, I, I, I, I, P, P, P, P, P, P, I, I, P, L, P, I, P],
     "alm_sq_decode": [P, I, I, I, I, I, I, P, P, P, P, I, I, P, L, P],
+    "alm_hubert_conv0": [P, P, P, P, I, I, I, I, I, P],
+    "alm_hubert_chan_stats": [P, P, I, I, I, P],
+    "alm_hubert_norm_act": [P, P, I, P, L, P, P, I, P, P, L, I, P],
+    "alm_hubert_add_ln": [P, P, I, I, P, I, P, P, I, P, P, L, I, P],
+    "alm_hubert_pos_pack": [P, P, I, I, I, I, I, I, P],
+    "alm_hubert_qkv_heads": [P, P, P, P, I, I, I, I, P],
+    "alm_hubert_merge_heads": [P, P, I, I, I, I, P],
 }
 
 

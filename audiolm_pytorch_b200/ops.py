@@ -1141,3 +1141,119 @@ def resid_ln_bwd(r_new, gamma, stats, dr_out, dxn, dextra, g_gamma, *, out_scale
     dr_b = torch.empty(M, d, device=r_new.device, dtype=bf16) if want_bf16 else None
     _lib.call("alm_resid_ln_bwd", r_new, gamma, stats, dr_out, dxn, dextra, dr, dr_b, g_gamma, float(out_scale), M, d)
     return dr, dr_b
+
+
+# ---- HuBERT feature path (csrc/hubert.cu; the network itself is audiolm_pytorch_b200/hubert.py) ----------------------
+def pack_split_weight(w):
+    """fp32 weight [N, K] -> bf16 [N, 3K] = [w_hi | w_hi | w_lo], the B operand of a split-bf16 GEMM against activation
+    rows [x_hi | x_lo | x_hi] (the packing of rvq_pack_codebooks)"""
+    return rvq_pack_codebooks(w[None])[1][0]
+
+
+def pack_split_conv_weight(w):
+    """conv weight [Cout, Cin, k] -> bf16 [Cout, k * 3 Cin]: per output channel, the k taps' packed rows in tap order,
+    matching a window of k split rows of the input"""
+    Cout, Cin, k = w.shape
+    return pack_split_weight(w.permute(0, 2, 1).reshape(Cout * k, Cin)).view(Cout, k * 3 * Cin)
+
+
+def split_gemm(xs, w_packed, bias=None, cls="hubert_gemm"):
+    """fp32 [..., N] = x @ w^T (+ bias) for x in the split layout xs [..., 3K] and w_packed = pack_split_weight(w)"""
+    lead = xs.shape[:-1]
+    out = gemm(xs.reshape(-1, xs.shape[-1]), w_packed, out_dtype=f32, bias=bias, cls=cls)
+    return out.view(*lead, w_packed.shape[0])
+
+
+def hubert_conv_gemm(xs, w_packed, bias, *, kernel_size, stride, cls="hubert_conv_gemm"):
+    """strided conv over the split layout xs [B, T, 3C] -> fp32 [B, T_out, Cout], one GEMM per clip whose A rows
+    overlap: output row t reads the kernel_size * 3C elements from row t * stride.  w_packed = pack_split_conv_weight(w).
+    (Clips run as separate GEMMs because every clip shares the weight, which the batched GEMM would need as a stride-0
+    operand.)"""
+    B, T, C3 = xs.shape
+    assert xs.is_contiguous()
+    T_out = (T - kernel_size) // stride + 1
+    a = xs.as_strided((B, T_out, kernel_size * C3), (T * C3, stride * C3, 1))
+    out = torch.empty(B, T_out, w_packed.shape[0], device=xs.device, dtype=f32)
+    for b in range(B):
+        gemm(a[b], w_packed, out=out[b], bias=bias, cls=cls)
+    return out
+
+
+def hubert_pos_conv(x, w_packed, *, kernel_size, cls="hubert_pos_gemm"):
+    """grouped positional conv (padding kernel_size // 2, the first T outputs kept) of x fp32 [B, T, D], without its
+    bias: per clip one GEMM batched over the groups, from the zero-padded group-major split copy (alm_hubert_pos_pack)
+    with overlapping A rows.  w_packed: [groups, D / groups, kernel_size * 3 D / groups] (per group
+    pack_split_conv_weight).  -> fp32 [B, groups, T, D / groups]"""
+    _check_cuda(x, w_packed)
+    B, T, D = x.shape
+    G, Dg, Kp = w_packed.shape
+    k = kernel_size
+    Tp = T + k - 1
+    xp = torch.empty(B, G, Tp, 3 * Dg, device=x.device, dtype=bf16)
+    _lib.call("alm_hubert_pos_pack", x, xp, B, T, D, G, k // 2, Tp)
+    out = torch.empty(B, G, T, Dg, device=x.device, dtype=f32)
+    for b in range(B):
+        a = xp[b].as_strided((G, T, Kp), (Tp * 3 * Dg, 3 * Dg, 1))
+        gemm(a, w_packed, out=out[b], cls=cls)
+    return out
+
+
+def hubert_conv0(wave, w, bias, *, stride):
+    """first conv of the feature extractor: wave fp32 [B, T], w [C, 1, K] (+ bias [C]) -> fp32 [B, T1, C]"""
+    _check_cuda(wave, w, bias)
+    B, T = wave.shape
+    C, _, K = w.shape
+    y = torch.empty(B, (T - K) // stride + 1, C, device=wave.device, dtype=f32)
+    _lib.call("alm_hubert_conv0", wave, w, bias, y, B, T, C, K, stride)
+    return y
+
+
+def hubert_chan_stats(y):
+    """GroupNorm(C, C) statistics of y fp32 [B, T, C] over time -> fp32 [B, C, 2] = {mean, 1 / sqrt(var + 1e-5)}"""
+    B, T, C = y.shape
+    stats = torch.empty(B, C, 2, device=y.device, dtype=f32)
+    _lib.call("alm_hubert_chan_stats", y, stats, B, T, C)
+    return stats
+
+
+def hubert_norm_act(y, *, bias=None, stats=None, ln=False, gamma=None, beta=None, gelu=False, want_out=False,
+                    want_split=True):
+    """per row of y fp32 [..., C]: (+ bias), GroupNorm (stats from hubert_chan_stats, y [B, T, C]) or LayerNorm (ln),
+    gamma / beta, GELU -> (fp32 [..., C] or None, split bf16 [..., 3C] or None)"""
+    _check_cuda(y, bias, stats, gamma, beta)
+    C = y.shape[-1]
+    M = y.numel() // C
+    mode = 1 if stats is not None else 2 if ln else 0
+    want_out = want_out or (mode == 2 and bias is not None)
+    out = torch.empty_like(y) if want_out else None
+    split = torch.empty(*y.shape[:-1], 3 * C, device=y.device, dtype=bf16) if want_split else None
+    _lib.call("alm_hubert_norm_act", y, bias, mode, stats, y.shape[1] if mode == 1 else 0, gamma, beta, int(gelu), out,
+              split, M, C)
+    return out, split
+
+
+def hubert_add_ln(r, y=None, *, T, groups=1, y_bias=None, y_gelu=False, gamma=None, beta=None, keep_ln=False,
+                  want_split=True):
+    """in place on the residual stream r fp32 [B * T, D] (or [B, T, D]): r_new = r + act(y + y_bias); with gamma,
+    LayerNorm(r_new) gamma + beta goes to the returned split bf16 [..., 3D] and, if keep_ln, into r"""
+    _check_cuda(r, y, y_bias, gamma, beta)
+    D = r.shape[-1]
+    split = torch.empty(*r.shape[:-1], 3 * D, device=r.device, dtype=bf16) if (want_split and gamma is not None) else None
+    _lib.call("alm_hubert_add_ln", r, y, groups, T, y_bias, int(y_gelu), gamma, beta, int(keep_ln), r, split,
+              r.numel() // D, D)
+    return split
+
+
+def hubert_attention(qkv, *, heads):
+    """multi-head self-attention (no mask, not causal) on the bf16 attention kernel: qkv fp32 [B, T, 3D] (q | k | v,
+    biases included) -> the merged heads in the split layout bf16 [B, T, 3D], for the output projection"""
+    _check_cuda(qkv)
+    B, T, D3 = qkv.shape
+    D = D3 // 3
+    dh = D // heads
+    q, k, v = (torch.empty(B * heads, T, dh, device=qkv.device, dtype=bf16) for _ in range(3))
+    _lib.call("alm_hubert_qkv_heads", qkv, q, k, v, B, T, D, heads)
+    o, _ = mqa_attn_fwd(q, k, v, heads=1, causal=False, scale=dh ** -0.5, return_lse=False)
+    split = torch.empty(B, T, 3 * D, device=qkv.device, dtype=bf16)
+    _lib.call("alm_hubert_merge_heads", o, split, B, T, D, heads)
+    return split

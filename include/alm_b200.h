@@ -515,6 +515,42 @@ int alm_sq_decode(const void* indices, int idx64, int Qi, int N, int groups, int
                   const float* b_out, const float* consts, const int32_t* ints, int dc, int Q, float* out, int64_t ldo,
                   alm_stream_t stream);
 
+/*
+ * HuBERT feature path (fairseq HubertModel.extract_features(mask=False, output_layer=L) as called by HubertWithKmeans,
+ * hubert_kmeans.py:107-112), csrc/hubert.cu: the fp32 kernels between the network's GEMMs.  Every conv and linear runs
+ * on alm_gemm_bf16 in split bf16: activation rows in the "split layout" bf16 [rows, 3C] = [x_hi | x_lo | x_hi] against
+ * weight rows [w_hi | w_hi | w_lo] (alm_rvq_pack_codebooks).  A conv of kernel k and stride s over a split
+ * [B, T, 3C] tensor is one GEMM whose A rows overlap: row t starts at t * s * 3C and is k * 3C long.  Norms use eps 1e-5;
+ * GELU is the erf form; reductions run in a fixed order without atomics, so a clip's outputs are bitwise reproducible
+ * and do not depend on the other clips of the batch.
+ *   alm_hubert_conv0        y fp32 [B, T1, C] = conv(wave [B, T], w [C, K], stride) (+ bias [C]), T1 = (T - K) / stride + 1
+ *   alm_hubert_chan_stats   stats fp32 [B, C, 2] = {mean, 1 / sqrt(var + eps)} over time of y [B, T, C] (GroupNorm(C, C))
+ *   alm_hubert_norm_act     per row m of y [M, C]: v = y (+ bias); mode 1: GroupNorm with stats of batch m / rows_per_batch;
+ *                           mode 2: LayerNorm over the row (with a bias, `out` receives the biased row first); then
+ *                           gamma, beta; GELU if gelu -> out fp32 [M, C] and / or split bf16 [M, 3C] (either may be null)
+ *   alm_hubert_add_ln       r_new = r + act(y + y_bias) (y optional: [M, D], or the grouped conv output
+ *                           [B, groups, T, D / groups] when groups > 1; act = GELU if y_gelu); without gamma r_out = r_new,
+ *                           else ln = LayerNorm(r_new) gamma + beta -> split (optional) and r_out = keep_ln ? ln : r_new.
+ *                           M = B * T; r_out may alias r.
+ *   alm_hubert_pos_pack     xp bf16 [B, groups, Tp, 3 D / groups] = split layout of x [B, T, D] per group, row p holding
+ *                           time p - pad (zeros outside [0, T)): the A operand of the grouped positional conv.
+ *   alm_hubert_qkv_heads    qkv fp32 [B, T, 3D] -> q, k, v bf16 [B, heads, T, D / heads] (attention with batch B * heads)
+ *   alm_hubert_merge_heads  o bf16 [B, heads, T, D / heads] -> split bf16 [B, T, 3D] = [o | 0 | o] of the merged heads
+ */
+int alm_hubert_conv0(const float* wave, const float* w, const float* bias, float* y, int B, int T, int C, int K,
+                     int stride, alm_stream_t stream);
+int alm_hubert_chan_stats(const float* y, float* stats, int B, int T, int C, alm_stream_t stream);
+int alm_hubert_norm_act(const float* y, const float* bias, int mode, const float* stats, int64_t rows_per_batch,
+                        const float* gamma, const float* beta, int gelu, float* out, void* split, int64_t M, int C,
+                        alm_stream_t stream);
+int alm_hubert_add_ln(const float* r, const float* y, int groups, int T, const float* y_bias, int y_gelu,
+                      const float* gamma, const float* beta, int keep_ln, float* r_out, void* split, int64_t M, int D,
+                      alm_stream_t stream);
+int alm_hubert_pos_pack(const float* x, void* xp, int B, int T, int D, int groups, int pad, int Tp, alm_stream_t stream);
+int alm_hubert_qkv_heads(const float* qkv, void* q, void* k, void* v, int B, int T, int D, int heads,
+                         alm_stream_t stream);
+int alm_hubert_merge_heads(const void* o, void* split, int B, int T, int D, int heads, alm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
