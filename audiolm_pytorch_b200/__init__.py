@@ -8,6 +8,7 @@ __version__ = "0.2.0"
 
 from .audiolm import (AudioLM, CoarseTransformer, CoarseTransformerWrapper, FineTransformer,  # noqa: E402,F401
                       FineTransformerWrapper, SemanticTransformer, SemanticTransformerWrapper)
+from .encodec import EncodecWrapper  # noqa: E402,F401
 from .hubert import HubertWithKmeans  # noqa: E402,F401
 from .parallel import FlatGradBucket  # noqa: E402,F401
 from .soundstream import AudioLMSoundStream, MusicLMSoundStream, SoundStream  # noqa: E402,F401
@@ -15,4 +16,4 @@ from .transformer import Transformer  # noqa: E402,F401
 
 __all__ = ["AudioLM", "SemanticTransformer", "CoarseTransformer", "FineTransformer", "SemanticTransformerWrapper",
            "CoarseTransformerWrapper", "FineTransformerWrapper", "SoundStream", "AudioLMSoundStream",
-           "MusicLMSoundStream", "Transformer", "FlatGradBucket", "HubertWithKmeans"]
+           "MusicLMSoundStream", "Transformer", "FlatGradBucket", "HubertWithKmeans", "EncodecWrapper"]

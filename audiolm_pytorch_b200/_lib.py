@@ -89,6 +89,10 @@ SIGNATURES: dict[str, list] = {
     "alm_hubert_pos_pack": [P, P, I, I, I, I, I, I, P],
     "alm_hubert_qkv_heads": [P, P, P, P, I, I, I, I, P],
     "alm_hubert_merge_heads": [P, P, I, I, I, I, P],
+    "alm_encodec_pad1d": [P, P, L, I, I, I, P],
+    "alm_encodec_resblock_fp32": [P, P, P, P, P, P, P, I, I, I, I, P],
+    "alm_encodec_lstm": [P, P, P, P, P, I, I, I, I, P],
+    "alm_encodec_resblock_tc": [P, P, P, P, P, I, I, I, I, I, P],
 }
 
 
@@ -121,6 +125,8 @@ def load() -> C.CDLL:
     lib.alm_gemm_head_ce_tiles.argtypes = [I]
     lib.alm_codec_gate_loop_workspace.restype = C.c_longlong
     lib.alm_codec_gate_loop_workspace.argtypes = [I, I, I, I]
+    lib.alm_encodec_lstm_workspace.restype = C.c_longlong
+    lib.alm_encodec_lstm_workspace.argtypes = [I, I]
     lib.alm_decode_stack_grid.restype = I
     lib.alm_decode_stack_grid.argtypes = []
     lib.alm_decode_stack_plan.restype = I

@@ -87,6 +87,31 @@ __device__ __forceinline__ void gelu_parts(float x, float& cdf, float& xpdf) {
   xpdf = 0.3989422804014327f * x * e;
 }
 
+__device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {
+  unsigned v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+
+// Device-wide barrier: monotonic arrival counter, red.release / ld.acquire at gpu scope (the CTA's own writes are ordered
+// before the release by the __syncthreads).  A bounded spin (about 2 s) turns a lost CTA into an error flag instead of a
+// hung GPU.
+__device__ __forceinline__ void grid_barrier(unsigned* counter, unsigned& epoch, int* err) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    epoch += gridDim.x;
+    asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
+    const long long t0 = clock64();
+    while (ld_acquire(counter) < epoch) {
+      if (clock64() - t0 > 4000000000LL) {
+        *err = 1;
+        break;
+      }
+    }
+  }
+  __syncthreads();
+}
+
 // ---- dropout mask ------------------------------------------------------------------------------
 // Every dropout decision of the library is keep(seed, site, row, col): a pure function of its arguments, so the
 // backward regenerates the forward's mask instead of storing it.  Coordinates: elementwise sites on an [M, C]

@@ -22,6 +22,7 @@
 //   ru_tc_kernel<C, SE>    fused ResidualUnit: y = x + ELU(W1 ELU(W7 *_d x + b7) + b1); the k=7 result goes
 //                          registers -> (bias, ELU, split) -> shared memory as the bf16 A operand of the 1x1 conv.
 //                          SE = true adds the unit's SqueezeExcite (soundstream.py:145-169) as two more GEMMs per tile
+//                          RB = true: EnCodec's SEANet resnet block instead (EncodecWrapper; see RuCfg)
 //   conv_tc_kernel<..>     strided / plain causal conv as a pipelined implicit GEMM over (tap, k-step) units
 // Activation tiles are staged with 16-B cp.async by whole producer warps, weights with large bulk copies.
 #include "alm_common.cuh"
@@ -218,17 +219,26 @@ struct RuParams {
   const float* se_b1 = nullptr;  // SE only: biases of the two 1x1 convs ([se_ci], [C])
   const float* se_b2 = nullptr;
   int se_ci = 0;
+  int elu_out = 0;  // RB only: ELU on the block's output
 };
 
-template <int C, bool SE = false>
+// RB = true: EnCodec's SEANet resnet block (EncodecWrapper) on the same pipeline,
+//   y = [W1 | Ws] . [ELU(W3 *_k3 ELU(x) + b3) ; x] + b1 + bs   (ELU'd when elu_out), C -> C/2 -> C.
+// The staged tile is raw x; the consumers write ELU(x) (re-split) into the sA2 region, which D1 reads; E1 then
+// overwrites sA2 with the hidden activations.  D1 runs with N = C (W3's rows zero-padded from C/2), so the units, the
+// accumulator and E1 are the ResidualUnit's; D2 runs K over the hidden k-steps (A = sA2) and then the shortcut's
+// k-steps (A = the staged raw x, shifted by the 2-row halo), so the 1x1 shortcut folds into the second product.
+// Units: 3 W3 taps, W1 (columns zero-padded from C/2), Ws: 5 KSTEPS.  The staged tile is released after D2.
+template <int C, bool SE = false, bool RB = false>
 struct RuCfg {
   static constexpr int NCHUNK = C / 8;
   static constexpr int KSTEPS = C / 16;
   static constexpr bool RESIDENT = C <= 64;       // all weights stay in shared memory for the CTA's lifetime
   static constexpr int UNIT_BYTES = 2 * 2 * C * 16;  // hi [2 chunks][C][16 B] + lo
-  static constexpr int NUNITS = 8 * KSTEPS;
+  static constexpr int NUNITS = (RB ? 5 : 8) * KSTEPS;
   static constexpr int MAX_NW = 16;
-  static constexpr int A2_BYTES = 2 * NCHUNK * RU_TILE_M * 16;  // E1 output: [hi / lo][chunk][64 rows][16 B]
+  // E1 output: [hi / lo][chunk][64 rows][16 B]; RB: first ELU(x) with the 2-row halo
+  static constexpr int A2_BYTES = 2 * NCHUNK * (RU_TILE_M + (RB ? 2 : 0)) * 16;
   // squeeze-excite: inner width padded to NS (a multiple of 16, >= 32 for the smallest wgmma tile in use)
   static constexpr int NS = SE ? (C / 4 > 32 ? C / 4 : 32) : 0;
   static constexpr int SE1_UNIT_BYTES = 2 * 2 * NS * 16;  // one k-step of W1': hi / lo [2 chunks][NS][16 B]
@@ -254,9 +264,10 @@ struct RuCfg {
   }
 };
 
-template <int C, bool SE>
-__global__ void __launch_bounds__(RU_THREADS, RuCfg<C, SE>::CTAS_PER_SM) ru_tc_kernel(const RuParams p) {
-  using Cfg = RuCfg<C, SE>;
+template <int C, bool SE, bool RB>
+__global__ void __launch_bounds__(RU_THREADS, RuCfg<C, SE, RB>::CTAS_PER_SM) ru_tc_kernel(const RuParams p) {
+  using Cfg = RuCfg<C, SE, RB>;
+  constexpr int TAPS = RB ? 3 : 7;
   constexpr int NCHUNK = Cfg::NCHUNK, KSTEPS = Cfg::KSTEPS;
   constexpr bool RESIDENT = Cfg::RESIDENT;
   const int NA = p.na, NW = p.nw, A_ROWS = p.ar;
@@ -295,7 +306,7 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C, SE>::CTAS_PER_SM) ru_tc_k
   }
   __syncthreads();
 
-  const int halo = 6 * p.d;
+  const int halo = (TAPS - 1) * p.d;
   auto tile_of = [&](int i) { return (int)blockIdx.x + i * (int)gridDim.x; };
   auto has = [&](int i) { return i >= 0 && tile_of(i) < p.total_tiles; };
 
@@ -397,7 +408,7 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C, SE>::CTAS_PER_SM) ru_tc_k
         if constexpr (SE) {
           if (lane == 0) stream_se_units(0, Cfg::ALL_UNITS);
         } else {
-          if (lane == 0) stream_units(0, 8 * KSTEPS);
+          if (lane == 0) stream_units(0, Cfg::NUNITS);
         }
         __syncwarp();
         if (NA == 1 && has(i + 1)) issue_a(i + 1);
@@ -447,16 +458,37 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C, SE>::CTAS_PER_SM) ru_tc_k
   for (int i = 0; has(i); ++i) {
     const int ab = i % NA;
     mbar_wait(&a_full[ab], ((uint32_t)(i / NA)) & 1u);
+    if constexpr (RB) {
+      // ---- ELU(x) of the staged tile (halo included) -> sA2, same [hi / lo][chunk][A_ROWS][16 B] layout ----
+      const uint8_t* src = sA + ab * A_BYTES;
+      for (int e = threadIdx.x - 128; e < NCHUNK * A_ROWS; e += 128) {
+        const uint4 h = *reinterpret_cast<const uint4*>(src + e * 16);
+        const uint4 l = *reinterpret_cast<const uint4*>(src + (NCHUNK * A_ROWS + e) * 16);
+        const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lw[4] = {l.x, l.y, l.z, l.w};
+        float v[8];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          v[2 * k] = elu1(bf16_lo(hw[k]) + bf16_lo(lw[k]));
+          v[2 * k + 1] = elu1(bf16_hi(hw[k]) + bf16_hi(lw[k]));
+        }
+        uint4 oh, ol;
+        split8(v, oh, ol);
+        *reinterpret_cast<uint4*>(sA2 + e * 16) = oh;
+        *reinterpret_cast<uint4*>(sA2 + (NCHUNK * A_ROWS + e) * 16) = ol;
+      }
+      fence_proxy_async_smem();  // generic-proxy writes -> wgmma operand reads
+      asm volatile("bar.sync 1, 128;" ::: "memory");
+    }
     // ---- D1 = W7 *_d x: 7 taps x KSTEPS units, three bf16 products each (x_hi w_hi + x_lo w_hi + x_hi w_lo) ----
     float d[C / 2];
     {
-      const uint32_t a_addr = smem_u32(sA + ab * A_BYTES);
+      const uint32_t a_addr = RB ? a2_addr : smem_u32(sA + ab * A_BYTES);
       // descriptors are built once; between MMAs only the 14-bit start-address field (>> 4) of the low word moves
       const uint64_t a_hi0 = wgmma_desc_nosw(a_addr, 128, A_ROWS * 16);
       const uint64_t a_lo0 = wgmma_desc_nosw(a_addr + NCHUNK * (A_ROWS * 16), 128, A_ROWS * 16);
       const uint32_t kstep_units = 2 * A_ROWS;       // two chunks, in 16-B units
 #pragma unroll 1
-      for (int j = 0; j < 7; ++j) {
+      for (int j = 0; j < TAPS; ++j) {
         const uint32_t row_units = (uint32_t)(j * p.d);
 #pragma unroll
         for (int kk = 0; kk < KSTEPS; ++kk) {
@@ -473,7 +505,8 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C, SE>::CTAS_PER_SM) ru_tc_k
       drain();
       wgmma_fence_acc(d);
     }
-    if (lane == 0) mbar_arrive(&a_empty[ab]);  // the staged tile may be overwritten
+    if (!RB && lane == 0) mbar_arrive(&a_empty[ab]);  // the staged tile may be overwritten
+    if constexpr (RB) asm volatile("bar.sync 1, 128;" ::: "memory");  // every warp's D1 reads of ELU(x) have retired
     // ---- E1: D1 (+b7, ELU, split) -> sA2, [hi / lo][chunk][64 rows][16 B] ----
 #pragma unroll
     for (int j = 0; j < C / 8; ++j)
@@ -491,7 +524,7 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C, SE>::CTAS_PER_SM) ru_tc_k
     // ---- D2 = W1 ELU(D1 + b7): A from sA2 ----
 #pragma unroll
     for (int kk = 0; kk < KSTEPS; ++kk) {
-      const uint64_t b_hi = unit_b(7 * KSTEPS + kk);
+      const uint64_t b_hi = unit_b((TAPS) * KSTEPS + kk);
       const uint64_t b_lo = b_hi + (uint64_t)(2 * C);
       const uint32_t a_off = a2_addr + kk * 2 * (RU_TILE_M * 16);
       const uint64_t a_hi = wgmma_desc_nosw(a_off, 128, RU_TILE_M * 16);
@@ -502,8 +535,26 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C, SE>::CTAS_PER_SM) ru_tc_k
       wgmma_ss<C>(d, a_hi, b_lo, 1u);
       unit_done();
     }
+    if constexpr (RB) {
+      // ---- shortcut: D2 += Ws x, A = the staged raw x from row `halo` on ----
+      const uint32_t a_addr = smem_u32(sA + ab * A_BYTES);
+      const uint64_t a_hi0 = wgmma_desc_nosw(a_addr, 128, A_ROWS * 16);
+      const uint64_t a_lo0 = wgmma_desc_nosw(a_addr + NCHUNK * (A_ROWS * 16), 128, A_ROWS * 16);
+#pragma unroll
+      for (int kk = 0; kk < KSTEPS; ++kk) {
+        const uint64_t b_hi = unit_b(4 * KSTEPS + kk);
+        const uint64_t b_lo = b_hi + (uint64_t)(2 * C);
+        const uint64_t off = (uint64_t)(kk * 2 * A_ROWS + halo);
+        wgmma_fence();
+        wgmma_ss<C>(d, a_hi0 + off, b_hi, 1u);
+        wgmma_ss<C>(d, a_lo0 + off, b_hi, 1u);
+        wgmma_ss<C>(d, a_hi0 + off, b_lo, 1u);
+        unit_done();
+      }
+    }
     drain();
     wgmma_fence_acc(d);
+    if (RB && lane == 0) mbar_arrive(&a_empty[ab]);  // the staged tile may be overwritten
     const int tile = tile_of(i);
     const int b = tile / p.tiles_per_clip;
     const int t0 = (tile - b * p.tiles_per_clip) * RU_TILE_M;
@@ -593,6 +644,27 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C, SE>::CTAS_PER_SM) ru_tc_k
           *reinterpret_cast<uint32_t*>(p.y + ya.off + (size_t)(NCHUNK + j) * ya.chunk_stride + c_lane) = ol;
         }
       }
+    } else if constexpr (RB) {
+      // ---- E2: D2 + (b1 + bs) (ELU if elu_out) -> split -> global (C8S) ----
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int t = t0 + rl + 8 * h;
+        if (t >= p.T) continue;
+        const RowAddr ya = c8s_row(b, t, 2 * NCHUNK, p.out_phases, p.T);
+#pragma unroll
+        for (int j = 0; j < C / 8; ++j) {
+          const int col = 8 * j + c_lane;
+          float v0 = d[4 * j + 2 * h] + sBias[C + col], v1 = d[4 * j + 2 * h + 1] + sBias[C + col + 1];
+          if (p.elu_out) {
+            v0 = elu1(v0);
+            v1 = elu1(v1);
+          }
+          uint32_t oh, ol;
+          split_bf16x2(v0, v1, oh, ol);
+          *reinterpret_cast<uint32_t*>(p.y + ya.off + (size_t)j * ya.chunk_stride + c_lane) = oh;
+          *reinterpret_cast<uint32_t*>(p.y + ya.off + (size_t)(NCHUNK + j) * ya.chunk_stride + c_lane) = ol;
+        }
+      }
     } else {
       // ---- E2: D2 (+b1, ELU, + skip) -> split -> global (C8S) ----
 #pragma unroll
@@ -620,11 +692,11 @@ __global__ void __launch_bounds__(RU_THREADS, RuCfg<C, SE>::CTAS_PER_SM) ru_tc_k
   }
 }
 
-template <int C, bool SE = false>
+template <int C, bool SE = false, bool RB = false>
 static int launch_ru(RuParams p, cudaStream_t stream) {
-  using Cfg = RuCfg<C, SE>;
-  auto kfn = ru_tc_kernel<C, SE>;
-  p.ar = RU_TILE_M + 6 * p.d;
+  using Cfg = RuCfg<C, SE, RB>;
+  auto kfn = ru_tc_kernel<C, SE, RB>;
+  p.ar = RU_TILE_M + (RB ? 2 : 6 * p.d);
   const int a_bytes = 2 * Cfg::NCHUNK * p.ar * 16;
   int smem;
   if (Cfg::RESIDENT) {
@@ -991,6 +1063,31 @@ extern "C" int alm_codec_conv_tc(const void* x, void* y, const void* w_units, co
   if (BN == 256) return ctc::launch_conv<256>(p, stream);
   if (BN == 128) return ctc::launch_conv<128>(p, stream);
   return ctc::launch_conv<64>(p, stream);
+}
+
+extern "C" int alm_encodec_resblock_tc(const void* x, void* y, const void* w_units, const float* b3, const float* b_out,
+                                       int B, int C, int T, int elu_out, int out_phases, alm_stream_t stream_) {
+  using namespace alm;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ALM_REQUIRE(x && y && w_units && b3 && b_out && B > 0, ALM_ERR_ARG);
+  ALM_REQUIRE(T > 2, ALM_ERR_ARG);  // the reflect halo of the k3 conv
+  ALM_REQUIRE(out_phases >= 1 && T % out_phases == 0, ALM_ERR_ARG);
+  ctc::RuParams p;
+  p.x = reinterpret_cast<const __nv_bfloat16*>(x);
+  p.y = reinterpret_cast<__nv_bfloat16*>(y);
+  p.w = reinterpret_cast<const __nv_bfloat16*>(w_units);
+  p.b7 = b3;
+  p.b1 = b_out;
+  p.B = B; p.T = T; p.d = 1; p.pad_mode = 0; p.out_phases = out_phases; p.elu_out = elu_out;
+  p.tiles_per_clip = ceil_div(T, ctc::RU_TILE_M);
+  p.total_tiles = p.tiles_per_clip * B;
+  switch (C) {
+    case 32: return ctc::launch_ru<32, false, true>(p, stream);
+    case 64: return ctc::launch_ru<64, false, true>(p, stream);
+    case 128: return ctc::launch_ru<128, false, true>(p, stream);
+    case 256: return ctc::launch_ru<256, false, true>(p, stream);
+    default: return ALM_ERR_UNSUPPORTED;
+  }
 }
 
 extern "C" int alm_codec_pack_c8s(const float* x, void* y, int B, int n, int C, alm_stream_t stream_) {

@@ -130,34 +130,10 @@ __device__ __forceinline__ float ld_bf16_cg(const __nv_bfloat16* p) {
   asm volatile("ld.global.cg.u16 %0, [%1];" : "=h"(u) : "l"(p));
   return __uint_as_float((uint32_t)u << 16);
 }
-__device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
 __device__ __forceinline__ float bf16r(float v) { return __bfloat162float(__float2bfloat16(v)); }
 template <typename T>
 __device__ __forceinline__ T* tptr(const unsigned long long* lp, int i) {
   return reinterpret_cast<T*>(lp[i]);
-}
-
-// Device-wide barrier: monotonic arrival counter, red.release / ld.acquire at gpu scope (the CTA's own writes are ordered
-// before the release by the __syncthreads).  A bounded spin (about 2 s) turns a lost CTA into an error flag instead of a
-// hung GPU.
-__device__ __forceinline__ void grid_barrier(unsigned* counter, unsigned& epoch, int* err) {
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    epoch += gridDim.x;
-    asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
-    const long long t0 = clock64();
-    while (ld_acquire(counter) < epoch) {
-      if (clock64() - t0 > 4000000000LL) {
-        *err = 1;
-        break;
-      }
-    }
-  }
-  __syncthreads();
 }
 
 // 32 values per lane -> lane L holds the warp total of value L (31 shuffles instead of 160)

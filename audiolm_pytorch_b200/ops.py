@@ -1040,6 +1040,104 @@ def rvq_decode(indices, codebooks):
     return out
 
 
+# ---- EnCodec 24 kHz (csrc/encodec.cu) -----------------------------------------------------------------
+def encodec_conv(x, weight, bias, *, stride=1, weight_packed=None):
+    """EnCodec's causal Conv1d (kernel K, stride s, dilation 1) on fp32 [B, Cin, L] -> [B, Cout, ceil(L / s)]:
+    reflect padding of K - s on the left and ceil(L / s) * s - L on the right.  The common case (no right padding,
+    L > K - s) is the SoundStream conv's own reflect halo; otherwise the row is padded first (alm_encodec_pad1d)
+    and the conv runs on it unpadded, dropping the outputs of its own (zero) halo."""
+    _check_cuda(x, weight, bias)
+    B, Cin, L = x.shape
+    K = weight.shape[-1]
+    pl, pr = K - stride, -L % stride
+    if pr == 0 and L > pl:
+        return causal_conv1d(x, weight, bias, stride=stride, pad_mode="reflect", weight_packed=weight_packed)
+    x = x.contiguous()
+    xp = torch.empty(B, Cin, pl + L + pr, device=x.device, dtype=f32)
+    _lib.call("alm_encodec_pad1d", x, xp, B * Cin, L, pl, pr)
+    y = causal_conv1d(xp, weight, bias, stride=stride, pad_mode="constant", weight_packed=weight_packed)
+    return y[..., pl // stride:].contiguous()
+
+
+def encodec_resblock(x, w3, b3, w1, ws, b_out, *, elu_out):
+    """SEANet resnet block on fp32 [B, C, T]: Ws x + W1 ELU(W3 * ELU(x) + b3) + b_out, ELU'd when elu_out.
+    w3 [C/2, C, 3], w1 [C, C/2], ws [C, C] and b_out = b1 + bs, all fp32 contiguous."""
+    _check_cuda(x, w3, b3, w1, ws, b_out)
+    x = x.contiguous()
+    B, C, T = x.shape
+    assert x.dtype == f32 and w3.shape == (C // 2, C, 3) and w1.shape == (C, C // 2) and ws.shape == (C, C)
+    y = torch.empty_like(x)
+    with _timed("encodec_resblock", 2.0 * B * T * (3 * C * C // 2 + C * C // 2 + C * C)):
+        _lib.call("alm_encodec_resblock_fp32", x, w3, b3, w1, ws, b_out, y, B, C, T, int(elu_out))
+    return y
+
+
+ENCODEC_LSTM_H = 512
+ENCODEC_LSTM_UNITS = 4  # hidden units per CTA (csrc/encodec.cu)
+
+
+def encodec_lstm_pack(w_ih, w_hh, b_ih, b_hh):
+    """two layers' torch.nn.LSTM parameters (lists of [4H, H] / [4H]) -> (w [H/4, 32, 2H], bias [H/4, 32]) fp32:
+    CTA k's row (layer l, gate g, unit u) at (l * 4 + g) * 4 + u is [W_ih_l | W_hh_l] of hidden unit 4k + u; the two
+    biases are added in fp64."""
+    H, U = ENCODEC_LSTM_H, ENCODEC_LSTM_UNITS
+    w = torch.stack([torch.cat((wi, wh), dim=1).reshape(4, H // U, U, 2 * H) for wi, wh in zip(w_ih, w_hh)])
+    b = torch.stack([(bi.double() + bh.double()).reshape(4, H // U, U) for bi, bh in zip(b_ih, b_hh)])
+    w = w.permute(2, 0, 1, 3, 4).reshape(H // U, 32, 2 * H)  # [cta][layer][gate][unit][K]
+    b = b.permute(2, 0, 1, 3).reshape(H // U, 32)
+    return w.float().contiguous(), b.float().contiguous()
+
+
+def encodec_lstm(x, packed, *, elu_out, check=False):
+    """EnCodec's LSTM block y = LSTM2(LSTM1(x)) + x (ELU'd when elu_out) on fp32 [B, 512, T] or on C8S
+    [B, 128, 1, T, 8] (bf16, the tensor-core codec layout); packed from encodec_lstm_pack.  One persistent cooperative
+    kernel (csrc/encodec.cu).  check=True synchronises and raises if a device-wide barrier of the kernel timed out."""
+    w, b = packed
+    _check_cuda(x, w, b)
+    x = x.contiguous()
+    c8s = x.dtype == bf16
+    if c8s:
+        B, nch2, P, T, _ = x.shape
+        assert nch2 * 4 == ENCODEC_LSTM_H and P == 1
+    else:
+        B, H, T = x.shape
+        assert H == ENCODEC_LSTM_H and x.dtype == f32
+    y = torch.empty_like(x)
+    ws = torch.empty(int(_lib.load().alm_encodec_lstm_workspace(B, T)), device=x.device, dtype=torch.uint8)
+    H = ENCODEC_LSTM_H
+    with _timed("encodec_lstm", 2.0 * B * T * 2 * 4 * H * 2 * H):
+        _lib.call("alm_encodec_lstm", x, w, b, y, ws, B, T, int(elu_out), int(c8s))
+    if check and int(ws[-12:-8].view(torch.int32).item()) != 0:
+        raise _lib.AlmError("alm_encodec_lstm: a device-wide barrier timed out (the output is not valid)")
+    return y
+
+
+def pack_encodec_resblock(w3, w1, ws):
+    """resnet-block weights w3 [C/2, C, 3], w1 [C, C/2], ws [C, C] (fp32) -> the 5-tap unit layout of
+    alm_encodec_resblock_tc: W3's taps with rows zero-padded to C, W1 with columns zero-padded to C, then Ws."""
+    C = ws.shape[0]
+    w = torch.zeros(C, C, 5, device=ws.device, dtype=f32)
+    w[: C // 2, :, :3] = w3.detach().float()
+    w[:, : C // 2, 3] = w1.detach().float()
+    w[:, :, 4] = ws.detach().float()
+    return _split_units(w)
+
+
+def encodec_resblock_tc(x, w_units, b3_pad, b_out, *, elu_out, out_phases=1):
+    """the resnet block on C8S activations (P = 1 in, `out_phases` planes out) on the tensor cores; w_units from
+    pack_encodec_resblock, b3_pad = b3 zero-padded to C."""
+    _check_cuda(x, w_units, b3_pad, b_out)
+    B, nch2, P, T, _ = x.shape
+    C = nch2 * 4
+    assert P == 1 and x.dtype == bf16 and x.is_contiguous() and w_units.dtype == bf16 and w_units.is_contiguous()
+    assert w_units.numel() == 5 * (C // 16) * 2 * 2 * C * 8 and b3_pad.numel() == C and b_out.numel() == C
+    y = torch.empty(B, nch2, out_phases, T // out_phases, 8, device=x.device, dtype=bf16)
+    with _timed("encodec_resblock_tc", 2.0 * B * T * 5 * C * C):
+        _lib.call("alm_encodec_resblock_tc", x, y, w_units, b3_pad, b_out, B, C, T, int(elu_out), int(out_phases))
+    return y
+
+
+
 SQ_MODES = {"fsq": 0, "lfq": 1}
 
 

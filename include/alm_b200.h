@@ -459,6 +459,33 @@ int alm_codec_gate_loop_tc(const void* x, const void* w_units, void* y, float* w
 int alm_causal_convT1d_fwd(const float* x, const float* w, const float* bias, float* y, int B, int Cin, int Cout,
                            int n, int stride, alm_stream_t stream);
 /*
+ * EnCodec 24 kHz (encodec.py, csrc/encodec.cu), fp32 on CUDA cores; activations fp32 [B][C][T].
+ * alm_encodec_pad1d: EnCodec's reflect padding of rows x [rows][L] -> y [rows][pad_left + L + pad_right], including
+ *   the zero-extension it applies first when L <= max(pad_left, pad_right).
+ * alm_encodec_resblock_fp32: SEANet resnet block  y = Ws x + W1 ELU(W3 * ELU(x) + b3) + b_out  (ELU(y) if elu_out),
+ *   W3 [C/2][C][3] causal with reflect-left padding 2, W1 [C][C/2], Ws [C][C], b_out = b1 + bs; C even, C <= 512.
+ * alm_encodec_lstm: y = LSTM2(LSTM1(x)) + x (ELU(.) if elu_out) over 512 channels, zero initial state, gates i, f, g, o.
+ *   One cooperative launch of 128 CTAs (the device needs >= 128 SMs) with T + 1 device-wide barriers.
+ *   w_packed [128][32][1024] (ops.encodec_lstm_pack): CTA k's rows (layer l, gate g, unit u) at (l * 4 + g) * 4 + u hold
+ *   [W_ih_l | W_hh_l] of hidden unit 4k + u; bias_packed [128][32] = b_ih + b_hh in the same order.  Every sum runs in a
+ *   fixed order without atomics: a clip's output does not depend on the rest of the batch.
+ *   x and y are fp32 [B][512][T], or C8S (P = 1, the tensor-core codec layout of alm_codec_conv_tc) when c8s = 1.
+ *   workspace: alm_encodec_lstm_workspace(B, T) bytes, 16-byte aligned; it ends in the barrier counter (uint32), an
+ *   error flag (int32 at byte size - 12: non-zero if a device-wide barrier timed out) and 8 bytes of padding.
+ * alm_encodec_resblock_tc: the resnet block on the tensor cores (csrc/codec_tc.cu, split bf16 as alm_codec_ru_tc),
+ *   x C8S (P = 1), y C8S with out_phases planes; C in {32, 64, 128, 256}, T > 2.  w_units (ops.pack_encodec_resblock):
+ *   the alm_codec_ru_tc unit layout with 5 taps: W3's 3 taps with rows zero-padded to C, W1 with columns zero-padded to
+ *   C, Ws.  b3 [C] (zero-padded from C/2), b_out = b1 + bs [C].
+ */
+int alm_encodec_pad1d(const float* x, float* y, int64_t rows, int L, int pad_left, int pad_right, alm_stream_t stream);
+int alm_encodec_resblock_fp32(const float* x, const float* w3, const float* b3, const float* w1, const float* ws,
+                              const float* b_out, float* y, int B, int C, int T, int elu_out, alm_stream_t stream);
+long long alm_encodec_lstm_workspace(int B, int T);
+int alm_encodec_lstm(const void* x, const float* w_packed, const float* bias_packed, void* y, void* workspace,
+                     int B, int T, int elu_out, int c8s, alm_stream_t stream);
+int alm_encodec_resblock_tc(const void* x, void* y, const void* w_units, const float* b3, const float* b_out, int B,
+                            int C, int T, int elu_out, int out_phases, alm_stream_t stream);
+/*
  * Residual VQ, eval path (vector-quantize-pytorch ResidualVQ.forward as called at soundstream.py:840):
  * for q in 0..Q-1: idx = argmin_c sqrt(max(|r|^2 + |e_c|^2 - 2 r.e_c, 0)) (lowest index on ties);
  * r -= e_idx; quantized += e_idx.  x [N, D] (row stride ldx), codebooks [Q, C, D], indices [N, Q] int64.
