@@ -13,7 +13,9 @@ from .hubert import HubertWithKmeans  # noqa: E402,F401
 from .parallel import FlatGradBucket  # noqa: E402,F401
 from .soundstream import AudioLMSoundStream, MusicLMSoundStream, SoundStream  # noqa: E402,F401
 from .transformer import Transformer  # noqa: E402,F401
+from .vq_wav2vec import FairseqVQWav2Vec  # noqa: E402,F401
 
 __all__ = ["AudioLM", "SemanticTransformer", "CoarseTransformer", "FineTransformer", "SemanticTransformerWrapper",
            "CoarseTransformerWrapper", "FineTransformerWrapper", "SoundStream", "AudioLMSoundStream",
-           "MusicLMSoundStream", "Transformer", "FlatGradBucket", "HubertWithKmeans", "EncodecWrapper"]
+           "MusicLMSoundStream", "Transformer", "FlatGradBucket", "HubertWithKmeans",
+           "EncodecWrapper", "FairseqVQWav2Vec"]

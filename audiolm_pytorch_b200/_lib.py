@@ -89,6 +89,8 @@ SIGNATURES: dict[str, list] = {
     "alm_hubert_pos_pack": [P, P, I, I, I, I, I, I, P],
     "alm_hubert_qkv_heads": [P, P, P, P, I, I, I, I, P],
     "alm_hubert_merge_heads": [P, P, I, I, I, I, P],
+    "alm_w2v_group_stats": [P, P, P, I, I, I, I, P],
+    "alm_w2v_norm_act": [P, P, P, P, I, P, I, I, F, I, P, P, I, I, I, I, P],
     "alm_encodec_pad1d": [P, P, L, I, I, I, P],
     "alm_encodec_resblock_fp32": [P, P, P, P, P, P, P, I, I, I, I, P],
     "alm_encodec_lstm": [P, P, P, P, P, I, I, I, I, P],

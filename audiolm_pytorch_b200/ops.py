@@ -1355,3 +1355,37 @@ def hubert_attention(qkv, *, heads):
     split = torch.empty(B, T, 3 * D, device=qkv.device, dtype=bf16)
     _lib.call("alm_hubert_merge_heads", o, split, B, T, D, heads)
     return split
+
+
+# ---- vq-wav2vec feature path (csrc/vq_wav2vec.cu; the network itself is audiolm_pytorch_b200/vq_wav2vec.py) ----------
+W2V_STATS_ROWS = 64  # ALM_W2V_STATS_ROWS: rows per fp64 partial of alm_w2v_group_stats
+W2V_ACT = {None: 0, "relu": 1, "gelu": 2}
+
+
+def w2v_group_stats(y, groups=1):
+    """GroupNorm(groups, C) statistics of y fp32 [B, T, C] over the (C / groups) x T elements of each group ->
+    fp32 [B, groups, 2] = {mean, 1 / sqrt(var + 1e-5)}; fixed-order fp64 partial sums, so batch-independent"""
+    _check_cuda(y)
+    assert y.dtype == f32 and y.is_contiguous()
+    B, T, C = y.shape
+    stats = torch.empty(B, groups, 2, device=y.device, dtype=f32)
+    work = torch.empty(B * groups * -(-T // W2V_STATS_ROWS) * 2, device=y.device, dtype=torch.float64)
+    _lib.call("alm_w2v_group_stats", y, stats, work, B, T, C, groups)
+    return stats
+
+
+def w2v_norm_act(y, stats, *, gamma=None, beta=None, act=None, residual=None, step=1, residual_scale=1.0,
+                 log_compress=False, want_out=False, want_split=True):
+    """per element of y fp32 [B, T, C]: GroupNorm with stats [B, G, 2] (w2v_group_stats), the optional per-channel
+    gamma / beta, act (None, "relu" or "gelu"); with residual fp32 [B, Tr, C]:
+    (v + residual[:, ::step][:, :T]) * residual_scale; log(|v| + 1) if log_compress
+    -> (fp32 [B, T, C] or None, split bf16 [B, T, 3C] or None)"""
+    _check_cuda(y, stats, gamma, beta, residual)
+    assert y.dtype == f32 and y.is_contiguous() and (residual is None or residual.is_contiguous())
+    B, T, C = y.shape
+    out = torch.empty_like(y) if want_out else None
+    split = torch.empty(B, T, 3 * C, device=y.device, dtype=bf16) if want_split else None
+    Tr = residual.shape[1] if residual is not None else 0
+    _lib.call("alm_w2v_norm_act", y, stats, gamma, beta, W2V_ACT[act], residual, Tr, int(step), float(residual_scale),
+              int(log_compress), out, split, B, T, C, stats.shape[1])
+    return out, split

@@ -578,6 +578,28 @@ int alm_hubert_qkv_heads(const float* qkv, void* q, void* k, void* v, int B, int
                          alm_stream_t stream);
 int alm_hubert_merge_heads(const void* o, void* split, int B, int T, int D, int heads, alm_stream_t stream);
 
+/*
+ * vq-wav2vec feature path (fairseq's wav2vec ConvFeatureExtractionModel and KmeansVectorQuantizer as called by
+ * FairseqVQWav2Vec, vq_wav2vec.py:75-76), csrc/vq_wav2vec.cu: the fp32 kernels between the split-bf16 GEMMs.  The
+ * convs run on alm_hubert_conv0 (conv 0) and alm_gemm_bf16 in the split layout of the HuBERT block above; the grouped
+ * 1x1 projection is one GEMM against a block-diagonal weight; the codeword search is alm_rvq_select.  GroupNorm eps is
+ * 1e-5; GELU is the erf form.  Reductions run in a fixed order without atomics, so a clip's outputs are bitwise
+ * reproducible and do not depend on the other clips of the batch.
+ *   alm_w2v_group_stats  stats fp32 [B, G, 2] = {mean, 1 / sqrt(var + eps)} of y fp32 [B, T, C] over the (C / G) x T
+ *                        elements of each group (GroupNorm(G, C), biased variance), from fp64 sums over chunks of
+ *                        ALM_W2V_STATS_ROWS rows merged in chunk order.  work: fp64 [B, G, ceil(T / ALM_W2V_STATS_ROWS), 2].
+ *                        (C / G) % 4 == 0.
+ *   alm_w2v_norm_act     per element of y fp32 [B, T, C]: v = (y - mean) rstd of its (b, c / (C / G)) stats, then
+ *                        v gamma[c] + beta[c] (both or neither), act (0 none, 1 ReLU, 2 GELU); with a residual
+ *                        fp32 [B, Tr, C]: v = (v + residual[b, t * step, c]) * scale; if log_compress v = log(|v| + 1)
+ *                        -> out fp32 [B, T, C] and / or split bf16 [B, T, 3C] (either may be null).  C % 4 == 0.
+ */
+#define ALM_W2V_STATS_ROWS 64
+int alm_w2v_group_stats(const float* y, float* stats, double* work, int B, int T, int C, int G, alm_stream_t stream);
+int alm_w2v_norm_act(const float* y, const float* stats, const float* gamma, const float* beta, int act,
+                     const float* residual, int Tr, int step, float scale, int log_compress, float* out, void* split,
+                     int B, int T, int C, int G, alm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
