@@ -985,39 +985,58 @@ def rvq_encode(x, codebooks):
     return quant, idx
 
 
+def rvq_search_width(D):
+    """width the tensor-core search runs at: D rounded up to a multiple of 8 (the score GEMM's row pitch 3D must be
+    one).  The extra columns are zero in the codebooks and in the residual, so they add exact zeros to every norm and
+    dot product and the fp32 argmin is that of width D."""
+    return -(-D // 8) * 8
+
+
 def rvq_pack_codebooks(codebooks):
-    """codebooks fp32 [Q, C, D] -> (packed bf16 [Q, C, 3D] = [hi | hi | lo], e2 fp32 [Q, C]) for rvq_encode_tc."""
+    """codebooks fp32 [Q, C, D] -> (codebooks fp32 [Q, C, Dp], packed bf16 [Q, C, 3Dp] = [hi | hi | lo], e2 fp32 [Q, C])
+    for rvq_encode_tc, zero-padded to Dp = rvq_search_width(D)."""
     _check_cuda(codebooks)
     Q, C, D = codebooks.shape
+    Dp = rvq_search_width(D)
     cb = codebooks.to(f32).contiguous()
-    packed = torch.empty(Q, C, 3 * D, device=cb.device, dtype=bf16)
-    e2 = torch.empty(Q, C, device=cb.device, dtype=f32)
-    _lib.call("alm_rvq_pack_codebooks", cb, packed, e2, Q * C, D)
-    return cb, packed, e2
+    if Dp != D:
+        cb = torch.nn.functional.pad(cb, (0, Dp - D))
+    packed, e2 = _split_pack(cb.view(Q * C, Dp))
+    return cb, packed.view(Q, C, 3 * Dp), e2.view(Q, C)
+
+
+def _split_pack(rows):
+    """fp32 [R, K] contiguous -> (bf16 [R, 3K] = [hi | hi | lo], fp32 |row|^2 [R])"""
+    R, K = rows.shape
+    packed = torch.empty(R, 3 * K, device=rows.device, dtype=bf16)
+    e2 = torch.empty(R, device=rows.device, dtype=f32)
+    _lib.call("alm_rvq_pack_codebooks", rows, packed, e2, R, K)
+    return packed, e2
 
 
 def rvq_encode_tc(x, packed_codebooks):
     """x [N, D] fp32 -> (quantized [N, D] fp32, indices [N, Q] int64); distance GEMMs on the tensor cores, the
-    winner of every stage chosen by exact fp32 re-evaluation of the candidates (csrc/rvq_tc.cu)."""
+    winner of every stage chosen by exact fp32 re-evaluation of the candidates (csrc/rvq_tc.cu).  Any D: the search
+    runs at the padded width of rvq_pack_codebooks."""
     cb, packed, e2 = packed_codebooks
     _check_cuda(x, cb)
     assert x.dtype == f32 and x.stride(-1) == 1
     N, D = x.shape
-    Q, C, _ = cb.shape
-    assert D % 8 == 0
+    Q, C, Dp = cb.shape
+    assert Dp == rvq_search_width(D), f"codebooks packed for width {Dp}, x has {D}"
     dev = x.device
-    r = torch.empty(N, D, device=dev, dtype=f32)
-    quant = torch.empty(N, D, device=dev, dtype=f32)
-    rp = torch.empty(N, 3 * D, device=dev, dtype=bf16)
+    r = torch.empty(N, Dp, device=dev, dtype=f32)
+    quant = torch.empty(N, Dp, device=dev, dtype=f32)
+    rp = torch.empty(N, 3 * Dp, device=dev, dtype=bf16)
     scores = torch.empty(N, C, device=dev, dtype=f32)
     idx = torch.empty(N, Q, device=dev, dtype=torch.int64)
     with _timed("rvq_encode_tc", 2.0 * N * Q * C * D):
-        _lib.call("alm_rvq_prepare", x, x.stride(0), r, quant, D, rp, N, D)
+        _lib.call("alm_rvq_prepare", x, x.stride(0), r, quant, Dp, rp, N, D, Dp)
         for q in range(Q):
             gemm(rp, packed[q], out=scores, cls="rvq_score_gemm")
-            _lib.call("alm_rvq_select", scores, C, e2[q], cb[q], r, quant, D, rp, idx[:, q:], Q, N, D, C,
+            _lib.call("alm_rvq_select", scores, C, e2[q], cb[q], r, quant, Dp, rp, idx[:, q:], Q, N, Dp, C,
                       int(q + 1 < Q))
-    return quant, idx
+    return (quant if Dp == D else quant[:, :D].contiguous()), idx
 
 
 def nearest_centroid(x, packed_centroids):
@@ -1244,8 +1263,9 @@ def resid_ln_bwd(r_new, gamma, stats, dr_out, dxn, dextra, g_gamma, *, out_scale
 # ---- HuBERT feature path (csrc/hubert.cu; the network itself is audiolm_pytorch_b200/hubert.py) ----------------------
 def pack_split_weight(w):
     """fp32 weight [N, K] -> bf16 [N, 3K] = [w_hi | w_hi | w_lo], the B operand of a split-bf16 GEMM against activation
-    rows [x_hi | x_lo | x_hi] (the packing of rvq_pack_codebooks)"""
-    return rvq_pack_codebooks(w[None])[1][0]
+    rows [x_hi | x_lo | x_hi] (the packing of rvq_pack_codebooks, without its padding)"""
+    _check_cuda(w)
+    return _split_pack(w.to(f32).contiguous())[0]
 
 
 def pack_split_conv_weight(w):

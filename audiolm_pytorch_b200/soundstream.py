@@ -239,7 +239,7 @@ class ResidualVQ(nn.Module):
             raise RuntimeError("codebooks are not initialised (load a checkpoint; k-means init is not built)")
         b, n, d = x.shape
         flat = x.reshape(b * n, d).to(f32).contiguous()
-        if RVQ_ON_TENSOR_CORES and d % 8 == 0:
+        if RVQ_ON_TENSOR_CORES:   # any width: rvq_encode_tc zero-pads to a multiple of 8
             embeds = [l._codebook.embed for l in self.layers]
             key = tuple((e.data_ptr(), e._version) for e in embeds)
             if self.__dict__.get("_tc_key") != key:

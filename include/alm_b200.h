@@ -501,11 +501,13 @@ int alm_rvq_encode(const float* x, int64_t ldx, const float* codebooks, float* e
  * select re-evaluates every candidate within the bf16x3 error bound of the best approximate score with the exact fp32
  * expansion sqrt(max(|r|^2 + |e|^2 - 2 r.e, 0)) (lowest index on ties), then r -= e, quantized += e, R' <- split(r).
  * alm_rvq_pack_codebooks: codebooks fp32 [rows = Q*C, D] -> packed bf16 [rows, 3D] + e2 [rows] (once per weight version).
- * alm_rvq_prepare: r = x, quantized = 0, R' = split(x).
+ * alm_rvq_prepare: r = x, quantized = 0, R' = split(x), x [N, Dx] zero-padded to the search width D >= Dx.  Any
+ * codebook width runs here: the host pads it to D = a multiple of 8 (3D is the GEMM's row pitch); zero columns add
+ * exact zeros to every norm and dot product, so the fp32 argmin is that of the unpadded width.
  */
 int alm_rvq_pack_codebooks(const float* codebooks, void* packed, float* e2, int64_t rows, int D, alm_stream_t stream);
-int alm_rvq_prepare(const float* x, int64_t ldx, float* r, float* quantized, int64_t ldq, void* rp, int N, int D,
-                    alm_stream_t stream);
+int alm_rvq_prepare(const float* x, int64_t ldx, float* r, float* quantized, int64_t ldq, void* rp, int N, int Dx,
+                    int D, alm_stream_t stream);
 int alm_rvq_select(const float* scores, int64_t lds, const float* e2, const float* codebook, float* r, float* quantized,
                    int64_t ldq, void* rp, int64_t* indices, int64_t ldi, int N, int D, int C, int write_rp,
                    alm_stream_t stream);

@@ -79,37 +79,6 @@ def test_soundstream_golden_end_to_end():
     assert err(recon_idx, recon) < 1e-5  # README.md:100-113 round trip
 
 
-@pytest.mark.parametrize("impl", ["fp32_cuda_cores", "tensor_cores"])
-def test_rvq_bit_exact_at_config_size(impl):
-    """C1 sizes: 8 stages x 1024 codes x 512 dims.  Rows whose best/second-best gap exceeds fp32 noise must
-    match the oracle exactly; the flip rate on the rest is reported."""
-    from audiolm_pytorch_b200 import ops
-    from oracle import codec as oc
-
-    torch.manual_seed(7)
-    cb = torch.randn(8, 1024, 512)
-    x = torch.randn(600, 512) * 3
-    q_ref, i_ref = oc.rvq_encode(x, cb)
-    margin = oc.rvq_margin(x, cb)
-    if impl == "tensor_cores":   # distance GEMM on wgmma + exact fp32 re-rank of the candidates (csrc/rvq_tc.cu)
-        q, i = ops.rvq_encode_tc(x.to(DEV), ops.rvq_pack_codebooks(cb.to(DEV)))
-    else:
-        q, i = ops.rvq_encode(x.to(DEV), cb.to(DEV))
-    safe = margin > 1e-3
-    assert safe.float().mean() > 0.9
-    assert torch.equal(i.cpu()[safe], i_ref[safe])
-    flips = (i.cpu() != i_ref).any(-1).float().mean().item()
-    print(f"rvq rows differing from the oracle: {flips:.4%} (margin-safe rows: {safe.float().mean().item():.2%})")
-    same = (i.cpu() == i_ref).all(-1)
-    assert err(q[same.to(DEV)], q_ref[same]) < 1e-5
-    dec = ops.rvq_decode(i, cb.to(DEV))
-    assert err(dec, oc.rvq_decode(i.cpu(), cb)) < 1e-5
-    # dropped quantizers (-1) contribute nothing
-    i2 = i.clone()
-    i2[:, 5:] = -1
-    assert err(ops.rvq_decode(i2, cb.to(DEV)), oc.rvq_decode(i2.cpu(), cb)) < 1e-5
-
-
 # ---- the kernels the C1 bench times, at C1 shapes (VERDICT r1, weak #1) --------------------------------------------
 C1_LAYERS = [(32, 48000), (64, 24000), (128, 6000), (256, 1200)]
 
