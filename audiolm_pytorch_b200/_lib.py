@@ -79,6 +79,9 @@ SIGNATURES: dict[str, list] = {
     "alm_rvq_pack_codebooks": [P, P, P, L, I, P],
     "alm_rvq_prepare": [P, L, P, P, L, P, I, I, I, P],
     "alm_rvq_select": [P, L, P, P, P, P, L, P, P, L, I, I, I, I, P],
+    "alm_rvq_prepare_cos": [P, L, P, P, L, P, I, I, I, P],
+    "alm_rvq_select_cos": [P, L, P, P, P, P, L, P, P, L, I, I, I, I, P],
+    "alm_split_rows": [P, L, P, I, I, P],
     "alm_rvq_decode": [P, L, P, P, L, I, I, I, I, P],
     "alm_sq_encode": [P, L, I, I, I, I, P, P, P, P, P, P, I, I, P, L, P, I, P],
     "alm_sq_decode": [P, I, I, I, I, I, I, P, P, P, P, I, I, P, L, P],

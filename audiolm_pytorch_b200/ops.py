@@ -1014,10 +1014,15 @@ def _split_pack(rows):
     return packed, e2
 
 
-def rvq_encode_tc(x, packed_codebooks):
+RVQ_METRICS = {"euclid": ("alm_rvq_prepare", "alm_rvq_select"), "cosine": ("alm_rvq_prepare_cos", "alm_rvq_select_cos")}
+
+
+def rvq_encode_tc(x, packed_codebooks, *, metric="euclid"):
     """x [N, D] fp32 -> (quantized [N, D] fp32, indices [N, Q] int64); distance GEMMs on the tensor cores, the
     winner of every stage chosen by exact fp32 re-evaluation of the candidates (csrc/rvq_tc.cu).  Any D: the search
-    runs at the padded width of rvq_pack_codebooks."""
+    runs at the padded width of rvq_pack_codebooks.  metric "euclid": argmin of the Euclidean distance; "cosine":
+    argmax of F.normalize(r) . e_c (VectorQuantize(use_cosine_sim=True)); both lowest index on ties."""
+    prepare, select = RVQ_METRICS[metric]
     cb, packed, e2 = packed_codebooks
     _check_cuda(x, cb)
     assert x.dtype == f32 and x.stride(-1) == 1
@@ -1030,13 +1035,29 @@ def rvq_encode_tc(x, packed_codebooks):
     rp = torch.empty(N, 3 * Dp, device=dev, dtype=bf16)
     scores = torch.empty(N, C, device=dev, dtype=f32)
     idx = torch.empty(N, Q, device=dev, dtype=torch.int64)
-    with _timed("rvq_encode_tc", 2.0 * N * Q * C * D):
-        _lib.call("alm_rvq_prepare", x, x.stride(0), r, quant, Dp, rp, N, D, Dp)
+    with _timed("rvq_encode_tc" if metric == "euclid" else f"rvq_encode_tc_{metric}", 2.0 * N * Q * C * D):
+        _lib.call(prepare, x, x.stride(0), r, quant, Dp, rp, N, D, Dp)
         for q in range(Q):
             gemm(rp, packed[q], out=scores, cls="rvq_score_gemm")
-            _lib.call("alm_rvq_select", scores, C, e2[q], cb[q], r, quant, Dp, rp, idx[:, q:], Q, N, Dp, C,
+            _lib.call(select, scores, C, e2[q], cb[q], r, quant, Dp, rp, idx[:, q:], Q, N, Dp, C,
                       int(q + 1 < Q))
     return (quant if Dp == D else quant[:, :D].contiguous()), idx
+
+
+def split_rows(x):
+    """fp32 [N, D] (unit column stride) -> bf16 [N, 3D] = [x_hi | x_lo | x_hi], the activation operand of split_gemm"""
+    _check_cuda(x)
+    assert x.dtype == f32 and x.stride(-1) == 1
+    N, D = x.shape
+    out = torch.empty(N, 3 * D, device=x.device, dtype=bf16)
+    _lib.call("alm_split_rows", x, x.stride(0), out, N, D)
+    return out
+
+
+def split_linear(x, w_packed, bias):
+    """nn.Linear on fp32 rows x [N, K] in split bf16: x @ w^T + bias -> fp32 [N, Nout], w_packed = pack_split_weight(w),
+    the bias added in the GEMM's epilogue"""
+    return split_gemm(split_rows(x), w_packed, bias, cls="split_linear")
 
 
 def nearest_centroid(x, packed_centroids):

@@ -3,7 +3,8 @@
 Drop-in surface of /root/reference/audiolm_pytorch/soundstream.py:314-395, 451-866 for the calls the AudioLM
 hot path makes: `forward(x, return_encoded=True | return_codes_only=True | return_recons_only=True)`,
 `tokenize`, `decode_from_codebook_indices`, `decode`, with the reference's constructor kwargs and
-state_dict keys for `encoder.*`, `decoder.*`, `rq.*` (including the gate-loop layers of `use_gate_loop_layers`).  The quantizer is the residual VQ, residual FSQ
+state_dict keys for `encoder.*`, `decoder.*`, `rq.*` (including the gate-loop layers of `use_gate_loop_layers`).  The quantizer is the residual VQ
+(Euclidean or cosine-similarity codebooks, optionally behind `codebook_dim` projections), residual FSQ
 (`use_finite_scalar_quantizer`) or residual LFQ (`use_lookup_free_quantizer`), eval path only.  GAN / mel training
 losses, quantizer training and FiLM denoising are outside this build; the local-attention bottleneck lives in
 local_attn.py.
@@ -224,21 +225,72 @@ class _VQLayer(nn.Module):
         self._codebook = _Codebook(dim, codebook_size)
 
 
+# VectorQuantize / ResidualVQ kwargs that only shape training (EMA, k-means init, dead-code expiry, losses, sampling,
+# gradient estimators, quantize dropout); eval computes the same with or without them
+_VQ_TRAINING_KWARGS = {"decay", "eps", "commitment_weight", "kmeans_init", "kmeans_iters", "sync_kmeans",
+                       "threshold_ema_dead_code", "stochastic_sample_codes", "sample_codebook_temp", "straight_through",
+                       "rotation_trick", "reinmax", "sync_codebook", "ema_update", "learnable_codebook",
+                       "commitment_use_cross_entropy_loss"}
+_VQ_TRAINING_PREFIXES = ("orthogonal_reg_", "codebook_diversity_", "quantize_dropout")
+
+
+def _check_vq_kwargs(kwargs):
+    unknown = sorted(k for k in kwargs if k not in _VQ_TRAINING_KWARGS and not k.startswith(_VQ_TRAINING_PREFIXES))
+    if unknown:
+        raise NotImplementedError(f"ResidualVQ: rq_kwargs {unknown} are outside this build")
+
+
 class ResidualVQ(nn.Module):
-    def __init__(self, *, dim, num_quantizers, codebook_size, **_):
+    """vector-quantize-pytorch ResidualVQ, eval path: r = project_in(x); per stage the nearest code (Euclidean, or the
+    largest cosine similarity with use_cosine_sim) is subtracted from r and added to the output; project_out(output).
+    The projections are Linear(dim, codebook_dim) / Linear(codebook_dim, dim) with bias, absent when the widths agree;
+    they and the cosine search run on the tensor cores only."""
+
+    def __init__(self, *, dim, num_quantizers, codebook_size, codebook_dim=None, use_cosine_sim=False, **kwargs):
         super().__init__()
-        self.layers = nn.ModuleList([_VQLayer(dim, codebook_size) for _ in range(num_quantizers)])
+        _check_vq_kwargs(kwargs)
+        if not isinstance(codebook_size, int):
+            raise NotImplementedError(f"ResidualVQ: codebook_size={codebook_size!r} is outside this build (one int)")
+        dc = dim if codebook_dim is None else codebook_dim
+        self.projected = dc != dim
+        if self.projected and (dim % 8 or dc % 8):
+            raise NotImplementedError(f"ResidualVQ: projection {dim} -> {dc} is outside this build (dim per group and "
+                                      "codebook_dim multiples of 8)")
+        self.use_cosine_sim = bool(use_cosine_sim)
+        self.codebook_dim = dc
+        self.project_in = nn.Linear(dim, dc) if self.projected else nn.Identity()
+        self.project_out = nn.Linear(dc, dim) if self.projected else nn.Identity()
+        self.layers = nn.ModuleList([_VQLayer(dc, codebook_size) for _ in range(num_quantizers)])
 
     def codebooks(self):
         return torch.stack([l._codebook.embed[0] for l in self.layers]).to(f32)
+
+    def _projections(self):
+        """(w_in packed, b_in, w_out packed, b_out) for ops.split_linear, cached per weight version"""
+        mods = (self.project_in, self.project_out)
+        params = [p_ for m in mods for p_ in (m.weight, m.bias)]
+        return SoundStream._cached(self, "_proj", params, lambda: tuple(
+            t for m in mods for t in (ops.pack_split_weight(m.weight.detach()), m.bias.detach().float().contiguous())))
+
+    def _project(self, x, side):
+        if not self.projected:
+            return x
+        w_in, b_in, w_out, b_out = self._projections()
+        return ops.split_linear(x, *((w_in, b_in) if side == "in" else (w_out, b_out)))
+
+    def _check_tensor_cores(self):
+        if not RVQ_ON_TENSOR_CORES and (self.use_cosine_sim or self.projected):
+            raise NotImplementedError("ResidualVQ: cosine-similarity and projected codebooks run on the tensor-core "
+                                      "search only (RVQ_ON_TENSOR_CORES = True)")
 
     def forward(self, x):
         if self.training:
             raise NotImplementedError("RVQ training (EMA / k-means / commitment loss) is outside this build")
         if not all(bool(l._codebook.initted.item()) for l in self.layers):
             raise RuntimeError("codebooks are not initialised (load a checkpoint; k-means init is not built)")
+        self._check_tensor_cores()
         b, n, d = x.shape
-        flat = x.reshape(b * n, d).to(f32).contiguous()
+        flat = self._project(x.reshape(b * n, d).to(f32).contiguous(), "in")
         if RVQ_ON_TENSOR_CORES:   # any width: rvq_encode_tc zero-pads to a multiple of 8
             embeds = [l._codebook.embed for l in self.layers]
             key = tuple((e.data_ptr(), e._version) for e in embeds)
@@ -246,14 +298,17 @@ class ResidualVQ(nn.Module):
                 with torch.inference_mode(False), torch.no_grad():
                     self.__dict__["_tc_pack"] = ops.rvq_pack_codebooks(self.codebooks())
                 self.__dict__["_tc_key"] = key
-            quant, idx = ops.rvq_encode_tc(flat, self.__dict__["_tc_pack"])
+            quant, idx = ops.rvq_encode_tc(flat, self.__dict__["_tc_pack"],
+                                           metric="cosine" if self.use_cosine_sim else "euclid")
         else:
             quant, idx = ops.rvq_encode(flat, self.codebooks())
+        quant = self._project(quant, "out")
         return quant.view(b, n, d), idx.view(b, n, -1), torch.zeros(1, len(self.layers), device=x.device)
 
     def get_output_from_indices(self, indices):
         b, n, q = indices.shape
-        return ops.rvq_decode(indices.reshape(b * n, q), self.codebooks()).view(b, n, -1)
+        out = self._project(ops.rvq_decode(indices.reshape(b * n, q), self.codebooks()), "out")
+        return out.view(b, n, -1)
 
 
 class GroupedResidualVQ(nn.Module):
@@ -465,8 +520,15 @@ class SoundStream(nn.Module):
             assert exists(codebook_size) and not exists(finite_scalar_quantizer_levels), \
                 "if use_finite_scalar_quantizer is set to False, `codebook_size` must be set (and not " \
                 "`finite_scalar_quantizer_levels`)"
+            # the training-only kwargs the reference passes (soundstream.py:592-607) are accepted and unused here
             self.rq = GroupedResidualVQ(dim=codebook_dim, num_quantizers=rq_num_quantizers,
-                                        codebook_size=codebook_size, groups=rq_groups)
+                                        codebook_size=codebook_size, groups=rq_groups, decay=rq_ema_decay,
+                                        commitment_weight=rq_commitment_weight,
+                                        quantize_dropout_multiple_of=rq_quantize_dropout_multiple_of, kmeans_init=True,
+                                        threshold_ema_dead_code=2, quantize_dropout=True,
+                                        quantize_dropout_cutoff_index=quantize_dropout_cutoff_index,
+                                        stochastic_sample_codes=rq_stochastic_sample_codes,
+                                        rotation_trick=rq_rotation_trick, **rq_kwargs)
             self.codebook_size = codebook_size
         decoder_blocks = []
         for (ci, co), s in zip(reversed(pairs), reversed(strides)):

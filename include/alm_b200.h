@@ -511,6 +511,21 @@ int alm_rvq_prepare(const float* x, int64_t ldx, float* r, float* quantized, int
 int alm_rvq_select(const float* scores, int64_t lds, const float* e2, const float* codebook, float* r, float* quantized,
                    int64_t ldq, void* rp, int64_t* indices, int64_t ldi, int N, int D, int C, int write_rp,
                    alm_stream_t stream);
+/*
+ * Cosine-similarity codebooks (VectorQuantize(use_cosine_sim=True)): the same stage loop with
+ * idx = argmax_c r^.e_c, r^ = r / max(|r|, 1e-12) (lowest index on ties), e_c the stored row as is; r -= e, quantized += e.
+ * alm_rvq_prepare_cos: as alm_rvq_prepare, with R' = split(x^).  alm_rvq_select_cos: candidates within the bf16x3 window
+ * of the best maximum score (S = R' B'^T ~ r^.e, same GEMM), re-ranked by r.e in fp32; then r, quantized and
+ * R' <- split(r^) of the new residual.  Same arguments as their Euclidean counterparts.
+ * alm_split_rows: x fp32 [N, D] (row stride ldx) -> out bf16 [N, 3D] = [x_hi | x_lo | x_hi], the activation operand of
+ * a split-bf16 GEMM (the project_in / project_out Linears of a residual VQ with codebook_dim != dim).
+ */
+int alm_rvq_prepare_cos(const float* x, int64_t ldx, float* r, float* quantized, int64_t ldq, void* rp, int N, int Dx,
+                        int D, alm_stream_t stream);
+int alm_rvq_select_cos(const float* scores, int64_t lds, const float* e2, const float* codebook, float* r,
+                       float* quantized, int64_t ldq, void* rp, int64_t* indices, int64_t ldi, int N, int D, int C,
+                       int write_rp, alm_stream_t stream);
+int alm_split_rows(const float* x, int64_t ldx, void* out, int N, int D, alm_stream_t stream);
 
 /* get_output_from_indices (soundstream.py:697): out[n,:] = sum_q codebooks[q][indices[n,q]] (-1 -> skip) */
 int alm_rvq_decode(const int64_t* indices, int64_t ldi, const float* codebooks, float* out, int64_t ldo, int N, int D,
