@@ -268,7 +268,7 @@ __device__ __noinline__ void hc_pre_row(const Ctx& cx, const bool first, const u
   }
   // mix the streams; the branch input stays in registers for the LayerNorm
   float2 bi[MAXP];
-  float s1 = 0.f, s2 = 0.f;
+  float s1 = 0.f, s2 = 0.f, dummy = 0.f;
 #pragma unroll
   for (int k = 0; k < MAXP; ++k) {
     const int c = 2 * (threadIdx.x + k * NT);
@@ -282,7 +282,6 @@ __device__ __noinline__ void hc_pre_row(const Ctx& cx, const bool first, const u
       }
       bi[k] = acc;
       s1 += acc.x + acc.y;
-      s2 = fmaf(acc.x, acc.x, fmaf(acc.y, acc.y, s2));
       *reinterpret_cast<__nv_bfloat162*>(bin + c) = __floats2bfloat162_rn(acc.x, acc.y);
 #pragma unroll
       for (int t = 1; t < HT; ++t) {
@@ -296,9 +295,16 @@ __device__ __noinline__ void hc_pre_row(const Ctx& cx, const bool first, const u
       }
     }
   }
-  block_sum2(s1, s2, cx.sRed2, which);
+  block_sum2(s1, dummy, cx.sRed2, which);
   const float mean = s1 * inv_d;
-  const float rstd = rsqrtf(fmaxf(s2 * inv_d - mean * mean, 0.f) + 1e-5f);
+  // the variance in a second pass over the registers (as hc2::pre_fwd_kernel)
+#pragma unroll
+  for (int k = 0; k < MAXP; ++k)
+    if (2 * (threadIdx.x + k * NT) < d)
+      s2 = fmaf(bi[k].x - mean, bi[k].x - mean, fmaf(bi[k].y - mean, bi[k].y - mean, s2));
+  dummy = 0.f;
+  block_sum2(s2, dummy, cx.sRed2, which);
+  const float rstd = rsqrtf(s2 * inv_d + 1e-5f);
 #pragma unroll
   for (int k = 0; k < MAXP; ++k) {
     const int c = 2 * (threadIdx.x + k * NT);
@@ -688,7 +694,7 @@ __device__ __noinline__ void geglu_rows(const Args& a, const Ctx& cx, const floa
   for (int r = 0; r < a.b; ++r) {
     const __nv_bfloat16* hr = a.h + (size_t)r * 2 * ip;
     float v[MAXG][8], gm[MAXG][8];
-    float s1 = 0.f, s2 = 0.f;
+    float s1 = 0.f, s2 = 0.f, dummy = 0.f;
 #pragma unroll
     for (int k = 0; k < MAXG; ++k) {
       const int c0 = (threadIdx.x + k * NT) * 8;
@@ -718,13 +724,22 @@ __device__ __noinline__ void geglu_rows(const Args& a, const Ctx& cx, const floa
           const float val = c0 + e < inner ? gt[e] * cdf * av[e] : 0.f;
           v[k][e] = val;
           s1 += val;
-          s2 = fmaf(val, val, s2);
         }
       }
     }
-    block_sum2(s1, s2, cx.sRed2, which);
+    block_sum2(s1, dummy, cx.sRed2, which);
     const float mean = s1 * a.inv_inner;
-    const float rstd = rsqrtf(fmaxf(s2 * a.inv_inner - mean * mean, 0.f) + 1e-5f);
+    // the variance in a second pass over the registers (as geglu_ln_fwd_kernel)
+#pragma unroll
+    for (int k = 0; k < MAXG; ++k) {
+      const int c0 = (threadIdx.x + k * NT) * 8;
+#pragma unroll
+      for (int e = 0; e < 8; ++e)
+        if (c0 + e < inner) s2 = fmaf(v[k][e] - mean, v[k][e] - mean, s2);
+    }
+    dummy = 0.f;
+    block_sum2(s2, dummy, cx.sRed2, which);
+    const float rstd = rsqrtf(s2 * a.inv_inner + 1e-5f);
 #pragma unroll
     for (int k = 0; k < MAXG; ++k) {
       const int c0 = (threadIdx.x + k * NT) * 8;

@@ -135,7 +135,7 @@ geglu_ln_fwd_kernel(const __nv_bfloat16* __restrict__ h, long long ldh, int gate
       }
     }
     float g[NCH][8];
-    float s12[2] = {0.f, 0.f};  // sum, sum of squares: one block reduction per row
+    float s[1] = {0.f};
 #pragma unroll
     for (int k = 0; k < NCH; ++k) {
       const int c0 = (threadIdx.x + k * NT) * 8;
@@ -152,14 +152,23 @@ geglu_ln_fwd_kernel(const __nv_bfloat16* __restrict__ h, long long ldh, int gate
           gelu_parts(gt[e], cdf, xpdf);
           const float v = e < nv ? gt[e] * cdf * a[e] : 0.f;
           g[k][e] = v;
-          s12[0] += v;
-          s12[1] = fmaf(v, v, s12[1]);
+          s[0] += v;
         }
       }
     }
-    block_sum_nt<2, NT>(s12, buf);
-    const float mean = s12[0] / inner;
-    const float rstd = rsqrtf(fmaxf(s12[1] / inner - mean * mean, 0.f) + 1e-5f);
+    block_sum_nt<1, NT>(s, buf);
+    const float mean = s[0] / inner;
+    // the variance in a second pass over the registers: E[v^2] - mean^2 loses (mean / sigma)^2 2^-24 of it in fp32
+    float q[1] = {0.f};
+#pragma unroll
+    for (int k = 0; k < NCH; ++k) {
+      const int c0 = (threadIdx.x + k * NT) * 8;
+#pragma unroll
+      for (int e = 0; e < 8; ++e)
+        if (c0 + e < inner) q[0] = fmaf(g[k][e] - mean, g[k][e] - mean, q[0]);
+    }
+    block_sum_nt<1, NT>(q, buf);
+    const float rstd = rsqrtf(q[0] / inner + 1e-5f);
 #pragma unroll
     for (int k = 0; k < NCH; ++k) {
       const int c0 = (threadIdx.x + k * NT) * 8;

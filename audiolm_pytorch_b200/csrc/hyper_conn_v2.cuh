@@ -245,7 +245,7 @@ pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
     }
     // mixed residual streams out; branch input kept for the LayerNorm
     float bi[NCH][8];
-    float st[2] = {0.f, 0.f};  // sum, sum of squares of the branch input (LayerNorm statistics in one reduction)
+    float st[1] = {0.f};  // sum of the branch input (channels >= d hold 0)
 #pragma unroll
     for (int k = 0; k < NCH; ++k) {
 #pragma unroll
@@ -255,7 +255,6 @@ pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
         for (int s = 0; s < S; ++s) a = fmaf(alpha[s][0], R[s][k][e], a);
         bi[k][e] = a;
         st[0] += a;
-        st[1] = fmaf(a, a, st[1]);
       }
       if (act[k]) {
 #pragma unroll
@@ -273,9 +272,18 @@ pre_fwd_kernel(const __nv_bfloat16* __restrict__ R_in, const __nv_bfloat16* __re
         if (bin != nullptr) *reinterpret_cast<uint4*>(bin + (size_t)m * d + ch[k]) = pack8(bi[k]);
       }
     }
-    slot_sum<2, TPT, MAILW>(st, mail, which, w2, lane, bar_id);
+    slot_sum<1, TPT, MAILW>(st, mail, which, w2, lane, bar_id);
     const float mean = st[0] / d;
-    const float rstd = rsqrtf(fmaxf(st[1] / d - mean * mean, 0.f) + 1e-5f);
+    // the variance in a second pass over the registers: E[x^2] - mean^2 loses (mean / sigma)^2 2^-24 of it in fp32
+    float q[1] = {0.f};
+#pragma unroll
+    for (int k = 0; k < NCH; ++k)
+      if (act[k]) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) q[0] = fmaf(bi[k][e] - mean, bi[k][e] - mean, q[0]);
+      }
+    slot_sum<1, TPT, MAILW>(q, mail, which, w2, lane, bar_id);
+    const float rstd = rsqrtf(q[0] / d + 1e-5f);
 #pragma unroll
     for (int k = 0; k < NCH; ++k)
       if (act[k]) {

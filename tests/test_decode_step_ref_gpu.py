@@ -22,12 +22,12 @@ KEYS_PER_SPLIT, MAX_SPLITS = 32, 16   # flash-decoding slices of csrc/decode_ste
 RATIO = 1.5
 
 
-def case(b, d, heads, depth, n0, value_residual, mask, bound, *, id, streams=4, fused=True):
-    return pytest.param(b, d, heads, depth, n0, value_residual, mask, streams, fused, bound, id=id)
+def case(b, d, heads, depth, n0, value_residual, mask, bound, *, id, streams=4, fused=True, dc=0.0):
+    return pytest.param(b, d, heads, depth, n0, value_residual, mask, streams, fused, bound, dc, id=id)
 
 
 # (b, d, heads, depth, n0 = cached positions before the first step, value residual, key mask, bound, streams,
-# one-kernel step taken).  `bound` caps the RMS-relative error of every vector checked (an output row, one layer's
+# one-kernel step taken, DC offset added to every token vector).  `bound` caps the RMS-relative error of every vector checked (an output row, one layer's
 # appended k or v row of one sequence) on both paths: about 3x the largest error either path showed in the case on an
 # H100 SXM (132 SMs, 700 W power limit).  The 64-layer model is ill-conditioned: its fp64 forward already moves 15-25x
 # as much as a bf16-sized change of its input, so both paths sit 0.1-0.4 from it and only gross errors show there.
@@ -44,6 +44,10 @@ CASES = [
     case(2, 1024, 8, 1, 64, True, "holes", 1.2e-2, id="d1024-accepted"),
     case(2, 1280, 8, 1, 64, True, "holes", 1.1e-2, fused=False, id="d1280-refused-falls-back"),
     case(2, 1536, 8, 1, 64, True, "holes", 1.2e-2, fused=False, id="d1536-refused-falls-back"),
+    # token vectors with a DC offset: the branch inputs' LayerNorms see mean / sigma of about dc.  Larger offsets drown
+    # in the bf16 rounding of the residual streams (2^-9 dc per element), which both paths store and the oracle does not
+    case(2, 1024, 8, 2, 64, True, "holes", 5.5e-2, dc=4.0, id="dc4-offset"),
+    case(1, 256, 16, 3, 95, True, "holes", 5.6e-2, dc=16.0, id="dc16-offset"),
 ]
 
 
@@ -147,13 +151,14 @@ def _run_path(fused_flag, tr, st, b, n0, kv, mask, xs, ref_kw):
         decode.FUSED_STACK_STEP = default
 
 
-@pytest.mark.parametrize("b,d,heads,depth,n0,value_residual,mask_kind,streams,fused,bound", CASES)
-def test_step_matches_fp64_reference(b, d, heads, depth, n0, value_residual, mask_kind, streams, fused, bound, request):
+@pytest.mark.parametrize("b,d,heads,depth,n0,value_residual,mask_kind,streams,fused,bound,dc", CASES)
+def test_step_matches_fp64_reference(b, d, heads, depth, n0, value_residual, mask_kind, streams, fused, bound, dc,
+                                     request):
     torch.manual_seed(d * 7 + b * 3 + depth + n0)
     tr, st = _model(d, heads, depth, value_residual, streams)
     kv = torch.randn(depth, 2, b, n0, 64).to(bf16)
     mask = _key_mask(mask_kind, b, n0)
-    xs = torch.randn(STEPS, b, d).to(bf16).float()
+    xs = torch.randn(STEPS, b, d).to(bf16).float() + dc
     ref_kw = dict(heads=heads, depth=depth, streams=streams, value_residual=value_residual)
     multi_on, multi = _run_path(False, tr, st, b, n0, kv, mask, xs, ref_kw)
     fused_on, one = _run_path(True, tr, st, b, n0, kv, mask, xs, ref_kw)

@@ -89,6 +89,36 @@ def test_hc_pre_fwd_bwd_streams(S, d, expand):
         assert rel_err(g_ln, ref_ln) < 3e-2
 
 
+@pytest.mark.parametrize("S", [2, 4, 5, 8])
+@pytest.mark.parametrize("d", [64, 1000, 1024])
+@pytest.mark.parametrize("dc,expand", [(1024.0, False), (1024.0, True), (8192.0, True)])
+def test_hc_pre_fwd_dc_offset(S, d, dc, expand):
+    """branch inputs with a DC offset on the second-generation forward (d <= 1024: S <= 4 at one and two chunks per
+    thread, S >= 5 at 128 threads per token): R_in = dc with the variation carried by Y, or x_expand = dc + noise.
+    xn and the LayerNorm statistics in aux against an fp64 hc_ref; a variance taken as E[x^2] - mean^2 in fp32 is
+    rounding noise on these rows.  (With R_in = 8192 the fp32 residual R_in + beta Y itself carries 2^-11 per element,
+    more than the bound allows once the stream weights nearly cancel.)"""
+    from audiolm_pytorch_b200 import ops
+
+    M = 777
+    hc, ln_gamma = make_hc(d, S=S, seed=S + d)
+    kin, raw = _inputs(M, S, d, expand, S * d)
+    if expand:
+        kin["x_expand"] = raw["x"] = raw["x"] + dc
+    else:
+        kin["R_in"] = raw["R_in"] = torch.full_like(raw["R_in"], dc)
+    _, _, xn, _, aux = ops.hc_pre_fwd(hc, ln_gamma, **kin, M=M, d=d, streams=S)
+    hc64 = {k: v.double() for k, v in hc.items()}
+    R = (raw["x"].double()[:, None, :].expand(M, S, d) if expand
+         else raw["R_in"].double() + raw["bp"].double()[..., None] * raw["Y"].double()[:, None, :])
+    _, bin_ref, xn_ref, _ = hc_ref(hc64, ln_gamma.double(), R, d)
+    rstd_ref = (bin_ref.var(-1, unbiased=False) + 1e-5).rsqrt()
+    # the rows are ill-conditioned (less than dc where the branch's stream weights nearly cancel)
+    assert (bin_ref.mean(-1).abs() / bin_ref.std(-1, unbiased=False)).min() > dc / 64
+    assert rel_err(xn, xn_ref) < 1.5e-2
+    assert ((aux[:, -1].double() - rstd_ref).abs() / rstd_ref).max().item() < 1e-2
+
+
 @pytest.mark.parametrize("S", [2, 3, 5, 8])
 @pytest.mark.parametrize("d,expand", [(1024, False), (1000, True), (2048, False)])
 def test_hc_param_grads_vs_fp64_streams(S, d, expand):
