@@ -98,6 +98,7 @@ SIGNATURES: dict[str, list] = {
     "alm_encodec_resblock_fp32": [P, P, P, P, P, P, P, I, I, I, I, P],
     "alm_encodec_lstm": [P, P, P, P, P, I, I, I, I, P],
     "alm_encodec_resblock_tc": [P, P, P, P, P, I, I, I, I, I, P],
+    "alm_resample": [P, L, L, P, L, L, I, P, P, I, I, I, P],
 }
 
 

@@ -580,7 +580,7 @@ class SemanticTransformerWrapper(nn.Module):
         dev = self.device
         if exists(prime_wave):
             assert not exists(prime_ids) and exists(self.wav2vec)
-            ids = self.wav2vec(prime_wave, flatten=False, input_sample_hz=prime_wave_input_sample_hz)
+            ids = self.wav2vec(prime_wave.to(dev), flatten=False, input_sample_hz=prime_wave_input_sample_hz)
         elif exists(prime_ids):
             ids = prime_ids
         else:
@@ -748,7 +748,7 @@ class CoarseTransformerWrapper(nn.Module):
             coarse = prime_coarse_token_ids.long()
         elif exists(prime_wave):
             assert exists(self.codec)
-            coarse = self._codec_ids(prime_wave, prime_wave_input_sample_hz)[..., :self.num_coarse_quantizers]
+            coarse = self._codec_ids(prime_wave.to(dev), prime_wave_input_sample_hz)[..., :self.num_coarse_quantizers]
             coarse = coarse.reshape(batch, -1)
         else:
             coarse = torch.empty((batch, 0), device=dev, dtype=torch.long)
@@ -876,7 +876,8 @@ class FineTransformerWrapper(nn.Module):
             assert exists(self.codec)
             with torch.inference_mode():
                 self.codec.eval()
-                _, ids, _ = self.codec(prime_wave, return_encoded=True, input_sample_hz=prime_wave_input_sample_hz)
+                _, ids, _ = self.codec(prime_wave.to(dev), return_encoded=True,
+                                       input_sample_hz=prime_wave_input_sample_hz)
             fine = ids[..., self.num_coarse_quantizers:].reshape(batch, -1).long()
         else:
             fine = torch.empty((batch, 0), device=dev, dtype=torch.long)

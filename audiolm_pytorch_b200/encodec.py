@@ -289,11 +289,10 @@ class EncodecWrapper(nn.Module):
         assert not self.training, "Encodec is pretrained and should never be called outside eval mode."
         lead = x.shape[:-1]
         x = x.reshape(-1, x.shape[-1])  # the reference packs every leading dim ('* n')
-        if input_sample_hz is not None and input_sample_hz != self.target_sample_hz:
-            from torchaudio.functional import resample
-            x = resample(x, input_sample_hz, self.target_sample_hz)
         if not x.is_cuda:
             raise AlmError("EncodecWrapper: the input is on the CPU; the hot path has no CPU implementation")
+        if input_sample_hz is not None and input_sample_hz != self.target_sample_hz:
+            x = ops.resample(x, input_sample_hz, self.target_sample_hz)
         with torch.no_grad():
             h = self.encode_frames(x.to(f32).contiguous())
             _, codes, _ = self.rq(h)

@@ -237,6 +237,15 @@ def curtail_to_multiple(t, mult):
     return t[..., :t.shape[-1] // mult * mult]
 
 
+def resample_curtailed(wave, input_sample_hz, target_sample_hz, mult):
+    """the wave resampled from input_sample_hz (None: as is) with only the samples curtail_to_multiple(., mult) keeps
+    computed"""
+    if input_sample_hz is None:
+        return wave
+    total = ops.resample_length(wave.shape[-1], input_sample_hz, target_sample_hz)
+    return ops.resample(wave, input_sample_hz, target_sample_hz, count=total if mult is None else total // mult * mult)
+
+
 class HubertWithKmeans(nn.Module):
     """checkpoint and kmeans as published at https://github.com/facebookresearch/fairseq/tree/main/examples/hubert
     (or your own); see the module docstring for what runs where"""
@@ -378,9 +387,7 @@ class HubertWithKmeans(nn.Module):
         if not wav_input.is_cuda:
             raise _lib.AlmError("HubertWithKmeans runs on the GPU only (no CPU fallback); move the module and the "
                                 "wave to a CUDA device")
-        if input_sample_hz is not None:
-            from torchaudio.functional import resample
-            wav_input = resample(wav_input, input_sample_hz, self.target_sample_hz)
+        wav_input = resample_curtailed(wav_input, input_sample_hz, self.target_sample_hz, self.seq_len_multiple_of)
         if self.seq_len_multiple_of is not None:
             wav_input = curtail_to_multiple(wav_input, self.seq_len_multiple_of)
         clusters = self.assign(self.extract_features(wav_input))

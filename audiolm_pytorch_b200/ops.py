@@ -1430,3 +1430,106 @@ def w2v_norm_act(y, stats, *, gamma=None, beta=None, act=None, residual=None, st
     _lib.call("alm_w2v_norm_act", y, stats, gamma, beta, W2V_ACT[act], residual, Tr, int(step), float(residual_scale),
               int(log_compress), out, split, B, T, C, stats.shape[1])
     return out, split
+
+
+# ---- band-limited resampling (csrc/resample.cu) ----------------------------------------------------------------------
+RESAMPLE_ZEROS = 6        # torchaudio's lowpass_filter_width, the reference never changes it
+RESAMPLE_ROLLOFF = 0.99   # torchaudio's rolloff, likewise
+
+
+def resample_rates(orig_hz, new_hz):
+    """the rates reduced by their gcd, (o, n); ValueError for a non-positive or non-integer rate, as torchaudio"""
+    for r in (orig_hz, new_hz):
+        if not r > 0:
+            raise ValueError(f"resample: sample rates must be positive, got {orig_hz} -> {new_hz}")
+        if int(r) != r:
+            raise ValueError(f"resample: sample rates must be integers, got {orig_hz} -> {new_hz}")
+    o, n = int(orig_hz), int(new_hz)
+    g = math.gcd(o, n)
+    return o // g, n // g
+
+
+def resample_length(L, orig_hz, new_hz):
+    """samples torchaudio.functional.resample makes of L input samples: ceil(n L / o)"""
+    o, n = resample_rates(orig_hz, new_hz)
+    return -(-n * L // o)
+
+
+@functools.lru_cache(maxsize=None)
+def resample_table(o, n):
+    """compact polyphase filter of the reduced rates o -> n (o != n), in fp64: (taps [n, T], first [n], counts [n]).
+
+    torchaudio's dense filter is K[p, m] = (base / o) sinc(pi t) cos^2(pi t / 12), m < 2 width + o, with
+    t = clamp(base ((m - width) / o - p / n), -6, 6), base = 0.99 min(o, n), width = ceil(6 o / base).  Phase p keeps
+    the taps with |t| < 6 before the clamp, a run of counts[p] taps from input offset first[p] relative to k o: at
+    |t| = 6 the window is cos^2(pi / 2), so every dropped tap is below 1e-48.  t is formed with the same fp64 operations
+    as torchaudio, so the kept taps are torchaudio's fp64 taps.  Row p of taps holds the run, zero-padded to
+    T = max(counts)."""
+    assert o > 0 and n > 0 and o != n and math.gcd(o, n) == 1
+    f64 = torch.float64
+    base = min(o, n) * RESAMPLE_ROLLOFF
+    width = math.ceil(RESAMPLE_ZEROS * o / base)
+    # t rises by base / o <= 0.99 per tap: the run of |t| < 6 is at most 12 o / base + 1 taps long and starts after
+    # m = width + o (p / n - 6 / base); evaluate two taps of margin on each side
+    span = math.floor(2 * RESAMPLE_ZEROS * o / base) + 6
+    p = torch.arange(n, dtype=f64)
+    m = torch.floor(width + o * (p / n - RESAMPLE_ZEROS / base)).long()[:, None] - 2 + torch.arange(span)
+    t = ((-p / n)[:, None] + (m - width).to(f64) / o) * base
+    assert bool((t[:, 0] <= -RESAMPLE_ZEROS).all() and (t[:, -1] >= RESAMPLE_ZEROS).all())
+    keep = (t.abs() < RESAMPLE_ZEROS) & (m >= 0) & (m < 2 * width + o)
+    counts = keep.sum(1)
+    lead = keep.long().argmax(1)
+    T = int(counts.max())
+    i = torch.arange(T)
+    valid = i[None] < counts[:, None]
+    col = (lead[:, None] + i).clamp(max=span - 1)
+    tk = t.gather(1, col)
+    window = torch.cos(tk * math.pi / RESAMPLE_ZEROS / 2) ** 2
+    tk = tk * math.pi
+    taps = torch.where(tk == 0, torch.ones_like(tk), tk.sin() / tk) * (window * (base / o))
+    taps = torch.where(valid, taps, torch.zeros_like(taps))
+    first = m.gather(1, lead[:, None])[:, 0] - width
+    return taps, first, counts
+
+
+_RESAMPLE_DEVICE_TABLES: dict = {}
+
+
+def _resample_device_table(o, n, device):
+    key = (o, n, device)
+    if key not in _RESAMPLE_DEVICE_TABLES:
+        taps, first, _ = resample_table(o, n)
+        _RESAMPLE_DEVICE_TABLES[key] = (taps.t().to(f32).contiguous().to(device),
+                                        first.to(torch.int32).to(device), taps.shape[1])
+    return _RESAMPLE_DEVICE_TABLES[key]
+
+
+def resample(x, orig_hz, new_hz, *, start=0, count=None):
+    """torchaudio.functional.resample(x, orig_hz, new_hz) with its defaults (Hann-windowed sinc, 6 zero crossings,
+    rolloff 0.99) on the compact polyphase filter, one launch: x CUDA [..., L], any float dtype -> fp32 [..., count],
+    the output samples [start, start + count) of the ceil(n L / o) torchaudio makes (count=None: up to the end).
+
+    Computes in fp32; a row's output is bitwise the same alone or in a batch.  orig_hz == new_hz returns the input
+    unchanged (sliced to the window), as torchaudio does.  No autograd.  Rates must be positive integers (ValueError)."""
+    o, n = resample_rates(orig_hz, new_hz)
+    L = x.shape[-1]
+    total = -(-n * L // o)
+    if count is None:
+        count = total - start
+    if not (0 <= start and 0 <= count and start + count <= total):
+        raise ValueError(f"resample: window [{start}, {start} + {count}) is outside the {total} output samples")
+    if o == n:
+        return x if (start, count) == (0, L) else x[..., start:start + count]
+    _check_cuda(x)
+    lead = x.shape[:-1]
+    y = torch.empty(*lead, count, device=x.device, dtype=f32)
+    rows = y.numel() // count if count else 0
+    if rows == 0 or L == 0:
+        return y.zero_()
+    x2 = x.detach().reshape(rows, L)
+    if x2.dtype != f32 or x2.stride(1) != 1 or (rows > 1 and x2.stride(0) < L):
+        x2 = x2.to(f32).contiguous()
+    taps, first, T = _resample_device_table(o, n, x.device)
+    with _timed("resample", 4.0 * rows * (L + count), unit="byte"):
+        _lib.call("alm_resample", x2, x2.stride(0) if rows > 1 else L, L, y, start, count, rows, taps, first, T, o, n)
+    return y

@@ -36,6 +36,15 @@ def exists(v):
     return v is not None
 
 
+def curtail_window(total, mult, from_left=False):
+    """(start, count) of the samples the reference's curtail_to_multiple (utils.py:8-12) keeps of `total`.  From the
+    left it slices [-keep:], which keeps everything when keep is 0."""
+    keep = total // mult * mult
+    if from_left and keep:
+        return total - keep, keep
+    return 0, total if from_left else keep
+
+
 class CausalConv1d(nn.Module):
     """soundstream.py:332-345; parameters live in `.conv` (nn.Conv1d) for state_dict compatibility."""
 
@@ -732,12 +741,13 @@ class SoundStream(nn.Module):
     def process_input(self, x, input_sample_hz=None, curtail_from_left=False):
         lead = x.shape[:-1]
         x = x.reshape(-1, x.shape[-1])  # the reference packs every leading dim ('* n', soundstream.py:785)
-        if exists(input_sample_hz) and input_sample_hz != self.target_sample_hz:
-            from torchaudio.functional import resample
-            x = resample(x, input_sample_hz, self.target_sample_hz)
-        mult = self.seq_len_multiple_of
-        keep = x.shape[-1] // mult * mult
-        x = x[..., -keep:] if curtail_from_left else x[..., :keep]
+        resampling = exists(input_sample_hz) and input_sample_hz != self.target_sample_hz
+        total = ops.resample_length(x.shape[-1], input_sample_hz, self.target_sample_hz) if resampling else x.shape[-1]
+        start, count = curtail_window(total, self.seq_len_multiple_of, curtail_from_left)
+        if resampling:
+            x = ops.resample(x, input_sample_hz, self.target_sample_hz, start=start, count=count)
+        else:
+            x = x[..., start:start + count]
         return x[:, None, :], lead
 
     def decode_from_codebook_indices(self, quantized_indices):

@@ -29,7 +29,7 @@ from torch import nn
 
 from . import _lib, ops
 from .hubert import (_conv_flops, _Node, _plain, _register, curtail_to_multiple, getattr_path, load_checkpoint,
-                     parse_conv_layers, receptive_field)
+                     parse_conv_layers, receptive_field, resample_curtailed)
 from .soundstream import SoundStream
 
 f32 = torch.float32
@@ -248,9 +248,7 @@ class FairseqVQWav2Vec(nn.Module):
         if not wav_input.is_cuda:
             raise _lib.AlmError("FairseqVQWav2Vec runs on the GPU only (no CPU fallback); move the module and the "
                                 "wave to a CUDA device")
-        if input_sample_hz is not None:
-            from torchaudio.functional import resample
-            wav_input = resample(wav_input, input_sample_hz, self.target_sample_hz)
+        wav_input = resample_curtailed(wav_input, input_sample_hz, self.target_sample_hz, self.seq_len_multiple_of)
         if self.seq_len_multiple_of is not None:
             wav_input = curtail_to_multiple(wav_input, self.seq_len_multiple_of)
         idx = self.assign(self.quantizer_input(wav_input))

@@ -617,6 +617,20 @@ int alm_w2v_norm_act(const float* y, const float* stats, const float* gamma, con
                      const float* residual, int Tr, int step, float scale, int log_compress, float* out, void* split,
                      int B, int T, int C, int G, alm_stream_t stream);
 
+/*
+ * Band-limited resampling, csrc/resample.cu: torchaudio.functional.resample(x, orig, new) with its defaults (Hann
+ * window, 6 zero crossings, rolloff 0.99) as the reference calls it at soundstream.py:788, hubert_kmeans.py:102,
+ * vq_wav2vec.py:70 and encodec.py:105.  With the rates reduced by their gcd to o -> n, output j = k n + p (p < n) is
+ *     y[r, j - start] = sum_{i < T} taps[i, p] x[r, k o + off[p] + i]   (x = 0 outside [0, L))
+ * for j in [start, start + count), r < rows; x fp32 [rows, ldx] (L samples per row), y fp32 [rows, count].
+ * taps fp32 [T, n] and off int32 [n] are the compact polyphase table the caller builds once per (o, n): each phase's
+ * taps inside the +-6 zero crossings from its first input offset, zero-padded to T.  A full resample is start = 0,
+ * count = ceil(n L / o).  One launch; taps are summed in index order without atomics, so a row's output is bitwise
+ * reproducible and independent of the batch and of the window.
+ */
+int alm_resample(const float* x, int64_t ldx, int64_t L, float* y, int64_t start, int64_t count, int rows,
+                 const float* taps, const int* off, int T, int o, int n, alm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
